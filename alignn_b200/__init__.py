@@ -1,4 +1,4 @@
-"""alignn_b200: B200-native (sm_100a) edge-gated graph-convolution hot path of ALIGNN.
+"""alignn_b200: H100-native (sm_90a) edge-gated graph-convolution hot path of ALIGNN.
 
 Keeps the reference's ALIGNN / ALIGNNConfig / forward((g, lg, lat)) surface
 (alignn/models/alignn.py) on top of hand-written CUDA kernels behind a C-ABI

@@ -139,10 +139,7 @@ _SIGNATURES = {
     "alignn_b200_radius_graph_fill": (C.c_int, [_fp, _fp, C.c_int64, C.c_int64, C.c_double, C.c_double, _fp, _fp, _fp, _fp, _fp, _fp]),
     "alignn_b200_pair_force_scatter": (C.c_int, [_fp, _fp, _fp, _fp, _fp, C.c_int64, C.c_int, _fp, _fp]),
     "alignn_b200_virial_stress": (C.c_int, [_fp, _fp, _fp, _fp, _fp, C.c_int64, C.c_float, _fp, _fp]),
-    "alignn_b200_debug_gemm_flags": (None, [C.c_int]),
-    "alignn_b200_debug_gemm_pair": (None, [C.c_int]),
     "alignn_b200_debug_egc_flags": (None, [C.c_int]),
-    "alignn_b200_debug_gemm_trace": (None, [_fp]),
     "alignn_b200_segment_mean": (C.c_int, [_fp, _fp, C.c_int64, C.c_int, _fp, _fp]),
     "alignn_b200_segment_mean_backward": (C.c_int, [_fp, _fp, C.c_int64, C.c_int, _fp, _fp]),
 }
@@ -160,7 +157,7 @@ def load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"{LIB_PATH} not found: the CUDA extension is not built. Run `python -c 'import __graft_entry__ as g; "
-            "g.build()'` (nvcc, sm_100a). alignn_b200 has no CPU or eager fallback.")
+            "g.build()'` (nvcc, sm_90a). alignn_b200 has no CPU or eager fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in _SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError if the .so does not export what the header declares
@@ -202,7 +199,7 @@ def require_cuda(*tensors: torch.Tensor) -> None:
             continue
         if not t.is_cuda:
             raise RuntimeError("alignn_b200 kernels need CUDA tensors (no CPU path exists); got a tensor on "
-                               f"{t.device}. Move the model and graphs to a B200 with .to('cuda').")
+                               f"{t.device}. Move the model and graphs to the GPU with .to('cuda').")
         if t.dtype not in (torch.float32, torch.int32):
             raise RuntimeError(f"alignn_b200 kernels are fp32/int32 only; got {t.dtype}")
         if not t.is_contiguous():

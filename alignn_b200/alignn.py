@@ -1,4 +1,4 @@
-"""ALIGNN property model on the B200 edge-gated conv kernels.
+"""ALIGNN property model on the H100 edge-gated conv kernels.
 
 Host-side mirror of the reference module alignn/models/alignn.py: same public names
 (`ALIGNNConfig`, `EdgeGatedGraphConv`, `ALIGNNConv`, `MLPLayer`, `ALIGNN`), same constructor
@@ -69,7 +69,7 @@ class RBFExpansion(nn.Module):
 
 def mlp_forward(layer: nn.Sequential, x: torch.Tensor) -> torch.Tensor:
     """Linear -> norm -> SiLU.  On CUDA fp32 inputs the Linear (forward, data gradient, weight gradient) runs on
-    the tcgen05 bf16x3 kernels when its shape is one the library supports (the angle/bond embeddings act on
+    the wgmma bf16x3 kernels when its shape is one the library supports (the angle/bond embeddings act on
     T = 276 480 rows per batch); train-mode BatchNorm, LayerNorm and (without autograd) eval-mode BatchNorm run fused with
     the SiLU on the library's row kernels (SURVEY.md section 8f row 3)."""
     lin, norm = layer[0], layer[1]

@@ -1,4 +1,4 @@
-"""EdgeGatedGraphConv / ALIGNNConv on the B200 kernels.
+"""EdgeGatedGraphConv / ALIGNNConv on the H100 kernels.
 
 Mirrors the reference operator interface for this path:
     EdgeGatedGraphConv(input_features, output_features, residual=True).forward(g, node_feats, edge_feats) -> (x, y)
@@ -8,7 +8,7 @@ with identical attribute / state_dict names (SURVEY.md App. A) so reference chec
 with `load_state_dict`.
 
 The four node Linear layers run as ONE [Nn,d]x[d,4d] GEMM and the edge gate as one [Ne,d]x[d,d]
-GEMM, both on the tcgen05 bf16x3 tensor-core kernel (csrc/gemm_tc.cu); everything else of the layer --
+GEMM, both on the wgmma bf16x3 tensor-core kernel (csrc/gemm_tc.cu); everything else of the layer --
 u_add_v, sigmoid, both update_all reductions, the division, both norms, SiLU, residuals -- is a single
 fused CUDA kernel forward and two backward (csrc/egc_kernels.cu); data gradients reuse the GEMM kernel with
 transposed weight images, weight gradients run on the split-K tensor-core kernel (csrc/wgrad_tc.cu).  All of
@@ -27,12 +27,12 @@ from .graph import as_graph
 from .ops import NORM_AFFINE, NORM_LAYER, NORM_STATS
 
 GATE_EPS = 1e-6   # alignn.py:109
-# True: pass 1 = TMA-fed gather GEMM writes m and its batch statistics, pass 2 = segment reductions + edge tail.
+# True: pass 1 = gather GEMM writes m and its batch statistics, pass 2 = segment reductions + edge tail.
 # False: the round-1 composition (plain GEMM writes G, the edge kernel forms m); kept for A/B runs and bit-identity tests.
 USE_GATHER_GEMM = os.environ.get("ALIGNN_B200_GATHER_GEMM", "1") != "0"
-# "1": independent kernels of a conv backward on parallel streams (see _Fork).  Measured on B200 (batch 64): 9.74 ms per
-# step forked vs 9.62 ms serial -- every one of these kernels already fills the SMs (or is a cooperative launch), so the
-# default is serial; the switch stays for small-graph workloads.
+# "1": independent kernels of a conv backward on parallel streams (see _Fork).  At batch 64 every one of these kernels
+# already fills the SMs (or is a cooperative launch), so the default is serial; the switch stays for small-graph
+# workloads.
 USE_SIDE_STREAMS = os.environ.get("ALIGNN_B200_SIDE_STREAMS", "0") != "0"
 
 
@@ -160,8 +160,8 @@ class _EdgeGatedConvFn(torch.autograd.Function):
         if USE_GATHER_GEMM:
             img = cfg.images            # operand images, refreshed by one table-driven launch per step (ops.ImageTable)
             P = ops.gemm_gather(x, img.images["cat"], img.vectors["bcat"])
-            # pass 1 over the edge rows (csrc/gemm_fused_tc.cu): m = e_src[src] + e_dst[dst] + edge_gate(y) on tcgen05,
-            # y streamed by TMA, the P rows gathered in the epilogue, BatchNorm batch statistics of m on the way out
+            # pass 1 over the edge rows (csrc/gemm_tc.cu): m = e_src[src] + e_dst[dst] + edge_gate(y) on wgmma,
+            # the P rows gathered in the epilogue, BatchNorm batch statistics of m on the way out
             e_part = None
             if Ne > 0:
                 res = ops.gemm_gather(y, img.images["eg"], None, add0=P[:, 0:d], idx0=ix.src,
@@ -276,7 +276,7 @@ class _EdgeGatedConvFn(torch.autograd.Function):
         GM, GP, vd, vs = ops.egc_backward(cfg.index, P, M, XP, S, H, gx_out, gy_out, n, e, reduce=params and not deferred,
                                           norm_nodes=cfg.norm_nodes, norm_edges=cfg.norm_edges,
                                           gate_eps=GATE_EPS, ln_eps=cfg.ln_eps)
-        # GEMM halves of the backward on the tensor cores: data gradients (gemm_fused_tc.cu, transposed weight images,
+        # GEMM halves of the backward on the tensor cores: data gradients (gemm_tc.cu, transposed weight images,
         # residual added in the epilogue) and weight gradients (wgrad_tc.cu, split-K over rows); four independent
         # kernels, forked over side streams
         need = ctx.needs_input_grad
@@ -385,7 +385,7 @@ class EdgeGatedGraphConvBase(nn.Module):
                                f"alignn/config.py:163); got {node_feats.dtype}")
         if not node_feats.is_cuda:
             raise RuntimeError("alignn_b200.EdgeGatedGraphConv has no CPU path: move the model, features and graphs "
-                               "to a CUDA device (B200).")
+                               "to a CUDA device.")
         if g.device != node_feats.device:
             raise RuntimeError(f"graph is on {g.device} but features are on {node_feats.device}; call g.to(device)")
         if node_feats.shape[0] != g.num_nodes() or edge_feats.shape[0] != g.num_edges():

@@ -1,4 +1,4 @@
-// Shared device helpers for the edge-gated conv kernels (sm_100a).
+// Shared device helpers for the edge-gated conv kernels (sm_90a).
 //
 // Row-per-warp layout: a feature row of D floats is spread over the 32 lanes of a warp,
 // lane l holding CH vectors of W floats: channels  c*32*W + l*W + j  (c < CH, j < W).
@@ -13,7 +13,7 @@ namespace alignn {
 
 constexpr int kWarpsPerBlock = 8;
 constexpr int kThreads = kWarpsPerBlock * 32;
-constexpr int kNumSMs = 148;                       // B200
+constexpr int kNumSMs = 132;                       // H100 SXM
 constexpr int kMaxBlocks = kNumSMs * 4;            // rows of per-block partials are bounded by this
 
 template <int D>
@@ -81,7 +81,7 @@ __device__ __forceinline__ void ld_vec(float (&v)[RowCfg<D>::VPL], const float* 
 
 // sigmoid in four instructions (FMUL, MUFU.EX2, FADD, MUFU.RCP; <= 2 ulp) instead of ~25 with an IEEE division and the
 // denormal paths of the non-ftz approximations: the edge kernels are bound by instruction issue at 4 warps per
-// scheduler, not by HBM (profiles/r02_ncu_full_summary.md).  exp(-x) underflowing to 0 and overflowing to +inf give
+// scheduler, not by HBM.  exp(-x) underflowing to 0 and overflowing to +inf give
 // exactly 1 and 0.
 __device__ __forceinline__ float sigmoidf_(float x) {
   float e, r;

@@ -1,5 +1,5 @@
 // Edge-gated graph convolution: gather / gate / segment-reduce / norm kernels, forward and
-// backward, fp32, sm_100a.  One warp owns one destination node (one CSR segment): it walks the
+// backward, fp32, sm_90a.  One warp owns one destination node (one CSR segment): it walks the
 // node's in-edges in sorted order, gathers the source rows by edge index, and reduces the gated
 // messages in registers -- no atomics, deterministic, every global access a coalesced row.
 //
@@ -15,7 +15,7 @@ namespace alignn {
 // Forward
 // =============================================================================================
 // GIM ("gate is m"): a.G already holds the pre-activation gate m = e_src[src] + e_dst[dst] + edge_gate(y), written
-// (together with its batch statistics) by the gather GEMM (gemm_fused_tc.cu).  The kernel then neither gathers
+// (together with its batch statistics) by the gather GEMM (gemm_tc.cu).  The kernel then neither gathers
 // e_src / e_dst nor writes M nor accumulates edge statistics: it is the second and last pass over the edge rows.
 template <int D, bool GIM>
 __global__ void __launch_bounds__(kThreads, 2)
@@ -597,9 +597,8 @@ egc_backward_dst_kernel(alignn_b200_egc_bwd_args a) {
 // twice, 128 channels (one float4 per lane) at a time: the six vector halves (24 registers), the node's gradient halves and
 // the two accumulators then live in registers for the whole segment, and shared memory is touched once per (node, half)
 // instead of per edge.  Every global access is still a fully used 512-byte warp request.  (LayerNorm needs the whole row
-// for its statistics and keeps the full-row kernel.)  MEASURED SLOWER on B200 (dst + src 418 us vs 370 us at the L(g)
-// shape, profiles/r02_egc_ring_ab.json): with 512-byte instead of 1 KB requests and the same 16 warps per SM the bytes in
-// flight halve and the kernel turns from LSU-bound into latency-bound.  Kept opt-in (alignn_b200_debug_egc_flags bit 1).  The per-warp partial sums are accumulated per segment before they
+// for its statistics and keeps the full-row kernel.)  With 512-byte instead of 1 KB requests and the same
+// 16 warps per SM the bytes in flight halve, which made it slower than the full-row kernel where it was measured.  Kept opt-in (alignn_b200_debug_egc_flags bit 1).  The per-warp partial sums are accumulated per segment before they
 // are added to the running totals, so the parameter-gradient partials differ from the full-row kernel in the last bits;
 // GM and GP are bit-identical.
 template <int NORM>

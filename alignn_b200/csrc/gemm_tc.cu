@@ -1,21 +1,27 @@
-// C[M,N] = A[M,K] * W[N,K]^T (+ bias[N]) (+ R[M,N]) in fp32 parity on the 5th-gen tensor cores:
-// tcgen05.mma kind::f16 (bf16 x bf16 -> fp32 in TMEM) with the bf16x3 operand split (tc_common.cuh).
+// Linear layers in fp32 parity on the Hopper tensor cores: wgmma (bf16 x bf16 -> fp32 in registers) with the bf16x3
+// operand split (tc_common.cuh).
 //
-// This is the Linear-layer workhorse of the conv path: the four node projections (one
-// [Nn,d]x[d,4d] GEMM), the edge gate (alignn.py:101) and the two data-gradient GEMMs of the
-// backward.  A is the fp32 activation matrix, streamed from HBM once; it is converted to bf16 hi/lo
-// planes by the loader warps on its way into shared memory (software-pipelined: the global loads of
-// chunk k+1 are in flight while chunk k is converted).  W is pre-split once per step into an image
-// that already has the UMMA core-matrix order (gemm_prepare_weights), so a K-chunk of it is ONE
-// contiguous TMA bulk copy (cp.async.bulk -> UBLKCP) signalled on the stage's mbarrier.
+//   C[r, :] = A[r, :] * W^T (+ bias) (+ add0[i0(r), :]) (+ add1[i1(r), :])                                  r < M
+//   stats[cta][0/1][c] = partial sums over the CTA's tiles of C[r, c] and C[r, c]^2                         (optional)
 //
-// Persistent, warp-specialised CTA (one per SM), 128 x BN output tiles (BN = 256 when N allows):
-//   warp 0      : TMEM owner + MMA issuer (one lane)
-//   warps 1-4   : epilogue -- tcgen05.ld -> registers -> warp-private smem transpose -> coalesced
-//                 128-byte row segments to HBM (+ bias, + residual)
-//   warps 5-12  : loaders / fp32->bf16x2 converters
-// 4-stage smem ring of BK=32 chunks (mbarrier full/empty), double-buffered TMEM accumulator
-// (mbarrier tfull/tempty) so the epilogue of tile i overlaps the main loop of tile i+1.
+// gemm_nt is the plain form (add0 = the residual, no index).  gemm_gather is the edge-gate kernel of the conv path: with
+// A = edge features y, add0 = P[src, 0:d] (e_src), add1 = P[dst, 2d:3d] (e_dst + both biases) it is the pre-activation
+// gate  m = e_src[src] + e_dst[dst] + edge_gate(y)  of alignn/models/alignn.py:98-101 in ONE pass over y, plus the
+// per-channel batch statistics BatchNorm1d(m) needs (alignn.py:123).  With add0 = the incoming gradient it is the
+// data-gradient GEMM of the backward (residual in the epilogue); with bn_scale set, add1 rows are the pre-norm rows m of
+// the BatchNorm + SiLU that produced this GEMM's input gradient, and the statistics are sum gu, sum gu (m - mean).
+//
+// A is the fp32 activation matrix, streamed from HBM once; it is converted to bf16 hi/lo planes by the loader warps on
+// its way into shared memory (software-pipelined: the global loads of chunk k+1 are in flight while chunk k is
+// converted).  W is pre-split once per step into an image that already has the GMMA core-matrix order
+// (gemm_prepare_weights), so a K-chunk of it is ONE contiguous bulk copy (cp.async.bulk) signalled on the stage's
+// mbarrier.
+//
+// Persistent, warp-specialised CTA (one per SM), 128 x BN output tiles, BN <= 128: the 128 x BN fp32 accumulator lives
+// in the registers of two consumer warpgroups (BN / 2 per thread), which also run the epilogue straight from registers.
+//   warps 0-7   : two consumer warpgroups, rows 0-63 / 64-127 of the tile: wgmma m64nBNk16, then the epilogue
+//   warps 8-15  : loaders / fp32->bf16x2 converters, up to STAGES chunks ahead of the MMAs
+#include "common.cuh"
 #include "tc_common.cuh"
 #include "api_common.h"
 #include "alignn_b200.h"
@@ -23,20 +29,15 @@
 namespace alignn {
 namespace gemm {
 
-// Development aid (tools/time_kernels.py): knock out one pipeline agent to find the limiter.
-// bit0: no A loads, bit1: no W bulk copy, bit2: no C stores, bit3: no MMA.  0 in production.
-static int g_debug_flags = 0;
-
-constexpr int BM = 128;       // rows per tile (UMMA M)
-constexpr int BK = 32;        // K per pipeline stage (2 UMMA K=16 steps)
-constexpr int STAGES = 3;
-constexpr int EPI_WARPS = 4;
+constexpr int BM = 128;       // rows per tile (two m64 warpgroup MMAs)
+constexpr int BK = 32;        // K per pipeline stage (2 MMA K=16 steps)
+constexpr int STAGES = 4;
+constexpr int MMA_WARPS = 8;
 constexpr int LOAD_WARPS = 8;
-constexpr int THREADS = 32 * (1 + EPI_WARPS + LOAD_WARPS);   // 416
+constexpr int THREADS = 32 * (MMA_WARPS + LOAD_WARPS);   // 512
 constexpr uint32_t LBO = 128;               // next 8-element K chunk
 constexpr uint32_t SBO = (BK / 8) * 128;    // next 8-row group (chunk-local image): 512 B
-constexpr int EPI_COLS = 128;               // columns staged per epilogue pass (BN < 128: BN)
-constexpr int EPI_STRIDE = EPI_COLS + 4;    // floats; padded staging row
+constexpr int kMaxStatN = 256;              // widest output with column statistics
 
 template <int BN>
 struct Cfg {
@@ -44,10 +45,22 @@ struct Cfg {
   static constexpr int B_PLANE = BN * BK * 2;
   static constexpr int STAGE = 2 * A_PLANE + 2 * B_PLANE;
   static constexpr int PIPE_BYTES = STAGES * STAGE;
-  static constexpr int EPI_BYTES = EPI_WARPS * 32 * EPI_STRIDE * 4;
-  static constexpr int BAR_OFF = PIPE_BYTES + EPI_BYTES;
+  static constexpr int STAT_BYTES = MMA_WARPS * 2 * kMaxStatN * 4;   // per consumer warp: [2][N] column partials
+  static constexpr int BAR_OFF = PIPE_BYTES + STAT_BYTES;
   static constexpr int SMEM = BAR_OFF + 128;
-  static constexpr int TMEM_COLS = 2 * BN < 32 ? 32 : 2 * BN;   // double-buffered accumulator: 64..512
+  static_assert(SMEM <= 232448, "shared memory budget of one sm_90 CTA");
+};
+
+struct Params {
+  const float* A; int64_t lda;
+  const uint8_t* w_image;
+  int M, N, K;
+  const float* bias;
+  const float* add0; int64_t ld0; const int32_t* idx0;   // addend rows: add0[idx0 ? idx0[r] : r][0 .. N)
+  const float* add1; int64_t ld1; const int32_t* idx1;
+  float* C; int64_t ldc;
+  float* stats;                                          // [gridDim.x][2][N] or NULL (requires N <= kMaxStatN)
+  const float* bn_scale; const float* bn_shift; const float* bn_mean;
 };
 
 // byte offset of element (r, k) inside one chunk plane (rows x BK, core-matrix order)
@@ -64,43 +77,38 @@ __device__ __forceinline__ void a_coord(int i, int lt, int& row, int& kq) {
   kq = (u & 1) * 4 + (lane >> 4) * 2 + (lane & 1);
 }
 
+__device__ __forceinline__ float dsilu_(float u) {          // d/du [u * sigmoid(u)], same formula as egc_kernels.cu
+  float e, sg;                                             // 4-instruction sigmoid, as common.cuh's sigmoidf_
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(u * -1.4426950408889634f));
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(sg) : "f"(1.f + e));
+  return sg * (1.f + u * (1.f - sg));
+}
+
 template <int BN>
 __global__ void __launch_bounds__(THREADS, 1)
-gemm_nt_bf16x3_kernel(const float* __restrict__ A, int64_t lda, const uint8_t* __restrict__ Wimg, int M, int N, int K,
-                      const float* __restrict__ bias, const float* __restrict__ R, int64_t ldr,
-                      float* __restrict__ C, int64_t ldc, int dbg) {
+gemm_bf16x3_kernel(const Params p) {
   using F = Cfg<BN>;
   extern __shared__ __align__(128) uint8_t smem[];
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + F::BAR_OFF);
   uint64_t* empty = full + STAGES;
-  uint64_t* tfull = empty + STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int nk = K / BK;
-  const int n_tiles = N / BN;
+  const int M = p.M, nk = p.K / BK;
+  const int n_tiles = p.N / BN;
   const int m_tiles = (M + BM - 1) / BM;
   const int total = m_tiles * n_tiles;
 
   if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full[s], LOAD_WARPS + 1); tc::mbar_init(&empty[s], 1); }
-    for (int a = 0; a < 2; ++a) { tc::mbar_init(&tfull[a], 1); tc::mbar_init(&tempty[a], EPI_WARPS); }
+    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full[s], LOAD_WARPS + 1); tc::mbar_init(&empty[s], MMA_WARPS); }
     tc::mbar_fence_init();
   }
-  if (warp == 0) tc::tmem_alloc(tmem_slot, F::TMEM_COLS);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
 
-  if (warp >= 1 + EPI_WARPS) {
+  if (warp >= MMA_WARPS) {
     // ================= loaders / converters =================
-    const int lt = tid - 32 * (1 + EPI_WARPS);          // 0..255
+    const int lt = tid - 32 * MMA_WARPS;                 // 0..255
     // The CTA's work is the stream of chunks c = (local tile, kc).  PF chunks of A are kept in flight in
-    // registers.  The inner loop is kept lean on purpose: with only two loader warps per scheduler the
-    // instruction stream is latency-bound, so every per-chunk address is an incremented pointer, not
-    // recomputed index math (an earlier version spent ~3000 cycles per chunk on it).
+    // registers; every per-chunk address is an incremented pointer, not recomputed index math.
     constexpr int PF = 3;
     float4 buf[PF][4];
     int soff[4];
@@ -112,24 +120,18 @@ gemm_nt_bf16x3_kernel(const float* __restrict__ A, int64_t lda, const uint8_t* _
     }
     const int my_tiles = (total - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
     const int nchunks = my_tiles * nk;
-    // load cursor (runs PF chunks ahead of the store cursor)
     int l_tile = blockIdx.x, l_kc = 0;
     const float* lp[4];
     bool lval[4];
     auto set_tile_ptrs = [&](int tile) {
       const int m0 = (tile / n_tiles) * BM;
-      // The epilogue adds the residual R row by row with only 4 warps: straight from HBM that costs ~1.5 us per
-      // dependent load (the gy GEMM ran at 574 us instead of 150).  Pull this tile's R rows into L2 now, about
-      // one tile ahead of the epilogue that will read them.
-      if (R && lt < BM && m0 + lt < M)
-        tc::bulk_prefetch_l2(R + (int64_t)(m0 + lt) * ldr + (tile % n_tiles) * BN, (uint32_t)BN * 4u);
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         int r_, kq;
         a_coord(i, lt, r_, kq);
         const int gr = m0 + r_;
-        lval[i] = (gr < M) && !(dbg & 1);
-        lp[i] = A + (int64_t)(lval[i] ? gr : 0) * lda + kq * 4;
+        lval[i] = gr < M;
+        lp[i] = p.A + (int64_t)(lval[i] ? gr : 0) * p.lda + kq * 4;
       }
     };
     auto load_next = [&](float4 (&v)[4]) {
@@ -144,141 +146,150 @@ gemm_nt_bf16x3_kernel(const float* __restrict__ A, int64_t lda, const uint8_t* _
 #pragma unroll
     for (int j = 0; j < PF; ++j)
       if (j < nchunks) load_next(buf[j]);
-    // store cursor
-    int s = 0, ph = 0, s_kc = 0, s_ntile = (int)blockIdx.x % n_tiles, s_tile = blockIdx.x;
-    const uint8_t* wsrc = Wimg + (int64_t)s_ntile * nk * 2 * F::B_PLANE;
+    int s = 0, ph = 0, s_kc = 0, s_tile = blockIdx.x;
+    const uint8_t* wsrc = p.w_image + (int64_t)(s_tile % n_tiles) * nk * 2 * F::B_PLANE;
     for (int c0 = 0; c0 < nchunks; c0 += PF) {
 #pragma unroll
       for (int j = 0; j < PF; ++j) {
         const int c = c0 + j;
         if (c < nchunks) {
-          if (c >= STAGES) { if (dbg & 512) tc::mbar_wait_poll(&empty[s], ph ^ 1); else tc::mbar_wait(&empty[s], ph ^ 1); }
+          if (c >= STAGES) tc::mbar_wait(&empty[s], ph ^ 1);
           uint8_t* st = smem + s * F::STAGE;
           if (lt == 0) {   // W chunk: one contiguous bulk copy (both planes), counted in bytes on full[s]
-            if (dbg & 2) {
-              tc::mbar_arrive(&full[s]);
-            } else {
-              tc::mbar_arrive_expect_tx(&full[s], 2 * F::B_PLANE);
-              tc::bulk_g2s(st + 2 * F::A_PLANE, wsrc, 2 * F::B_PLANE, &full[s]);
-            }
+            tc::mbar_arrive_expect_tx(&full[s], 2 * F::B_PLANE);
+            tc::bulk_g2s(st + 2 * F::A_PLANE, wsrc, 2 * F::B_PLANE, &full[s]);
           }
-          if (!(dbg & 16)) {
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              uint2 hi, lo;
-              tc::split4(buf[j][i], hi, lo);
-              *reinterpret_cast<uint2*>(st + soff[i]) = hi;
-              *reinterpret_cast<uint2*>(st + F::A_PLANE + soff[i]) = lo;
-            }
+          for (int i = 0; i < 4; ++i) {
+            uint2 hi, lo;
+            tc::split4(buf[j][i], hi, lo);
+            *reinterpret_cast<uint2*>(st + soff[i]) = hi;
+            *reinterpret_cast<uint2*>(st + F::A_PLANE + soff[i]) = lo;
           }
           if (c + PF < nchunks) load_next(buf[j]);           // refill this register slot
           tc::fence_async_smem();
           __syncwarp();
-          if ((lt & 31) == 0) { if (dbg & 1024) tc::mbar_arrive_relaxed(&full[s]); else tc::mbar_arrive(&full[s]); }  // one arrival per warp
-          // advance the store cursor
+          if ((lt & 31) == 0) tc::mbar_arrive(&full[s]);     // one arrival per warp
           wsrc += 2 * F::B_PLANE;
           if (++s_kc == nk) {
-            s_kc = 0; s_tile += gridDim.x; s_ntile = s_tile % n_tiles;
-            wsrc = Wimg + (int64_t)s_ntile * nk * 2 * F::B_PLANE;
+            s_kc = 0; s_tile += gridDim.x;
+            wsrc = p.w_image + (int64_t)(s_tile % n_tiles) * nk * 2 * F::B_PLANE;
           }
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
       }
     }
-  } else if (warp >= 1) {
-    // ================= epilogue =================
-    const int q = warp & 3;                              // TMEM lane quarter this warp may access
-    float* stg = reinterpret_cast<float*>(smem + F::PIPE_BYTES) + (warp - 1) * 32 * EPI_STRIDE;
-    uint32_t lt = 0;
-    for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++lt) {
-      const int acc = lt & 1;
-      const int m0 = (tile / n_tiles) * BM, n0 = (tile % n_tiles) * BN;
-      tc::mbar_wait(&tfull[acc], (lt >> 1) & 1);
-      tc::fence_after_sync();
-      // EC columns at a time: TMEM -> registers -> warp-private staging (thread per row) -> the warp writes one
-      // row's EC contiguous floats per instruction (512 B for EC = 128): long contiguous runs for DRAM.
-      constexpr int EC = BN < EPI_COLS ? BN : EPI_COLS;
-#pragma unroll 1
-      for (int c0 = 0; c0 < ((dbg & 32) ? 0 : BN); c0 += EC) {
-#pragma unroll 1
-        for (int cc = 0; cc < EC; cc += 32) {
-          float v[32];
-          tc::tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN + c0 + cc), v);
+    return;   // no block-wide barrier follows
+  }
+
+  // ================= consumers: MMA + epilogue =================
+  const int wg = warp >> 2;                                  // rows 64 wg .. 64 wg + 63 of the tile
+  const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's rows: r_lo, r_lo + 8
+  const int cq = 2 * (lane & 3);                             // and columns 8 j + cq, 8 j + cq + 1
+  const bool bnmode = p.bn_scale != nullptr;
+  const bool do_stats = p.stats != nullptr;
+  const int N = p.N;
+  float* stat = reinterpret_cast<float*>(smem + F::PIPE_BYTES) + warp * 2 * N;   // this warp's column partials
+  if (do_stats)
+    for (int i = lane; i < 2 * N; i += 32) stat[i] = 0.f;
+  const uint32_t sbase = tc::smem_u32(smem);
+  int s = 0, ph = 0;
+  for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+    const int m0 = (tile / n_tiles) * BM, n0 = (tile % n_tiles) * BN;
+    float acc[BN / 2];
 #pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            *reinterpret_cast<float4*>(stg + lane * EPI_STRIDE + cc + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-        }
-        __syncwarp();
-        constexpr int LPR = EC / 4;                          // lanes per row (float4 each): 32, 16 or 8
-        constexpr int RPI = 32 / LPR;                        // rows per store instruction
-        const int c4 = (lane % LPR) * 4;
-        float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (bias) b4 = __ldg(reinterpret_cast<const float4*>(bias + n0 + c0 + c4));
-        constexpr int RB = 8;                                // rows per batch: all residual loads of a batch first
-#pragma unroll 1
-        for (int rb = 0; rb < 32; rb += RB * RPI) {
-          float4 qv[RB];
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int kc = 0; kc < nk; ++kc) {
+      tc::mbar_wait(&full[s], ph);
+      const uint32_t sa = sbase + s * F::STAGE;
+      tc::wgmma_fence();
 #pragma unroll
-          for (int u = 0; u < RB; ++u) {
-            const int gr = m0 + q * 32 + rb + u * RPI + lane / LPR;
-            qv[u] = (R && gr < M) ? __ldcs(reinterpret_cast<const float4*>(R + (int64_t)gr * ldr + n0 + c0 + c4))
-                                  : make_float4(0.f, 0.f, 0.f, 0.f);
-          }
-#pragma unroll
-          for (int u = 0; u < RB; ++u) {
-            const int r = rb + u * RPI + lane / LPR;
-            const int gr = m0 + q * 32 + r;
-            float4 o = *reinterpret_cast<const float4*>(stg + r * EPI_STRIDE + c4);
-            o.x += b4.x + qv[u].x; o.y += b4.y + qv[u].y; o.z += b4.z + qv[u].z; o.w += b4.w + qv[u].w;
-            if (gr < M && !(dbg & 4)) *reinterpret_cast<float4*>(C + (int64_t)gr * ldc + n0 + c0 + c4) = o;
-          }
-        }
-        __syncwarp();
+      for (int j = 0; j < BK / 16; ++j) {
+        const uint32_t a_hi = sa + wg * 8 * SBO + j * 2 * LBO;
+        const uint32_t b_hi = sa + 2 * F::A_PLANE + j * 2 * LBO;
+        const uint64_t dah = tc::smem_desc(a_hi, LBO, SBO), dal = tc::smem_desc(a_hi + F::A_PLANE, LBO, SBO);
+        const uint64_t dbh = tc::smem_desc(b_hi, LBO, SBO), dbl = tc::smem_desc(b_hi + F::B_PLANE, LBO, SBO);
+        tc::Wgmma<BN>::template mma<0, 0>(acc, dal, dbh, 1);   // small terms first
+        tc::Wgmma<BN>::template mma<0, 0>(acc, dah, dbl, 1);
+        tc::Wgmma<BN>::template mma<0, 0>(acc, dah, dbh, 1);
       }
-      tc::fence_before_sync();
+      tc::wgmma_commit();
+      tc::wgmma_wait_all();
       __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&tempty[acc]);      // this accumulator buffer may be overwritten
+      if (lane == 0) tc::mbar_arrive(&empty[s]);             // this warp is done reading the stage
+      if (++s == STAGES) { s = 0; ph ^= 1; }
     }
-  } else if (lane == 0) {
-    // ================= MMA issuer (one thread) =================
-    constexpr uint32_t IDESC = tc::idesc_bf16_f32(BM, BN);
-    // descriptors differ only in their start-address field (bits [0,14), units of 16 bytes)
-    const uint64_t desc0 = tc::smem_desc(tc::smem_u32(smem), LBO, SBO);
-    uint32_t lt = 0;
-    int s = 0, ph = 0;
-    for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++lt) {
-      const int acc = lt & 1;
-      if (lt >= 2) tc::mbar_wait(&tempty[acc], ((lt >> 1) - 1) & 1);
-      tc::fence_after_sync();
-      const uint32_t d_tmem = tmem + (uint32_t)(acc * BN);
-      uint32_t accum = 0;
-      for (int kc = 0; kc < nk; ++kc) {
-        if (dbg & 512) tc::mbar_wait_poll(&full[s], ph); else tc::mbar_wait(&full[s], ph);
-        tc::fence_after_sync();
-        const uint64_t sd = desc0 + (uint64_t)((s * F::STAGE) >> 4);
-        if (!(dbg & 8)) {
+    // ---- epilogue from registers: (acc + bias) + (addend0 + addend1), row pieces of 8 bytes per lane ----
+    int ia[2], ib[2];
+    bool ok[2];
 #pragma unroll
-          for (int j = 0; j < BK / 16; ++j) {
-            const uint64_t a_hi = sd + (uint64_t)((j * 2 * LBO) >> 4);
-            const uint64_t a_lo = a_hi + (uint64_t)(F::A_PLANE >> 4);
-            const uint64_t b_hi = a_hi + (uint64_t)((2 * F::A_PLANE) >> 4);
-            const uint64_t b_lo = b_hi + (uint64_t)(F::B_PLANE >> 4);
-            tc::mma_bf16_ss(d_tmem, a_lo, b_hi, IDESC, accum);   // small terms first
-            tc::mma_bf16_ss(d_tmem, a_hi, b_lo, IDESC, 1);
-            tc::mma_bf16_ss(d_tmem, a_hi, b_hi, IDESC, 1);
-            accum = 1;
+    for (int h = 0; h < 2; ++h) {
+      const int gr = m0 + r_lo + 8 * h;
+      ok[h] = gr < M;
+      ia[h] = (p.add0 && ok[h]) ? (p.idx0 ? __ldg(p.idx0 + gr) : gr) : -1;
+      ib[h] = (p.add1 && ok[h]) ? (p.idx1 ? __ldg(p.idx1 + gr) : gr) : -1;
+    }
+    const float2 z2 = make_float2(0.f, 0.f);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int col = n0 + 8 * j + cq;
+      const float2 b2 = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : z2;
+      float2 sc = z2, sh = z2, mu = z2;
+      if (bnmode) {
+        sc = __ldg(reinterpret_cast<const float2*>(p.bn_scale + col));
+        sh = __ldg(reinterpret_cast<const float2*>(p.bn_shift + col));
+        mu = __ldg(reinterpret_cast<const float2*>(p.bn_mean + col));
+      }
+      float2 s2 = z2, q2 = z2;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float2 a0 = ia[h] >= 0 ? __ldg(reinterpret_cast<const float2*>(p.add0 + (int64_t)ia[h] * p.ld0 + col)) : z2;
+        const float2 mrow = ib[h] >= 0 ? __ldg(reinterpret_cast<const float2*>(p.add1 + (int64_t)ib[h] * p.ld1 + col)) : z2;
+        const float2 a1 = bnmode ? z2 : mrow;
+        float2 o;
+        o.x = (acc[4 * j + 2 * h] + b2.x) + (a0.x + a1.x);
+        o.y = (acc[4 * j + 2 * h + 1] + b2.y) + (a0.y + a1.y);
+        if (ok[h]) {
+          *reinterpret_cast<float2*>(p.C + (int64_t)(m0 + r_lo + 8 * h) * p.ldc + col) = o;
+          if (bnmode) {
+            // gu = o * silu'(m * scale + shift); sums of gu and gu * (m - mean): the two reductions of the train-mode
+            // BatchNorm backward for the layer that consumes this gradient
+            const float gx = o.x * dsilu_(fmaf(mrow.x, sc.x, sh.x)), gy = o.y * dsilu_(fmaf(mrow.y, sc.y, sh.y));
+            s2.x += gx; s2.y += gy;
+            q2.x = fmaf(gx, mrow.x - mu.x, q2.x); q2.y = fmaf(gy, mrow.y - mu.y, q2.y);
+          } else {
+            s2.x += o.x; s2.y += o.y;
+            q2.x = fmaf(o.x, o.x, q2.x); q2.y = fmaf(o.y, o.y, q2.y);
           }
         }
-        if (dbg & 256) tc::mbar_arrive(&empty[s]); else
-        tc::mma_commit(&empty[s]);                       // frees the stage when these MMAs retire
-        if (++s == STAGES) { s = 0; ph ^= 1; }
       }
-      tc::mma_commit(&tfull[acc]);                       // accumulator complete -> epilogue
+      if (do_stats) {
+        // lanes with equal (lane & 3) hold the same columns for the warp's 16 rows: fold them, fixed order
+#pragma unroll
+        for (int o = 4; o <= 16; o <<= 1) {
+          s2.x += __shfl_xor_sync(0xffffffffu, s2.x, o); s2.y += __shfl_xor_sync(0xffffffffu, s2.y, o);
+          q2.x += __shfl_xor_sync(0xffffffffu, q2.x, o); q2.y += __shfl_xor_sync(0xffffffffu, q2.y, o);
+        }
+        if (lane < 4) {
+          const int c = col;
+          stat[c] += s2.x; stat[c + 1] += s2.y;
+          stat[N + c] += q2.x; stat[N + c + 1] += q2.y;
+        }
+      }
     }
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tmem, F::TMEM_COLS);
+  if (do_stats) {
+    // one partial row per CTA: the eight consumer warps' partials summed in a fixed order
+    asm volatile("bar.sync 1, %0;" ::"n"(MMA_WARPS * 32) : "memory");
+    const float* all = reinterpret_cast<const float*>(smem + F::PIPE_BYTES);
+    float* out_row = p.stats + (int64_t)blockIdx.x * 2 * N;
+    for (int i = tid; i < 2 * N; i += MMA_WARPS * 32) {
+      float t = 0.f;
+#pragma unroll
+      for (int w = 0; w < MMA_WARPS; ++w) t += all[w * 2 * N + i];
+      out_row[i] = t;
+    }
+  }
 }
 
 // W[N,K] fp32 (row stride ldw; or, if transpose, the N x K matrix is W^T of a [K,N] array) ->
@@ -327,7 +338,7 @@ __global__ void prepare_weights_table_kernel(const alignn_b200_image_entry* __re
   uint2 h0, l0, h1, l1;
   tc::split4(make_float4(v[0], v[1], v[2], v[3]), h0, l0);
   tc::split4(make_float4(v[4], v[5], v[6], v[7]), h1, l1);
-  const int bn = (e.N % 256 == 0) ? 256 : (e.N % 128 == 0) ? 128 : (e.N % 64 == 0) ? 64 : 32;
+  const int bn = (e.N % 128 == 0) ? 128 : (e.N % 64 == 0) ? 64 : 32;   // pick_bn
   const int n = e.n_off + nl, k = e.k_off + k8 * 8;          // image coordinates (k_off is a multiple of 8)
   const int nt = n / bn, r = n % bn, kc = k / BK, kk = (k % BK) / 8;
   const int64_t b_plane = (int64_t)bn * BK * 2;
@@ -345,31 +356,46 @@ __global__ void prepare_bias_table_kernel(const alignn_b200_bias_entry* __restri
     e.dst[j] = e.a[j] + (e.b ? e.b[j] : 0.f);
 }
 
-inline int pick_bn(int N) { return (N % 256 == 0) ? 256 : (N % 128 == 0) ? 128 : (N % 64 == 0) ? 64 : (N % 32 == 0) ? 32 : 0; }
+// widest column tile that divides N: the accumulator of a 128 x BN tile is BN / 2 registers per consumer thread
+inline int pick_bn(int N) { return (N % 128 == 0) ? 128 : (N % 64 == 0) ? 64 : (N % 32 == 0) ? 32 : 0; }
+
+inline int num_sms() {
+  static int sms = 0;
+  if (!sms) {
+    int dev = 0, n = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    sms = n > 0 ? n : kNumSMs;
+  }
+  return sms;
+}
 
 template <int BN>
-int launch_gemm(const float* A, int64_t lda, const void* img, int M, int N, int K, const float* bias, const float* R,
-                int64_t ldr, float* C, int64_t ldc, cudaStream_t st) {
+int launch_bn(const Params& p, int grid, cudaStream_t st) {
   using F = Cfg<BN>;
   static alignn::DeviceOnce configured; int cfg_dev;   // idempotent attribute; a benign race sets it twice
   if (configured.needed(&cfg_dev)) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_nt_bf16x3_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, F::SMEM);
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16x3_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, F::SMEM);
     if (e != cudaSuccess) return record_cuda_error((int)e);
     configured.done(cfg_dev);
   }
-  const int total = ((M + BM - 1) / BM) * (N / BN);
-  const int grid = total < 148 ? total : 148;          // persistent: one CTA per SM
-  gemm_nt_bf16x3_kernel<BN><<<grid, THREADS, F::SMEM, st>>>(A, lda, reinterpret_cast<const uint8_t*>(img), M, N, K, bias, R,
-                                                           ldr, C, ldc, g_debug_flags);
+  gemm_bf16x3_kernel<BN><<<grid, THREADS, F::SMEM, st>>>(p);
   return check_launch();
+}
+
+inline int launch(const Params& p, int grid, cudaStream_t st) {
+  switch (pick_bn(p.N)) {
+    case 128: return launch_bn<128>(p, grid, st);
+    case 64: return launch_bn<64>(p, grid, st);
+    case 32: return launch_bn<32>(p, grid, st);
+    default: return ALIGNN_ERR_UNSUPPORTED_D;
+  }
 }
 
 }  // namespace gemm
 }  // namespace alignn
 
 extern "C" {
-
-void alignn_b200_debug_gemm_flags(int flags) { alignn::gemm::g_debug_flags = flags; }   /* not in the public header */
 
 size_t alignn_b200_gemm_weight_image_bytes(int N, int K) {
   if (N <= 0 || K <= 0 || alignn::gemm::pick_bn(N) == 0 || K % alignn::gemm::BK != 0) return 0;
@@ -386,8 +412,7 @@ int alignn_b200_gemm_prepare_weights(const float* W, int N, int K, int64_t ldw, 
   const int blocks = (int)((total + 255) / 256);
   cudaStream_t st = (cudaStream_t)stream;
   uint8_t* img = reinterpret_cast<uint8_t*>(image);
-  if (bn == 256) prepare_weights_kernel<256><<<blocks, 256, 0, st>>>(W, N, K, ldw, transpose, img);
-  else if (bn == 128) prepare_weights_kernel<128><<<blocks, 256, 0, st>>>(W, N, K, ldw, transpose, img);
+  if (bn == 128) prepare_weights_kernel<128><<<blocks, 256, 0, st>>>(W, N, K, ldw, transpose, img);
   else if (bn == 64) prepare_weights_kernel<64><<<blocks, 256, 0, st>>>(W, N, K, ldw, transpose, img);
   else prepare_weights_kernel<32><<<blocks, 256, 0, st>>>(W, N, K, ldw, transpose, img);
   return alignn::check_launch();
@@ -419,14 +444,55 @@ int alignn_b200_gemm_nt(const float* A, int64_t lda, const void* w_image, int64_
   if (!A || !w_image || !C || M > 0x7fffffff) return ALIGNN_ERR_BAD_ARG;
   if ((lda % 4) || (ldc % 4) || (R && (ldr % 4))) return ALIGNN_ERR_BAD_ARG;   // 16-byte row alignment
   const int bn = pick_bn(N);
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (bn) {
-    case 256: return launch_gemm<256>(A, lda, w_image, (int)M, N, K, bias, R, ldr, C, ldc, st);
-    case 128: return launch_gemm<128>(A, lda, w_image, (int)M, N, K, bias, R, ldr, C, ldc, st);
-    case 64: return launch_gemm<64>(A, lda, w_image, (int)M, N, K, bias, R, ldr, C, ldc, st);
-    case 32: return launch_gemm<32>(A, lda, w_image, (int)M, N, K, bias, R, ldr, C, ldc, st);
-    default: return ALIGNN_ERR_UNSUPPORTED_D;
-  }
+  if (bn == 0) return ALIGNN_ERR_UNSUPPORTED_D;
+  Params p = {};
+  p.A = A; p.lda = lda; p.w_image = reinterpret_cast<const uint8_t*>(w_image);
+  p.M = (int)M; p.N = N; p.K = K;
+  p.bias = bias;
+  p.add0 = R; p.ld0 = ldr;
+  p.C = C; p.ldc = ldc;
+  const int total = ((p.M + BM - 1) / BM) * (N / bn);
+  const int grid = total < num_sms() ? total : num_sms();   // persistent: one CTA per SM
+  return launch(p, grid, (cudaStream_t)stream);
+}
+
+int alignn_b200_gemm_gather_stat_rows(int64_t M, int N) {
+  using namespace alignn::gemm;
+  const int bn = pick_bn(N);
+  if (bn == 0 || M <= 0) return 0;
+  // CTAs of the launch, one partial row each
+  const int64_t total = (M + BM - 1) / BM * (N / bn);
+  return (int)(total < alignn::kNumSMs ? total : alignn::kNumSMs);
+}
+
+int alignn_b200_gemm_gather(const alignn_b200_gemm_gather_args* a) {
+  using namespace alignn::gemm;
+  if (!a) return ALIGNN_ERR_BAD_ARG;
+  if (a->struct_size != sizeof(*a)) return ALIGNN_ERR_STRUCT_SIZE;
+  if (a->M < 0 || a->N <= 0 || a->K <= 0 || a->K % BK != 0 || a->lda < a->K || a->ldc < a->N) return ALIGNN_ERR_BAD_ARG;
+  if (a->M == 0) return ALIGNN_OK;
+  if (!a->A || !a->w_image || !a->C || a->M > 0x7fffffff) return ALIGNN_ERR_BAD_ARG;
+  if ((a->lda % 4) || (a->ldc % 4) || ((uintptr_t)a->A & 15) || ((uintptr_t)a->C & 15)) return ALIGNN_ERR_BAD_ARG;
+  if (a->add0 && ((a->ld0 % 4) || a->ld0 < a->N || ((uintptr_t)a->add0 & 15))) return ALIGNN_ERR_BAD_ARG;
+  if (a->add1 && ((a->ld1 % 4) || a->ld1 < a->N || ((uintptr_t)a->add1 & 15))) return ALIGNN_ERR_BAD_ARG;
+  if ((a->idx0 && !a->add0) || (a->idx1 && !a->add1)) return ALIGNN_ERR_BAD_ARG;
+  const int bn = pick_bn(a->N);
+  if (bn == 0) return ALIGNN_ERR_UNSUPPORTED_D;
+  if (a->stats && a->N > kMaxStatN) return ALIGNN_ERR_BAD_ARG;   // column partials of every warp live in shared memory
+  if (a->bn_scale && (!a->bn_shift || !a->bn_mean || !a->add1 || !a->stats)) return ALIGNN_ERR_BAD_ARG;
+  Params p;
+  p.A = a->A; p.lda = a->lda;
+  p.M = (int)a->M; p.N = a->N; p.K = a->K;
+  p.w_image = reinterpret_cast<const uint8_t*>(a->w_image);
+  p.bias = a->bias;
+  p.add0 = a->add0; p.ld0 = a->ld0; p.idx0 = a->idx0;
+  p.add1 = a->add1; p.ld1 = a->ld1; p.idx1 = a->idx1;
+  p.C = a->C; p.ldc = a->ldc; p.stats = a->stats;
+  p.bn_scale = a->bn_scale; p.bn_shift = a->bn_shift; p.bn_mean = a->bn_mean;
+  const int total = ((p.M + BM - 1) / BM) * (p.N / bn);
+  int grid = total < num_sms() ? total : num_sms();
+  if (p.stats) grid = alignn_b200_gemm_gather_stat_rows(p.M, p.N);   // the caller sized `stats` for this many CTAs
+  return launch(p, grid, (cudaStream_t)a->stream);
 }
 
 }  // extern "C"

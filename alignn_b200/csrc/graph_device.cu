@@ -1,5 +1,5 @@
 // Device-side structure builders and the force / stress reductions of SURVEY.md section 8f -- the GPU twins of
-// csrc/graph_host.cu (sorted-CSR index, line graph, periodic radius scan; bit-identical outputs, validated on B200) and
+// csrc/graph_host.cu (sorted-CSR index, line graph, periodic radius scan; bit-identical outputs) and
 // the d=3 reductions of ALIGNN-FF (alignn/models/alignn_atomwise.py:547-563, 610-635).  Pure integer work except the two d=3 reductions; everything deterministic
 // (stable radix sort, fixed-order sums, integer atomics only for counting).  CUB (ships with the CUDA toolkit) does
 // the scans and the stable key-value sort; it is plumbing here, like cudart.

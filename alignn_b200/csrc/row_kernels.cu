@@ -1,4 +1,4 @@
-// Row-wise kernels around the conv stack, fp32, sm_100a (HBM-bound: every row is read once and written once,
+// Row-wise kernels around the conv stack, fp32, sm_90a (HBM-bound: every row is read once and written once,
 // one warp per row, 512 contiguous bytes per warp instruction -- common.cuh).
 //
 //   ln_silu_forward / ln_silu_backward: the LayerNorm -> SiLU tail of the embedding layers of the LayerNorm model
@@ -199,7 +199,7 @@ int alignn_b200_adamw_flat(float* param, float* grad, float* exp_avg, float* exp
   const int64_t n4 = n / 4;
   int64_t blocks = (n4 + 255) / 256;
   if (blocks < 1) blocks = 1;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > alignn::kNumSMs * 8) blocks = alignn::kNumSMs * 8;
   alignn::adamw_flat_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(param, grad, exp_avg, exp_avg_sq, n4, n, lr, beta1,
                                                                           beta2, eps, weight_decay, zero_grad, step, ticket);
   return alignn::check_launch();

@@ -1,12 +1,12 @@
 // STAGED WORK (see egc_fused.h): backward edge side of EdgeGatedGraphConv for train-mode BatchNorm in one persistent
-// tcgen05 kernel -- the per-edge part of egc_backward_dst_kernel fused with the data-gradient GEMM  gy = GM * W_eg.
+// wgmma kernel -- the per-edge part of egc_backward_dst_kernel fused with the data-gradient GEMM  gy = GM * W_eg.
 //
 //   gu_e  = gy_out_e * silu'(M_e * scale + shift) ;  xhat_e = (M_e - mean) * rstd                 (BatchNorm + SiLU backward)
 //   gm0_e = scale * gu_e - scale * (c1 + xhat_e * c2)
 //   sig_e = sigmoid(M_e) ;  gm_e = gm0_e + (GSh[dst_e] * P[src_e, d:2d] + GS[dst_e]) * sig_e * (1 - sig_e)   (gate backward)
 //   GM = gm ;  gy = GM * W_eg (+ gy_out) ;  GPB_v = sum_{e -> v} gm_e ;  partials = column sums of gm
 //
-// Warp roles: warp 0 = TMEM owner + MMA issuer; warps 1-4 = epilogue; warps 5-20 = PRODUCERS.  A producer thread owns
+// Warp roles: warps 0-3 = MMA warpgroup (accumulator tile in scratch, acc_sm90.cuh); warps 4-7 = epilogue; warps 8-23 = PRODUCERS.  A producer thread owns
 // one tile row and two 4-column fragments of every 128 x 32 chunk: it loads M, gy_out and the three gathered node-row
 // slices (all L2 hits: the next tile's M / gy_out rows are bulk-prefetched into L2 one tile ahead), forms gm, stores it
 // to GM and writes the bf16 hi/lo split of the same values into the operand planes -- the A operand never exists in
@@ -17,6 +17,7 @@
 #include <atomic>
 
 #include "../tc_common.cuh"
+#include "acc_sm90.cuh"
 #include "alignn_b200.h"
 #include "egc_fused.h"
 
@@ -31,12 +32,12 @@ constexpr int EPI_WARPS = 4;
 constexpr int EPI_THREADS = 32 * EPI_WARPS;
 constexpr int PROD_WARPS = 16;
 constexpr int NF = 32 / PROD_WARPS;           // fragments per producer thread and chunk: 2
-constexpr int THREADS = 32 * (1 + EPI_WARPS + PROD_WARPS);   // 672
+constexpr int THREADS = 32 * (4 + EPI_WARPS + PROD_WARPS);   // 768
 constexpr uint32_t LBO = 128;
 constexpr uint32_t SBO = (BK / 8) * 128;
 constexpr int EPI_COLS = 128;
 constexpr int EPI_STRIDE = EPI_COLS + 4;
-constexpr int kSMs = 148;
+constexpr int kSMs = 132;
 
 template <int D>
 struct Cfg {
@@ -55,8 +56,7 @@ struct Cfg {
   static constexpr int SEG_BYTES = ((2 * BM + 1) * 4 + 15) / 16 * 16;
   static constexpr int BAR_OFF = SEG_OFF + SEG_BYTES;
   static constexpr int SMEM = BAR_OFF + 128;
-  static constexpr int TMEM_COLS = 2 * D < 32 ? 32 : 2 * D;
-  static_assert(SMEM <= 232448, "shared memory budget of one sm_100 CTA");
+  static_assert(SMEM <= 232448, "shared memory budget of one sm_90 CTA");
 };
 
 __host__ __device__ constexpr int plane_off(int r, int k) { return (r >> 3) * (int)SBO + (k >> 3) * 128 + (r & 7) * 16 + (k & 7) * 2; }
@@ -79,7 +79,7 @@ __device__ __forceinline__ float gm_elem(float m, float go, bool has_go, float c
 
 template <int D>
 __global__ void __launch_bounds__(THREADS, 1)
-egc_backward_fused_kernel(const alignn_b200_egc_bwd_fused_args a) {
+egc_backward_fused_kernel(const alignn_b200_egc_bwd_fused_args a, float* __restrict__ scratch_all) {
   using F = Cfg<D>;
   extern __shared__ __align__(128) uint8_t smem[];
   float* stat = reinterpret_cast<float*>(smem + F::STAT_OFF);
@@ -90,7 +90,6 @@ egc_backward_fused_kernel(const alignn_b200_egc_bwd_fused_args a) {
   uint64_t* empty = full + STAGES;
   uint64_t* tfull = empty + STAGES;
   uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   constexpr int nk = D / BK;
@@ -108,24 +107,22 @@ egc_backward_fused_kernel(const alignn_b200_egc_bwd_fused_args a) {
   }
   for (int i = tid; i < EPI_WARPS * D; i += THREADS) stat[i] = 0.f;
   if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full[s], PROD_WARPS + 1); tc::mbar_init(&empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { tc::mbar_init(&tfull[b], 1); tc::mbar_init(&tempty[b], EPI_WARPS); }
+    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full[s], PROD_WARPS + 1); tc::mbar_init(&empty[s], 4); }
+    for (int b = 0; b < 2; ++b) { tc::mbar_init(&tfull[b], 128); tc::mbar_init(&tempty[b], EPI_WARPS); }
     tc::mbar_fence_init();
   }
-  if (warp == 0) tc::tmem_alloc(tmem_slot, F::TMEM_COLS);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
+  const uint32_t tmem = 0;                                  // accumulator "address": see acc_sm90.cuh
+  float* const scr = scratch_all + (size_t)blockIdx.x * staged_acc::kRows * 2 * D;
 
-  if (warp >= 1 + EPI_WARPS) {
+  if (warp >= 4 + EPI_WARPS) {
     // ================= producers: gm per element -> GM (HBM) and bf16 hi/lo planes (smem) =================
     // Thread -> ONE tile row and two (4-column) fragments of every chunk: row = 8 * warp + ((lane >> 1) & 7),
     // float4 index kq_i = 4 i + 2 (lane >> 4) + (lane & 1).  A half-warp covers 8 rows x 2 adjacent float4 per
     // fragment: conflict-free 64-bit plane stores and full 32-byte sectors on every global access.
     // No register prefetch ring (the register budget of 21 warps is 80): the NEXT tile's M / gy_out rows are pulled
     // into L2 by bulk prefetches one tile ahead, so every load below is an L2 hit and the 4 warps per scheduler cover it.
-    const int pt = tid - 32 * (1 + EPI_WARPS);          // 0..511
+    const int pt = tid - 32 * (4 + EPI_WARPS);          // 0..511
     const int pw = pt >> 5;
     const bool has_go = a.gy_out != nullptr;
     const int prow = pw * 8 + ((lane >> 1) & 7);
@@ -168,7 +165,6 @@ egc_backward_fused_kernel(const alignn_b200_egc_bwd_fused_args a) {
       const float* ph_ = a.GSh + tr * D;
       const float* ps = a.GS + tr * D;
       float* pgm = a.GM + e * D;
-      const uint8_t* wsrc = wimg;
 #pragma unroll 1
       for (int kc = 0; kc < nk; ++kc, ++c) {
         // all global loads of this chunk first (two fragments x five arrays), then the waits and the math
@@ -187,9 +183,8 @@ egc_backward_fused_kernel(const alignn_b200_egc_bwd_fused_args a) {
         uint8_t* st = smem + s * F::STAGE;
         if (pt == 0) {   // weight chunk: one contiguous bulk copy (both planes), counted in bytes on full[s]
           tc::mbar_arrive_expect_tx(&full[s], 2 * F::B_PLANE);
-          tc::bulk_g2s(st + 2 * F::A_PLANE, wsrc, 2 * F::B_PLANE, &full[s]);
+          staged_acc::copy_weight_chunk<D, nk>(st + 2 * F::A_PLANE, wimg, kc, &full[s]);
         }
-        wsrc += 2 * F::B_PLANE;
 #pragma unroll
         for (int i = 0; i < NF; ++i) {
           const int col = kc * BK + fkq[i] * 4;
@@ -216,12 +211,12 @@ egc_backward_fused_kernel(const alignn_b200_egc_bwd_fused_args a) {
         if (++s == STAGES) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp >= 1) {
+  } else if (warp >= 4) {
     // ================= epilogue: gy = acc (+ gy_out), then per-segment sums of the tile's GM rows =================
     const int q = warp & 3;
     const int et = q * 32 + lane;
-    float* stg = reinterpret_cast<float*>(smem + F::EPI_OFF) + (warp - 1) * 32 * EPI_STRIDE;
-    float* wstat = stat + (warp - 1) * D;
+    float* stg = reinterpret_cast<float*>(smem + F::EPI_OFF) + (warp - 4) * 32 * EPI_STRIDE;
+    float* wstat = stat + (warp - 4) * D;
     int4 n_desc = make_int4(0, 0, 0, 0);
     int n_e = 0, n_seg = 0, n_seg_last = 0;
     auto fetch_meta = [&](int tile) {
@@ -246,15 +241,14 @@ egc_backward_fused_kernel(const alignn_b200_egc_bwd_fused_args a) {
       fetch_meta(tile + gridDim.x);
       epi_bar();
       tc::mbar_wait(&tfull[acc], (lt >> 1) & 1);
-      tc::fence_after_sync();
-      if (a.gy) {
+            if (a.gy) {
         constexpr int EC = F::EC;
 #pragma unroll 1
         for (int c0 = 0; c0 < D; c0 += EC) {
 #pragma unroll 1
           for (int cc = 0; cc < EC; cc += 32) {
             float v[32];
-            tc::tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * D + c0 + cc), v);
+            staged_acc::ld<32>(scr, 2 * D, tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * D + c0 + cc), v);
 #pragma unroll
             for (int j = 0; j < 32; j += 4)
               *reinterpret_cast<float4*>(stg + lane * EPI_STRIDE + cc + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
@@ -286,14 +280,14 @@ egc_backward_fused_kernel(const alignn_b200_egc_bwd_fused_args a) {
           __syncwarp();
         }
       }
-      tc::fence_before_sync();
+      __threadfence_block();
       __syncwarp();
       if (lane == 0) tc::mbar_arrive(&tempty[acc]);      // accumulator drained: the next tile's MMAs may start
       // ---- per-segment sums of this tile's GM rows (written by the producers, read back through L2) ----
       constexpr int VPL = D / 32;                          // values per lane, row spread over the warp
       constexpr int W = (D % 128 == 0) ? 4 : ((D % 64 == 0) ? 2 : 1);
       constexpr int CH = D / (32 * W);
-      for (int j = warp - 1; j < nseg; j += EPI_WARPS) {
+      for (int j = warp - 4; j < nseg; j += EPI_WARPS) {
         float accb[VPL];
 #pragma unroll
         for (int k = 0; k < VPL; ++k) accb[k] = 0.f;
@@ -334,42 +328,11 @@ egc_backward_fused_kernel(const alignn_b200_egc_bwd_fused_args a) {
         out_row[i] = t;
       }
     }
-  } else if (lane == 0) {
-    // ================= MMA issuer (one thread) =================
-    constexpr uint32_t IDESC = tc::idesc_bf16_f32(BM, D);
-    const uint64_t desc0 = tc::smem_desc(tc::smem_u32(smem), LBO, SBO);
-    uint32_t lt = 0;
-    int s = 0, ph = 0;
-    for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++lt) {
-      const int acc = lt & 1;
-      if (lt >= 2) tc::mbar_wait(&tempty[acc], ((lt >> 1) - 1) & 1);
-      tc::fence_after_sync();
-      const uint32_t d_tmem = tmem + (uint32_t)(acc * D);
-      uint32_t accum = 0;
-      for (int kc = 0; kc < nk; ++kc) {
-        tc::mbar_wait(&full[s], ph);
-        tc::fence_after_sync();
-        const uint64_t sd = desc0 + (uint64_t)((s * F::STAGE) >> 4);
-#pragma unroll
-        for (int j = 0; j < BK / 16; ++j) {
-          const uint64_t a_hi = sd + (uint64_t)((j * 2 * LBO) >> 4);
-          const uint64_t a_lo = a_hi + (uint64_t)(F::A_PLANE >> 4);
-          const uint64_t b_hi = a_hi + (uint64_t)((2 * F::A_PLANE) >> 4);
-          const uint64_t b_lo = b_hi + (uint64_t)(F::B_PLANE >> 4);
-          tc::mma_bf16_ss(d_tmem, a_lo, b_hi, IDESC, accum);
-          tc::mma_bf16_ss(d_tmem, a_hi, b_lo, IDESC, 1);
-          tc::mma_bf16_ss(d_tmem, a_hi, b_hi, IDESC, 1);
-          accum = 1;
-        }
-        tc::mma_commit(&empty[s]);
-        if (++s == STAGES) { s = 0; ph ^= 1; }
-      }
-      tc::mma_commit(&tfull[acc]);
-    }
+  } else {
+    // ================= MMA warpgroup (warps 0-3): the accumulator tile in scratch =================
+    // 64-column blocks: 768 threads leave 80 registers per thread
+    staged_acc::mma_warpgroup<D, F::STAGE, F::A_PLANE, STAGES, (D < 64 ? D : 64)>(smem, full, empty, tfull, tempty, scr, total);
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tmem, F::TMEM_COLS);
 }
 
 template <int D>
@@ -382,7 +345,10 @@ int launch(const alignn_b200_egc_bwd_fused_args& a) {
     configured = true;
   }
   const int grid = a.num_tiles < kSMs ? a.num_tiles : kSMs;
-  egc_backward_fused_kernel<D><<<grid, THREADS, F::SMEM, (cudaStream_t)a.stream>>>(a);
+  cudaError_t se;
+  float* scr = staged_acc::scratch((size_t)grid * staged_acc::kRows * 2 * D * sizeof(float), &se);
+  if (!scr) { fused::g_last_cuda_error.store((int)se); return ALIGNN_ERR_CUDA; }
+  egc_backward_fused_kernel<D><<<grid, THREADS, F::SMEM, (cudaStream_t)a.stream>>>(a, scr);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { fused::g_last_cuda_error.store((int)e); return ALIGNN_ERR_CUDA; }
   return ALIGNN_OK;

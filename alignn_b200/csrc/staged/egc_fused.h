@@ -1,14 +1,12 @@
 /* EXPERIMENTAL -- not part of libalignn_b200.so, not declared in include/alignn_b200.h.
- * Status (round 2): ran on B200, bit-identical to the shipped two-kernel path (tests/test_staged.py), measured ~2x
- * SLOWER than it (profiles/r02_staged_fused_ab.jsonl): the row-per-thread epilogue is bound by L2 gather latency.
- * The shipped forward is the two-pass composition of DESIGN.md section 2.  Original header follows.
+ * Status: bit-identical to the shipped two-kernel forward (tests/test_staged.py) but not the shipped path.  On sm_90 the
+ * accumulator tile lives in a per-CTA global scratch tile (acc_sm90.cuh), which costs L2 traffic the shipped path
+ * does not pay.  The shipped forward is the two-pass composition of DESIGN.md.
  *
  * One-kernel forward of the edge side of EdgeGatedGraphConv (alignn/models/alignn.py:100-109,123,127):
- * the edge-gate Linear (`self.edge_gate(edge_feats)`, :101) runs on tcgen05 into TMEM and the gate / segment-sum
- * epilogue consumes the accumulator there, so G = edge_gate(y) never exists in HBM (DESIGN.md "known deviations"
- * item 1).  Written in round 1 after the GPU budget was spent: compiles for sm_100a, has NOT run on hardware yet.
- * tools/build_staged.py builds it into alignn_b200/csrc/staged/libalignn_b200_staged.so; tests/test_gpu_staged.py
- * (opt-in: ALIGNN_B200_STAGED=1) compares it bit for bit with the shipped two-kernel path.
+ * the edge-gate Linear (`self.edge_gate(edge_feats)`, :101) runs on wgmma and the gate / segment-sum epilogue
+ * consumes the accumulator tile, so G = edge_gate(y) is never written as a Linear output.
+ * tools/build_staged.py builds this library into alignn_b200/csrc/staged/libalignn_b200_staged.so.
  */
 #ifndef ALIGNN_B200_STAGED_EGC_FUSED_H
 #define ALIGNN_B200_STAGED_EGC_FUSED_H
@@ -49,7 +47,7 @@ typedef struct {
   float* y_out;     /* [Ne,d] or NULL; written for AFFINE / LAYER */
   float* XP;        /* [Nn,d] x' = src_update(x) + h  (always) */
   float* S; float* H; /* [Nn,d] or NULL (inference) */
-  float* partials;  /* STATS: [min(num_tiles,148)][2][d] = column sums of m and m^2 */
+  float* partials;  /* STATS: [min(num_tiles,132)][2][d] = column sums of m and m^2 */
   void* stream;
 } alignn_b200_egc_fused_fwd_args;
 
@@ -93,7 +91,7 @@ typedef struct {
   float* GM;             /* [Ne,d] */
   float* gy;             /* [Ne,d] or NULL */
   float* GPB; int64_t ld_gpb;   /* dL/d e_dst rows, e.g. GP + 2d with ld 4d */
-  float* partials;       /* [min(num_tiles,148)][d] column sums of gm (= bias gradients of edge_gate and dst_gate) */
+  float* partials;       /* [min(num_tiles,132)][d] column sums of gm (= bias gradients of edge_gate and dst_gate) */
   void* stream;
 } alignn_b200_egc_bwd_fused_args;
 

@@ -1,4 +1,4 @@
-// STAGED WORK (see egc_fused.h): edge-gate GEMM + gate + segment sums in ONE persistent tcgen05 kernel.
+// STAGED WORK (see egc_fused.h): edge-gate GEMM + gate + segment sums in ONE persistent wgmma kernel.
 //
 //   m_e   = edge_gate(y)_e + P[src_e, 0:d] + P[dst_e, 2d:3d]            (alignn.py:100-101)
 //   sig_e = sigmoid(m_e)                                                  (:103)
@@ -10,18 +10,19 @@
 // whole in-edge segments (host packer below), so every segment sum is finished inside one CTA -- no atomics, fixed
 // summation order (the same order as the shipped row-per-warp kernel, which makes M / S / H / x' bit-identical to it).
 //
-// Warp roles (as in gemm_tc.cu): warp 0 = TMEM owner + MMA issuer, warps 1-4 = epilogue, warps 5-12 = loaders
+// Warp roles: warps 0-3 = MMA warpgroup (accumulator tile in scratch, acc_sm90.cuh), then the epilogue warps, then 8 loaders
 // (gather y rows by edge id, fp32 -> bf16 hi/lo planes; the weight image arrives by cp.async.bulk).
 // Epilogue, per 32-column chunk of the [128 x d] accumulator:
-//   row phase    (thread = edge row = TMEM lane): tcgen05.ld, gather the three P slices of the row (128 B each),
+//   row phase    (thread = edge row): accumulator row, gather the three P slices of the row (128 B each),
 //                m, M store, sigmoid; sigma / Bh / m go to a padded smem staging tile;
 //   column phase (thread = column x row group): per-segment sums over consecutive staged rows -> S, H, x' rows
 //                (coalesced 128 B), BatchNorm column sums of m, m^2 into per-warp smem accumulators.
-// LayerNorm: m is written back into the accumulator (tcgen05.st) during the row phase, then two more TMEM passes
+// LayerNorm: m is written back into the accumulator during the row phase, then two more accumulator passes
 // give the two-pass variance and the normalised output, all by the thread that owns the row.
 #include <atomic>
 
 #include "../tc_common.cuh"
+#include "acc_sm90.cuh"
 #include "alignn_b200.h"
 #include "egc_fused.h"
 
@@ -35,7 +36,7 @@ constexpr int LOAD_WARPS = 8;
 constexpr int GROUP_THREADS = 128;            // one epilogue group = 4 warps = one thread per tile row
 constexpr uint32_t LBO = 128;
 constexpr uint32_t SBO = (BK / 8) * 128;
-constexpr int kSMs = 148;
+constexpr int kSMs = 132;
 
 std::atomic<int> g_last_cuda_error{0};   // shared with egc_bwd_fused_tc.cu
 
@@ -45,7 +46,7 @@ std::atomic<int> g_last_cuda_error{0};   // shared with egc_bwd_fused_tc.cu
 template <int D, int EG>
 struct Cfg {
   static constexpr int EPI_WARPS = 4 * EG;
-  static constexpr int THREADS = 32 * (1 + EPI_WARPS + LOAD_WARPS);   // 416 / 544
+  static constexpr int THREADS = 32 * (4 + EPI_WARPS + LOAD_WARPS);   // 512 / 640
   static constexpr int CC = 32 / EG;            // columns per epilogue chunk
   static constexpr int NG = GROUP_THREADS / CC; // row groups of the column phase (4 / 8)
   static constexpr int STG = CC + 4;            // staging row stride in floats (16-byte rows, conflict-free both ways)
@@ -65,8 +66,7 @@ struct Cfg {
   static constexpr int XCH_BYTES = EG * BM * 4;
   static constexpr int BAR_OFF = XCH_OFF + XCH_BYTES;
   static constexpr int SMEM = BAR_OFF + 128;
-  static constexpr int TMEM_COLS = 2 * D < 32 ? 32 : 2 * D;     // double-buffered accumulator
-  static_assert(SMEM <= 232448, "shared memory budget of one sm_100 CTA");
+  static_assert(SMEM <= 232448, "shared memory budget of one sm_90 CTA");
   static_assert(D % (EG * CC) == 0, "chunks must tile the row");
 };
 
@@ -85,65 +85,12 @@ __device__ __forceinline__ void group_bar(int grp) { asm volatile("bar.sync %0, 
 template <int EG>
 __device__ __forceinline__ void all_epi_bar() { asm volatile("bar.sync 3, %0;" ::"n"(EG * GROUP_THREADS) : "memory"); }
 
-// TMEM <-> registers, 32 lanes x N columns of fp32 (thread t of the warp <-> lane base + t)
-template <int N>
-__device__ __forceinline__ void tmem_ld(uint32_t taddr, float (&v)[N]) {
-  static_assert(N == 16 || N == 32, "chunk width");
-  uint32_t r[N];
-  if constexpr (N == 32) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-  } else {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-  }
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < N; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-template <int N>
-__device__ __forceinline__ void tmem_st(uint32_t taddr, const float (&v)[N]) {
-  static_assert(N == 16 || N == 32, "chunk width");
-#define U(i) "r"(__float_as_uint(v[i]))
-  if constexpr (N == 32) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), U(0), U(1), U(2), U(3), U(4), U(5), U(6), U(7), U(8), U(9), U(10), U(11), U(12), U(13), U(14), U(15),
-          U(16), U(17), U(18), U(19), U(20), U(21), U(22), U(23), U(24), U(25), U(26), U(27), U(28), U(29), U(30), U(31)
-        : "memory");
-  } else {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-        ::"r"(taddr), U(0), U(1), U(2), U(3), U(4), U(5), U(6), U(7), U(8), U(9), U(10), U(11), U(12), U(13), U(14), U(15)
-        : "memory");
-  }
-#undef U
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + __expf(-x)); }   // as common.cuh
 __device__ __forceinline__ float silu_(float u) { return u * sigmoidf_(u); }
 
 template <int D, int EG>
 __global__ void __launch_bounds__(Cfg<D, EG>::THREADS, 1)
-egc_forward_fused_kernel(const alignn_b200_egc_fused_fwd_args a) {
+egc_forward_fused_kernel(const alignn_b200_egc_fused_fwd_args a, float* __restrict__ scratch_all) {
   using F = Cfg<D, EG>;
   constexpr int CC = F::CC, STG = F::STG, NG = F::NG, EPI_WARPS = F::EPI_WARPS;
   extern __shared__ __align__(128) uint8_t smem[];
@@ -154,7 +101,6 @@ egc_forward_fused_kernel(const alignn_b200_egc_fused_fwd_args a) {
   uint64_t* empty = full + STAGES;
   uint64_t* tfull = empty + STAGES;
   uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   constexpr int nk = D / BK;
@@ -162,19 +108,17 @@ egc_forward_fused_kernel(const alignn_b200_egc_fused_fwd_args a) {
   const int4* tiles = reinterpret_cast<const int4*>(a.tiles);    // {v0, nseg, p0, rows}
 
   if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full[s], LOAD_WARPS + 1); tc::mbar_init(&empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { tc::mbar_init(&tfull[b], 1); tc::mbar_init(&tempty[b], EPI_WARPS); }
+    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full[s], LOAD_WARPS + 1); tc::mbar_init(&empty[s], 4); }
+    for (int b = 0; b < 2; ++b) { tc::mbar_init(&tfull[b], 128); tc::mbar_init(&tempty[b], EPI_WARPS); }
     tc::mbar_fence_init();
   }
-  if (warp == 0) tc::tmem_alloc(tmem_slot, F::TMEM_COLS);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
+  const uint32_t tmem = 0;                                  // accumulator "address": see acc_sm90.cuh
+  float* const scr = scratch_all + (size_t)blockIdx.x * staged_acc::kRows * 2 * D;
 
-  if (warp >= 1 + EPI_WARPS) {
+  if (warp >= 4 + EPI_WARPS) {
     // ================= loaders: gather y rows by edge id, split to bf16 hi/lo planes =================
-    const int lt = tid - 32 * (1 + EPI_WARPS);          // 0..255
+    const int lt = tid - 32 * (4 + EPI_WARPS);          // 0..255
     constexpr int PF = 3;
     float4 buf[PF][4];
     int soff[4], arow[4], akq[4];
@@ -227,7 +171,6 @@ egc_forward_fused_kernel(const alignn_b200_egc_fused_fwd_args a) {
       if (j < nchunks) load_next(buf[j]);
     int s = 0, ph = 0, s_kc = 0;
     const uint8_t* wimg = reinterpret_cast<const uint8_t*>(a.w_image);
-    const uint8_t* wsrc = wimg;
     for (int c0 = 0; c0 < nchunks; c0 += PF) {
 #pragma unroll
       for (int j = 0; j < PF; ++j) {
@@ -237,7 +180,7 @@ egc_forward_fused_kernel(const alignn_b200_egc_fused_fwd_args a) {
           uint8_t* st = smem + s * F::STAGE;
           if (lt == 0) {   // weight chunk: one contiguous bulk copy (both planes), counted in bytes on full[s]
             tc::mbar_arrive_expect_tx(&full[s], 2 * F::B_PLANE);
-            tc::bulk_g2s(st + 2 * F::A_PLANE, wsrc, 2 * F::B_PLANE, &full[s]);
+            staged_acc::copy_weight_chunk<D, nk>(st + 2 * F::A_PLANE, wimg, s_kc, &full[s]);
           }
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
@@ -250,16 +193,15 @@ egc_forward_fused_kernel(const alignn_b200_egc_fused_fwd_args a) {
           tc::fence_async_smem();
           __syncwarp();
           if ((lt & 31) == 0) tc::mbar_arrive(&full[s]);
-          wsrc += 2 * F::B_PLANE;
-          if (++s_kc == nk) { s_kc = 0; wsrc = wimg; }
+          if (++s_kc == nk) s_kc = 0;
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
       }
     }
-  } else if (warp >= 1) {
+  } else if (warp >= 4) {
     // ================= epilogue =================
-    const int q = warp & 3;                   // TMEM lane quarter this warp may access = its 32 tile rows
-    const int grp = (warp - 1) >> 2;          // epilogue group: owns chunks grp, grp + EG, ...
+    const int q = warp & 3;                   // this warp's 32 tile rows of the accumulator
+    const int grp = (warp - 4) >> 2;          // epilogue group: owns chunks grp, grp + EG, ...
     const int et = q * 32 + lane;             // tile row owned in the row phase (and: which seg[] entry it fills)
     const int ea = grp * GROUP_THREADS + et;  // index among all epilogue threads
     const int col = et % CC;                  // column phase: this thread's column inside the chunk ...
@@ -310,8 +252,7 @@ egc_forward_fused_kernel(const alignn_b200_egc_fused_fwd_args a) {
       if (et == 0 && nseg == BM) seg[BM] = n_seg_last;
       fetch_meta(tile + gridDim.x);
       tc::mbar_wait(&tfull[acc], (lt >> 1) & 1);
-      tc::fence_after_sync();
-      const uint32_t trow = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * D);
+            const uint32_t trow = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * D);
       const float* pa = a.P + s * 4 * D;              // [e_src | Bh] of the source row
       const float* pb = a.P + t * 4 * D + 2 * D;      // e_dst of the destination row
       float row_sum = 0.f;
@@ -319,7 +260,7 @@ egc_forward_fused_kernel(const alignn_b200_egc_fused_fwd_args a) {
       for (int c0 = grp * CC; c0 < D; c0 += EG * CC) {
         // ---------------- row phase ----------------
         float v[CC];
-        tmem_ld<CC>(trow + (uint32_t)c0, v);
+        staged_acc::ld<CC>(scr, 2 * D, trow + (uint32_t)c0, v);
         float* srow = sig + et * STG;
         float* crow = sgc + et * STG;
         float* mrow = mst + et * STG;
@@ -375,9 +316,9 @@ egc_forward_fused_kernel(const alignn_b200_egc_fused_fwd_args a) {
 #pragma unroll
           for (int j = 0; j < CC; j += 4) *reinterpret_cast<float4*>(mrow + j) = make_float4(0.f, 0.f, 0.f, 0.f);
         }
-        // LayerNorm: keep m in the accumulator for the two passes below.  tcgen05.st is warp-collective
+        // LayerNorm: keep m in the accumulator for the two passes below.  The store is per warp
         // (.sync.aligned), so it sits outside the `valid` branch; rows past the tile's end store junk nobody reads.
-        if (layer_out) tmem_st<CC>(trow + (uint32_t)c0, v);
+        if (layer_out) staged_acc::st<CC>(scr, 2 * D, trow + (uint32_t)c0, v);
         group_bar(grp);
         // ---------------- column phase: thread = (column `col`, row group `rg`) ----------------
         for (int j = rg; j < nseg; j += NG) {
@@ -411,8 +352,8 @@ egc_forward_fused_kernel(const alignn_b200_egc_fused_fwd_args a) {
         group_bar(grp);                        // staging tile (and, after the last chunk, seg[]) free again
       }
       if (layer_out) {
-        // two more passes over the row in TMEM: variance about the mean (two-pass, like torch), then the output.
-        // Every lane runs the warp-collective tcgen05.ld; only rows inside the tile store.  With two groups each
+        // two more passes over the row in the accumulator: variance about the mean (two-pass, like torch), then the output.
+        // Every lane runs the per-warp accumulator load; only rows inside the tile store.  With two groups each
         // holds the statistics of its own chunks: exchange through shared memory.
         float mean;
         if constexpr (EG == 1) {
@@ -430,7 +371,7 @@ egc_forward_fused_kernel(const alignn_b200_egc_fused_fwd_args a) {
 #pragma unroll 1
         for (int c0 = grp * CC; c0 < D; c0 += EG * CC) {
           float v[CC];
-          tmem_ld<CC>(trow + (uint32_t)c0, v);
+          staged_acc::ld<CC>(scr, 2 * D, trow + (uint32_t)c0, v);
 #pragma unroll
           for (int j = 0; j < CC; ++j) { const float dlt = v[j] - mean; qsum += dlt * dlt; }
         }
@@ -446,7 +387,7 @@ egc_forward_fused_kernel(const alignn_b200_egc_fused_fwd_args a) {
 #pragma unroll 1
         for (int c0 = grp * CC; c0 < D; c0 += EG * CC) {
           float v[CC];
-          tmem_ld<CC>(trow + (uint32_t)c0, v);
+          staged_acc::ld<CC>(scr, 2 * D, trow + (uint32_t)c0, v);
           if (valid) {
             float4* yo = reinterpret_cast<float4*>(a.y_out + e * D + c0);
             const float4* yi = reinterpret_cast<const float4*>(a.y + e * D + c0);
@@ -465,7 +406,7 @@ egc_forward_fused_kernel(const alignn_b200_egc_fused_fwd_args a) {
           }
         }
       }
-      tc::fence_before_sync();
+      __threadfence_block();
       __syncwarp();
       if (lane == 0) tc::mbar_arrive(&tempty[acc]);
     }
@@ -480,42 +421,10 @@ egc_forward_fused_kernel(const alignn_b200_egc_fused_fwd_args a) {
         out_row[i] = t;
       }
     }
-  } else if (lane == 0) {
-    // ================= MMA issuer (one thread) =================
-    constexpr uint32_t IDESC = tc::idesc_bf16_f32(BM, D);
-    const uint64_t desc0 = tc::smem_desc(tc::smem_u32(smem), LBO, SBO);
-    uint32_t lt = 0;
-    int s = 0, ph = 0;
-    for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++lt) {
-      const int acc = lt & 1;
-      if (lt >= 2) tc::mbar_wait(&tempty[acc], ((lt >> 1) - 1) & 1);
-      tc::fence_after_sync();
-      const uint32_t d_tmem = tmem + (uint32_t)(acc * D);
-      uint32_t accum = 0;
-      for (int kc = 0; kc < nk; ++kc) {
-        tc::mbar_wait(&full[s], ph);
-        tc::fence_after_sync();
-        const uint64_t sd = desc0 + (uint64_t)((s * F::STAGE) >> 4);
-#pragma unroll
-        for (int j = 0; j < BK / 16; ++j) {
-          const uint64_t a_hi = sd + (uint64_t)((j * 2 * LBO) >> 4);
-          const uint64_t a_lo = a_hi + (uint64_t)(F::A_PLANE >> 4);
-          const uint64_t b_hi = a_hi + (uint64_t)((2 * F::A_PLANE) >> 4);
-          const uint64_t b_lo = b_hi + (uint64_t)(F::B_PLANE >> 4);
-          tc::mma_bf16_ss(d_tmem, a_lo, b_hi, IDESC, accum);   // same order as gemm_tc.cu: bit-identical accumulators
-          tc::mma_bf16_ss(d_tmem, a_hi, b_lo, IDESC, 1);
-          tc::mma_bf16_ss(d_tmem, a_hi, b_hi, IDESC, 1);
-          accum = 1;
-        }
-        tc::mma_commit(&empty[s]);
-        if (++s == STAGES) { s = 0; ph ^= 1; }
-      }
-      tc::mma_commit(&tfull[acc]);
-    }
+  } else {
+    // ================= MMA warpgroup (warps 0-3): the accumulator tile in scratch =================
+    staged_acc::mma_warpgroup<D, F::STAGE, F::A_PLANE, STAGES>(smem, full, empty, tfull, tempty, scr, total);
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tmem, F::TMEM_COLS);
 }
 
 template <int D, int EG>
@@ -528,7 +437,10 @@ int launch(const alignn_b200_egc_fused_fwd_args& a) {
     configured = true;
   }
   const int grid = a.num_tiles < kSMs ? a.num_tiles : kSMs;
-  egc_forward_fused_kernel<D, EG><<<grid, F::THREADS, F::SMEM, (cudaStream_t)a.stream>>>(a);
+  cudaError_t se;
+  float* scr = staged_acc::scratch((size_t)grid * staged_acc::kRows * 2 * D * sizeof(float), &se);
+  if (!scr) { g_last_cuda_error.store((int)se); return ALIGNN_ERR_CUDA; }
+  egc_forward_fused_kernel<D, EG><<<grid, F::THREADS, F::SMEM, (cudaStream_t)a.stream>>>(a, scr);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { g_last_cuda_error.store((int)e); return ALIGNN_ERR_CUDA; }
   return ALIGNN_OK;

@@ -1,18 +1,19 @@
 // Weight gradients of the Linear layers: C[g][o][i] = sum_r A[r, g*DA + o] * B[r, i], r over the rows
 // (edges or nodes) of the batch -- a DA x DB output with a very long reduction (K = 276 480 rows for the
-// edge gate on L(g)).  Tensor cores via tcgen05.mma kind::f16, bf16x3 split (tc_common.cuh).
+// edge gate on L(g)).  Tensor cores via wgmma (bf16 x bf16 -> fp32 in registers), bf16x3 split (tc_common.cuh).
 //
 // Both operands are "MN-major" for this product (the contraction index is the ROW of the row-major
 // activations), so the loader threads convert fp32 -> bf16 hi/lo and store the canonical MN-major
-// SWIZZLE_NONE UMMA layout:  addr(mn, k) = (mn/8)*SBO + (k/8)*LBO + (k%8)*16 + (mn%8)*2,
+// SWIZZLE_NONE GMMA layout:  addr(mn, k) = (mn/8)*SBO + (k/8)*LBO + (k%8)*16 + (mn%8)*2,
 // SBO = 128 (next 8 channels), LBO = (rows_of_plane/8)*128 (next 8 rows of the contraction).
 //
-// Split-K: CTA c of group g reduces a contiguous slab of rows into a full D x D accumulator held in
-// TMEM (2 x 256 columns for D = 256), then writes its partial tile; a second kernel sums the partials
-// in a fixed order (deterministic, no float atomics).  Each input element is read from HBM exactly
-// once, which is the bound: the kernel moves 2*K*D*4 bytes.
+// Output tiles: a CTA owns a 128 x TN block of the DA x DB output (TN = min(DB, 128)), held in the registers of two
+// consumer warpgroups (rows 0-63 / 64-127, TN / 2 floats per thread); DA = 256 or DB = 256 take 2 or 4 CTAs per row
+// slab, each reading only its channels.  Split-K: CTA c of group g reduces a contiguous slab of rows into its block
+// and writes it into a partial tile; the partials are then summed in a fixed order (deterministic, no float atomics).
 #include <cooperative_groups.h>
 
+#include "common.cuh"
 #include "tc_common.cuh"
 #include "api_common.h"
 #include "alignn_b200.h"
@@ -20,72 +21,52 @@
 namespace alignn {
 namespace wgrad {
 
-constexpr int BK = 32;          // contraction rows per stage (2 UMMA K=16 steps)
-constexpr int STAGES = 3;
+constexpr int BK = 32;          // contraction rows per stage (2 MMA K=16 steps)
+constexpr int STAGES = 4;
 constexpr int LOAD_WARPS = 8;
-constexpr int LOADERS = LOAD_WARPS * 32;
-constexpr int THREADS = LOADERS + 32;
+constexpr int MMA_WARPS = 8;    // two consumer warpgroups
+constexpr int THREADS = 32 * (MMA_WARPS + LOAD_WARPS);
 constexpr uint32_t SBO = 128;
-constexpr int kNumSMsWgrad = 148;
+constexpr int kNumSMsWgrad = kNumSMs;
+// Contraction rows a wgmma accumulator sums before it is added into the fp32 running sum in shared memory: the tensor
+// core's own accumulation over the thousands of rows of one slab loses more than the 2e-5 budget allows.
+constexpr int PROMOTE_CHUNKS = 8;
 
-template <int DA, int DB>   // A: [K, groups*DA] (output-gradient side), B: [K, DB] (input side); out tile DA x DB
+__host__ __device__ constexpr int tiles_of(int DA, int DB) { return (DA > 128 ? DA / 128 : 1) * (DB > 128 ? DB / 128 : 1); }
+
+template <int DA, int DB>   // A: [K, groups*DA] (output-gradient side), B: [K, DB] (input side); out DA x DB
 struct Cfg {
-  static constexpr int MT = (DA + 127) / 128;         // number of M=128 UMMA tiles
-  static constexpr int A_ROWS = MT * 128;             // padded channel count of the A plane
-  static constexpr int A_PLANE = A_ROWS * BK * 2;
-  static constexpr int B_PLANE = DB * BK * 2;
-  static constexpr uint32_t LBO_A = (A_ROWS / 8) * 128;
-  static constexpr uint32_t LBO_B = (DB / 8) * 128;
+  static constexpr int TA = DA < 128 ? DA : 128;      // A channels of one CTA's block (plane padded to 128 rows)
+  static constexpr int TN = DB <= 128 ? DB : 128;     // B channels of one CTA's block
+  static constexpr int NT = DB / TN;
+  static constexpr int TILES = tiles_of(DA, DB);
+  static constexpr int A_PLANE = 128 * BK * 2;
+  static constexpr int B_PLANE = TN * BK * 2;
+  static constexpr uint32_t LBO_A = (128 / 8) * 128;
+  static constexpr uint32_t LBO_B = (TN / 8) * 128;
   static constexpr int STAGE = 2 * A_PLANE + 2 * B_PLANE;
   static constexpr int PIPE = STAGES * STAGE;
-  static constexpr int SMEM = PIPE + 128;
-  static constexpr int ACC_COLS = MT * DB;
-  static constexpr int TMEM_COLS = ACC_COLS <= 32 ? 32 : ACC_COLS <= 64 ? 64 : ACC_COLS <= 128 ? 128 : ACC_COLS <= 256 ? 256 : 512;
-  static constexpr int TASKS_A = 4 * (DA / 16);       // (8-row group, 16-channel group) tasks per stage
-  static constexpr int TASKS = TASKS_A + 4 * (DB / 16);
+  static constexpr int ACC = MMA_WARPS * 32 * (TN / 2) * 4;   // running sums, one column per consumer thread
+  static constexpr int SMEM = PIPE + ACC + 128;
+  static_assert(TILES * TA * TN == DA * DB, "output blocks cover the output");
 };
 
+// The pipeline of one CTA over consecutive chunks of contraction rows, shared by the single-problem and the batch
+// kernels: loader warps fill the stage ring, the consumer warpgroups accumulate; the caller brackets it.
 template <int DA, int DB>
-__global__ void __launch_bounds__(THREADS, 1)
-wgrad_bf16x3_kernel(const float* __restrict__ A, int64_t lda, const float* __restrict__ B, int64_t ldb, int64_t K,
-                    int rows_per_cta, float* __restrict__ partials, float* __restrict__ out, int64_t ld_out) {
+struct Pipe {
   using F = Cfg<DA, DB>;
-  extern __shared__ __align__(128) uint8_t smem[];
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + F::PIPE);
-  uint64_t* empty = full + STAGES;
-  uint64_t* accbar = empty + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accbar + 1);
+  uint8_t* smem;
+  uint64_t* full;
+  uint64_t* empty;
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int cta = blockIdx.x, group = blockIdx.y;
-  const int64_t r_begin = (int64_t)cta * rows_per_cta;
-  const int64_t r_end = (r_begin + rows_per_cta < K) ? r_begin + rows_per_cta : K;
-  const int nk = r_end > r_begin ? (int)((r_end - r_begin + BK - 1) / BK) : 0;
-  const float* Ag = A + (int64_t)group * DA;
-
-  if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full[s], LOAD_WARPS); tc::mbar_init(&empty[s], 1); }
-    tc::mbar_init(accbar, 1);
-    tc::mbar_fence_init();
-  }
-  if (DA < 128) {   // padded A rows [DA, 128) are never written by the loaders: zero the planes once
-    for (int i = tid; i < F::PIPE / 16; i += THREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
-  }
-  if (warp == LOAD_WARPS) tc::tmem_alloc(tmem_slot, F::TMEM_COLS);
-  tc::fence_async_smem();
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
-
-  if (warp < LOAD_WARPS) {
-    // ================= loader / converter =================
-    // Work split with compile-time structure: slot (mat, eg, j) of warp w covers the 16-channel group
-    // og = w + 8*j of 8-row group eg of matrix mat -- only og depends on the warp, so no index math is left
-    // in the hot loop (a flat task id cost register spills and ~2x the time).
-    // half-warp = 8 contraction rows x 2 adjacent float4 -> one 128-byte core matrix: conflict-free 64-bit stores
+  // loader warps: rows [r_begin, r_end) of A (channels a0 .. a0 + TA) and B (channels b0 .. b0 + TN), chunks numbered
+  // from g0 in the ring.  Work split with compile-time structure: slot (eg, j) of warp w covers the 16-channel group
+  // og = w + 8*j of 8-row group eg; a half-warp = 8 contraction rows x 2 adjacent float4 -> one 128-byte core matrix.
+  __device__ __forceinline__ void load(const float* __restrict__ Ag, int64_t lda, const float* __restrict__ Bg, int64_t ldb,
+                                       int64_t r_begin, int64_t r_end, int nk, int g0, int warp, int lane) {
     const int e_l = (lane >> 1) & 7, oq = (lane >> 4) * 2 + (lane & 1);
-    constexpr int JA = (DA / 16 + LOAD_WARPS - 1) / LOAD_WARPS, JB = (DB / 16 + LOAD_WARPS - 1) / LOAD_WARPS;
+    constexpr int JA = (F::TA / 16 + LOAD_WARPS - 1) / LOAD_WARPS, JB = (F::TN / 16 + LOAD_WARPS - 1) / LOAD_WARPS;
     constexpr int NT = 4 * (JA + JB);
     auto load_chunk = [&](float4 (&v)[NT], int kc) {
       const int64_t r0 = r_begin + (int64_t)kc * BK + e_l;
@@ -96,20 +77,20 @@ wgrad_bf16x3_kernel(const float* __restrict__ A, int64_t lda, const float* __res
 #pragma unroll
         for (int j = 0; j < JA; ++j) {
           const int og = warp + LOAD_WARPS * j;
-          v[eg * (JA + JB) + j] = (rv && og < DA / 16) ? __ldcs(reinterpret_cast<const float4*>(Ag + r * lda + (og * 4 + oq) * 4))
-                                                      : make_float4(0.f, 0.f, 0.f, 0.f);
+          v[eg * (JA + JB) + j] = (rv && og < F::TA / 16) ? __ldcs(reinterpret_cast<const float4*>(Ag + r * lda + (og * 4 + oq) * 4))
+                                                          : make_float4(0.f, 0.f, 0.f, 0.f);
         }
 #pragma unroll
         for (int j = 0; j < JB; ++j) {
           const int og = warp + LOAD_WARPS * j;
-          v[eg * (JA + JB) + JA + j] = (rv && og < DB / 16) ? __ldcs(reinterpret_cast<const float4*>(B + r * ldb + (og * 4 + oq) * 4))
-                                                           : make_float4(0.f, 0.f, 0.f, 0.f);
+          v[eg * (JA + JB) + JA + j] = (rv && og < F::TN / 16) ? __ldcs(reinterpret_cast<const float4*>(Bg + r * ldb + (og * 4 + oq) * 4))
+                                                               : make_float4(0.f, 0.f, 0.f, 0.f);
         }
       }
     };
-    auto store_chunk = [&](const float4 (&v)[NT], int kc) {
-      const int s = kc % STAGES;
-      if (kc >= STAGES) tc::mbar_wait(&empty[s], ((kc / STAGES) - 1) & 1);
+    auto store_chunk = [&](const float4 (&v)[NT], int gc) {
+      const int s = gc % STAGES;
+      if (gc >= STAGES) tc::mbar_wait(&empty[s], ((gc / STAGES) - 1) & 1);
       uint8_t* st = smem + s * F::STAGE;
 #pragma unroll
       for (int eg = 0; eg < 4; ++eg) {
@@ -118,7 +99,7 @@ wgrad_bf16x3_kernel(const float* __restrict__ A, int64_t lda, const float* __res
         for (int j = 0; j < JA + JB; ++j) {
           const bool isA = j < JA;
           const int og = warp + LOAD_WARPS * (isA ? j : j - JA);
-          if (og < (isA ? DA : DB) / 16) {
+          if (og < (isA ? F::TA : F::TN) / 16) {
             const int o4 = og * 4 + oq;
             uint2 hi, lo;
             tc::split4(v[eg * (JA + JB) + j], hi, lo);
@@ -140,83 +121,113 @@ wgrad_bf16x3_kernel(const float* __restrict__ A, int64_t lda, const float* __res
     if (nk > 0) load_chunk(b0, 0);
     for (int kc = 0; kc < nk; kc += 2) {
       if (kc + 1 < nk) load_chunk(b1, kc + 1);
-      store_chunk(b0, kc);
+      store_chunk(b0, g0 + kc);
       if (kc + 1 < nk) {
         if (kc + 2 < nk) load_chunk(b0, kc + 2);
-        store_chunk(b1, kc + 1);
+        store_chunk(b1, g0 + kc + 1);
       }
     }
-    // ================= epilogue: TMEM -> partial tile in global =================
-    tc::mbar_wait(accbar, 0);
-    tc::fence_after_sync();
-    float* out = partials + ((int64_t)group * gridDim.x + cta) * DA * DB;
-    const int q = warp & 3;                       // TMEM lane quarter this warp may read
-    const int row_in_tile = q * 32 + lane;
-    // DA = 256: warps 0-3 read M tile 0, warps 4-7 M tile 1.  One M tile and DB >= 128: the two warp quads
-    // split the columns.  Otherwise warps 0-3 read everything.
-    const int mt = (F::MT == 2) ? (warp >> 2) : 0;
-    const bool halves = (F::MT == 1) && (DB >= 128);
-    const int c_begin = halves ? (warp >> 2) * (DB / 2) : 0;
-    const int c_end = (F::MT == 2) ? DB : (halves ? c_begin + DB / 2 : ((warp >> 2) == 0 ? DB : 0));
-    const int o = mt * 128 + row_in_tile;
-    // Partial tiles are a private workspace, stored BLOCKED: element (o, c) at ((c / 32) * DA + o) * 32 + c % 32, so that
-    // the row-per-thread accumulator fragments leave as 128 contiguous bytes per lane and 4 KB per warp instruction
-    // (row-major would scatter every store over 32 lines).  The reduction below un-blocks.
-    if (nk > 0) {
-      for (int c0 = c_begin; c0 < c_end; c0 += 32) {
-        float v[32];
-        tc::tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(mt * DB + c0), v);
-        if (o < DA) {
-          float* dst = out + ((int64_t)(c0 >> 5) * DA + o) * 32;
+  }
+
+  // consumer warpgroup wg: acc = its 64 rows of the block summed over nk chunks numbered from g0
+  __device__ __forceinline__ void mma(float (&acc)[F::TN / 2], int nk, int g0, int wg, int lane) {
+    const uint32_t base0 = tc::smem_u32(smem);
+    float* run = reinterpret_cast<float*>(smem + F::PIPE) + wg * 128 + (threadIdx.x & 127);
 #pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            *reinterpret_cast<float4*>(dst + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-        }
-      }
-    } else if (o < DA) {
-      for (int c0 = c_begin; c0 < c_end; c0 += 4)
-        *reinterpret_cast<float4*>(out + ((int64_t)(c0 >> 5) * DA + o) * 32 + (c0 & 31)) = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-  } else if (lane == 0) {
-    // ================= MMA issuer =================
-    constexpr uint32_t IDESC = tc::idesc_bf16_f32(128, DB) | (1u << 15) | (1u << 16);   // A and B MN-major
+    for (int i = 0; i < F::TN / 2; ++i) { run[i * MMA_WARPS * 32] = 0.f; acc[i] = 0.f; }
     for (int kc = 0; kc < nk; ++kc) {
-      const int s = kc % STAGES;
-      tc::mbar_wait(&full[s], (kc / STAGES) & 1);
-      tc::fence_after_sync();
-      const uint32_t base = tc::smem_u32(smem + s * F::STAGE);
+      const int g = g0 + kc, s = g % STAGES;
+      tc::mbar_wait(&full[s], (g / STAGES) & 1);
+      const uint32_t base = base0 + s * F::STAGE;
+      tc::wgmma_fence();
 #pragma unroll
       for (int j = 0; j < BK / 16; ++j) {
         const uint64_t b_hi = tc::smem_desc(base + 2 * F::A_PLANE + j * 2 * F::LBO_B, F::LBO_B, SBO);
         const uint64_t b_lo = tc::smem_desc(base + 2 * F::A_PLANE + F::B_PLANE + j * 2 * F::LBO_B, F::LBO_B, SBO);
-#pragma unroll
-        for (int mt = 0; mt < F::MT; ++mt) {
-          const uint32_t ao = j * 2 * F::LBO_A + mt * 16 * SBO;
-          const uint64_t a_hi = tc::smem_desc(base + ao, F::LBO_A, SBO);
-          const uint64_t a_lo = tc::smem_desc(base + F::A_PLANE + ao, F::LBO_A, SBO);
-          const uint32_t d = tmem + (uint32_t)(mt * DB);
-          tc::mma_bf16_ss(d, a_lo, b_hi, IDESC, (kc | j) != 0);
-          tc::mma_bf16_ss(d, a_hi, b_lo, IDESC, 1);
-          tc::mma_bf16_ss(d, a_hi, b_hi, IDESC, 1);
-        }
+        const uint32_t ao = j * 2 * F::LBO_A + wg * 8 * SBO;
+        const uint64_t a_hi = tc::smem_desc(base + ao, F::LBO_A, SBO);
+        const uint64_t a_lo = tc::smem_desc(base + F::A_PLANE + ao, F::LBO_A, SBO);
+        tc::Wgmma<F::TN>::template mma<1, 1>(acc, a_lo, b_hi, 1);
+        tc::Wgmma<F::TN>::template mma<1, 1>(acc, a_hi, b_lo, 1);
+        tc::Wgmma<F::TN>::template mma<1, 1>(acc, a_hi, b_hi, 1);
       }
-      tc::mma_commit(&empty[s]);
+      tc::wgmma_commit();
+      tc::wgmma_wait_all();
+      __syncwarp();
+      if (lane == 0) tc::mbar_arrive(&empty[s]);
+      if ((kc + 1) % PROMOTE_CHUNKS == 0 || kc + 1 == nk) {
+#pragma unroll
+        for (int i = 0; i < F::TN / 2; ++i) { run[i * MMA_WARPS * 32] += acc[i]; acc[i] = 0.f; }
+      }
     }
-    tc::mma_commit(accbar);
+#pragma unroll
+    for (int i = 0; i < F::TN / 2; ++i) acc[i] = run[i * MMA_WARPS * 32];
   }
-  tc::fence_before_sync();
+
+  // Partial tiles are a private workspace, stored BLOCKED: element (o, c) at ((c / 32) * DA + o) * 32 + c % 32; the
+  // reduction un-blocks.  Block (mt, nt) of the output, consumer thread (warp, lane).
+  __device__ __forceinline__ static void store(const float (&acc)[F::TN / 2], float* out, int mt, int nt, int warp, int lane) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+      if (r >= F::TA) continue;
+      const int o = mt * F::TA + r;
+#pragma unroll
+      for (int j = 0; j < F::TN / 8; ++j) {
+        const int c = nt * F::TN + 8 * j + 2 * (lane & 3);
+        *reinterpret_cast<float2*>(out + ((int64_t)(c >> 5) * DA + o) * 32 + (c & 31)) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+      }
+    }
+  }
+};
+
+template <int DA, int DB>
+__device__ __forceinline__ void pipe_init(uint8_t* smem, uint64_t* full, uint64_t* empty) {
+  using F = Cfg<DA, DB>;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full[s], LOAD_WARPS); tc::mbar_init(&empty[s], MMA_WARPS); }
+    tc::mbar_fence_init();
+  }
+  if (F::TA < 128) {   // padded A rows [TA, 128) are never written by the loaders: zero the planes once
+    for (int i = threadIdx.x; i < F::PIPE / 16; i += THREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
+  }
+  tc::fence_async_smem();
   __syncthreads();
-  if (warp == LOAD_WARPS) tc::tmem_dealloc(tmem, F::TMEM_COLS);
+}
+
+// grid (ctas, groups, TILES): CTA (c, g, t) reduces rows [c * rows_per_cta, ...) of group g into output block t
+template <int DA, int DB>
+__global__ void __launch_bounds__(THREADS, 1)
+wgrad_bf16x3_kernel(const float* __restrict__ A, int64_t lda, const float* __restrict__ B, int64_t ldb, int64_t K,
+                    int rows_per_cta, float* __restrict__ partials, float* __restrict__ out, int64_t ld_out) {
+  using F = Cfg<DA, DB>;
+  extern __shared__ __align__(128) uint8_t smem[];
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + F::PIPE + F::ACC);
+  Pipe<DA, DB> pipe{smem, full, full + STAGES};
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int cta = blockIdx.x, group = blockIdx.y, mt = blockIdx.z / F::NT, nt = blockIdx.z % F::NT;
+  const int64_t r_begin = (int64_t)cta * rows_per_cta;
+  const int64_t r_end = (r_begin + rows_per_cta < K) ? r_begin + rows_per_cta : K;
+  const int nk = r_end > r_begin ? (int)((r_end - r_begin + BK - 1) / BK) : 0;
+  pipe_init<DA, DB>(smem, full, full + STAGES);
+
+  if (warp >= MMA_WARPS) {
+    pipe.load(A + (int64_t)group * DA + mt * F::TA, lda, B + nt * F::TN, ldb, r_begin, r_end, nk, 0, warp - MMA_WARPS, lane);
+  } else {
+    float acc[F::TN / 2];
+    pipe.mma(acc, nk, 0, warp >> 2, lane);
+    Pipe<DA, DB>::store(acc, partials + ((int64_t)group * gridDim.x + cta) * DA * DB, mt, nt, warp, lane);
+  }
   if (out) {
     // Split-K reduction inside the kernel (cooperative launch: every CTA is resident): once all partial tiles are
-    // written, CTA c of a group sums its slice of the DA x DB output over the group's partials in a fixed order.
-    // Replaces a second launch that spent ~15 us walking the partials with 64 CTAs.
+    // written, the CTAs of a group sum slices of the DA x DB output over the group's partials in a fixed order.
     __threadfence();
     cooperative_groups::this_grid().sync();
     const int ctas = gridDim.x;
+    const int64_t rank = (int64_t)blockIdx.z * gridDim.x + cta, parts = (int64_t)gridDim.z * gridDim.x;
     constexpr int64_t tile = (int64_t)DA * DB;
     const float* p = partials + (int64_t)group * ctas * tile;
-    for (int64_t idx = ((int64_t)cta * THREADS + tid) * 4; idx < tile; idx += (int64_t)ctas * THREADS * 4) {
+    for (int64_t idx = (rank * THREADS + tid) * 4; idx < tile; idx += parts * THREADS * 4) {
       // 16 partials per batch: the loads of a batch are independent (latency paid once per batch), the adds keep one
       // fixed order
       float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -241,10 +252,11 @@ wgrad_bf16x3_kernel(const float* __restrict__ A, int64_t lda, const float* __res
 // ---- many weight gradients in ONE launch ---------------------------------------------------------------------------
 // A training step of the 4+4 stack needs 24 square weight gradients (4 with K = T bond pairs, 12 with K = E bonds, 8 x 4
 // with K = N atoms); none of them is on the critical path of the backward pass, and launched one by one the small ones
-// cost ~30 us each for ~5 us of traffic (prologue, TMEM allocation, one partial tile per CTA, grid barrier).  The batch
-// kernel takes all of them as a list of problems, cuts the concatenated rows into slabs of equal cost, one sequence of
-// slabs per CTA, and runs the same loader / MMA / epilogue pipeline slab after slab; every slab leaves one partial tile,
-// and after the grid barrier all CTAs sum each problem's partial tiles in slab order (fixed order: deterministic).
+// cost a prologue, one partial tile per CTA and a grid barrier each.  The batch kernel takes all of them as a list of
+// problems, cuts the concatenated rows into slabs of equal cost, one sequence of slabs per CTA column (blockIdx.x; the
+// TILES CTAs of a column, blockIdx.y, own the output blocks), and runs the same loader / MMA / store pipeline slab after
+// slab; every slab leaves one partial tile, and after the grid barrier all CTAs sum each problem's partial tiles in slab
+// order (fixed order: deterministic).
 constexpr int kMaxProblems = 64;
 constexpr int kMaxSlabs = 320;
 
@@ -257,7 +269,7 @@ struct Slab { int prob, chunk_begin, chunks; };     // rows [chunk_begin*BK, min
 struct Batch {
   Problem prob[kMaxProblems];
   Slab slab[kMaxSlabs];
-  int cta_first[kNumSMsWgrad + 1];                  // CTA c runs slabs [cta_first[c], cta_first[c+1])
+  int cta_first[kNumSMsWgrad + 1];                  // CTA column c runs slabs [cta_first[c], cta_first[c+1])
   int nprob;
 };
 
@@ -266,165 +278,37 @@ __global__ void __launch_bounds__(THREADS, 1)
 wgrad_batch_kernel(const __grid_constant__ Batch bt, float* __restrict__ partials) {
   using F = Cfg<DA, DB>;
   extern __shared__ __align__(128) uint8_t smem[];
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + F::PIPE);
-  uint64_t* empty = full + STAGES;
-  uint64_t* accbar = empty + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accbar + 1);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + F::PIPE + F::ACC);
+  Pipe<DA, DB> pipe{smem, full, full + STAGES};
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int cta = blockIdx.x;
+  const int cta = blockIdx.x, mt = blockIdx.y / F::NT, nt = blockIdx.y % F::NT;
   const int s_first = bt.cta_first[cta], s_last = bt.cta_first[cta + 1];
+  pipe_init<DA, DB>(smem, full, full + STAGES);
 
-  if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full[s], LOAD_WARPS); tc::mbar_init(&empty[s], 1); }
-    tc::mbar_init(accbar, 1);
-    tc::mbar_fence_init();
-  }
-  if (DA < 128) {
-    for (int i = tid; i < F::PIPE / 16; i += THREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
-  }
-  if (warp == LOAD_WARPS) tc::tmem_alloc(tmem_slot, F::TMEM_COLS);
-  tc::fence_async_smem();
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
-
-  if (warp < LOAD_WARPS) {
-    const int e_l = (lane >> 1) & 7, oq = (lane >> 4) * 2 + (lane & 1);
-    constexpr int JA = (DA / 16 + LOAD_WARPS - 1) / LOAD_WARPS, JB = (DB / 16 + LOAD_WARPS - 1) / LOAD_WARPS;
-    constexpr int NT = 4 * (JA + JB);
-    int g = 0;                                     // chunks this CTA has pushed through the stage ring so far
-    for (int si = s_first; si < s_last; ++si) {
-      const Slab sl = bt.slab[si];
-      const Problem& pr = bt.prob[sl.prob];
-      const float* __restrict__ Ag = pr.A;
-      const float* __restrict__ Bg = pr.B;
-      const int64_t lda = pr.lda, ldb = pr.ldb;
+  int g = 0;                                     // chunks this CTA has pushed through the stage ring so far
+  for (int si = s_first; si < s_last; ++si) {
+    const Slab sl = bt.slab[si];
+    const Problem& pr = bt.prob[sl.prob];
+    const int nk = sl.chunks;
+    if (warp >= MMA_WARPS) {
       const int64_t r_begin = (int64_t)sl.chunk_begin * BK;
       const int64_t r_end = (r_begin + (int64_t)sl.chunks * BK < pr.K) ? r_begin + (int64_t)sl.chunks * BK : pr.K;
-      const int nk = sl.chunks;
-      auto load_chunk = [&](float4 (&v)[NT], int kc) {
-        const int64_t r0 = r_begin + (int64_t)kc * BK + e_l;
-#pragma unroll
-        for (int eg = 0; eg < 4; ++eg) {
-          const int64_t r = r0 + eg * 8;
-          const bool rv = r < r_end;
-#pragma unroll
-          for (int j = 0; j < JA; ++j) {
-            const int og = warp + LOAD_WARPS * j;
-            v[eg * (JA + JB) + j] = (rv && og < DA / 16) ? __ldcs(reinterpret_cast<const float4*>(Ag + r * lda + (og * 4 + oq) * 4))
-                                                        : make_float4(0.f, 0.f, 0.f, 0.f);
-          }
-#pragma unroll
-          for (int j = 0; j < JB; ++j) {
-            const int og = warp + LOAD_WARPS * j;
-            v[eg * (JA + JB) + JA + j] = (rv && og < DB / 16) ? __ldcs(reinterpret_cast<const float4*>(Bg + r * ldb + (og * 4 + oq) * 4))
-                                                             : make_float4(0.f, 0.f, 0.f, 0.f);
-          }
-        }
-      };
-      auto store_chunk = [&](const float4 (&v)[NT], int gc) {
-        const int s = gc % STAGES;
-        if (gc >= STAGES) tc::mbar_wait(&empty[s], ((gc / STAGES) - 1) & 1);
-        uint8_t* st = smem + s * F::STAGE;
-#pragma unroll
-        for (int eg = 0; eg < 4; ++eg) {
-          const int edge = eg * 8 + e_l;
-#pragma unroll
-          for (int j = 0; j < JA + JB; ++j) {
-            const bool isA = j < JA;
-            const int og = warp + LOAD_WARPS * (isA ? j : j - JA);
-            if (og < (isA ? DA : DB) / 16) {
-              const int o4 = og * 4 + oq;
-              uint2 hi, lo;
-              tc::split4(v[eg * (JA + JB) + j], hi, lo);
-              const int lbo = isA ? (int)F::LBO_A : (int)F::LBO_B;
-              const int plane = isA ? F::A_PLANE : F::B_PLANE;
-              uint8_t* base = st + (isA ? 0 : 2 * F::A_PLANE);
-              const int off = (o4 >> 1) * (int)SBO + (edge >> 3) * lbo + (edge & 7) * 16 + (o4 & 1) * 8;
-              *reinterpret_cast<uint2*>(base + off) = hi;
-              *reinterpret_cast<uint2*>(base + plane + off) = lo;
-            }
-          }
-        }
-        tc::fence_async_smem();
-        __syncwarp();
-        if (lane == 0) tc::mbar_arrive(&full[s]);
-      };
-      float4 b0[NT], b1[NT];
-      load_chunk(b0, 0);
-      for (int kc = 0; kc < nk; kc += 2) {
-        if (kc + 1 < nk) load_chunk(b1, kc + 1);
-        store_chunk(b0, g + kc);
-        if (kc + 1 < nk) {
-          if (kc + 2 < nk) load_chunk(b0, kc + 2);
-          store_chunk(b1, g + kc + 1);
-        }
-      }
-      g += nk;
-      // ---- slab epilogue: TMEM -> this slab's partial tile (blocked layout, see wgrad_bf16x3_kernel) ----
-      tc::mbar_wait(accbar, (si - s_first) & 1);
-      tc::fence_after_sync();
-      float* out = partials + (int64_t)si * DA * DB;
-      const int q = warp & 3;
-      const int row_in_tile = q * 32 + lane;
-      const int mt = (F::MT == 2) ? (warp >> 2) : 0;
-      const bool halves = (F::MT == 1) && (DB >= 128);
-      const int c_begin = halves ? (warp >> 2) * (DB / 2) : 0;
-      const int c_end = (F::MT == 2) ? DB : (halves ? c_begin + DB / 2 : ((warp >> 2) == 0 ? DB : 0));
-      const int o = mt * 128 + row_in_tile;
-      for (int c0 = c_begin; c0 < c_end; c0 += 32) {
-        float v[32];
-        tc::tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(mt * DB + c0), v);
-        if (o < DA) {
-          float* dst = out + ((int64_t)(c0 >> 5) * DA + o) * 32;
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            *reinterpret_cast<float4*>(dst + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-        }
-      }
-      tc::fence_before_sync();      // the accumulator is overwritten by the next slab only after these reads (ordered through `full`)
+      pipe.load(pr.A + mt * F::TA, pr.lda, pr.B + nt * F::TN, pr.ldb, r_begin, r_end, nk, g, warp - MMA_WARPS, lane);
+    } else {
+      float acc[F::TN / 2];
+      pipe.mma(acc, nk, g, warp >> 2, lane);
+      Pipe<DA, DB>::store(acc, partials + (int64_t)si * DA * DB, mt, nt, warp, lane);
     }
-  } else if (lane == 0) {
-    constexpr uint32_t IDESC = tc::idesc_bf16_f32(128, DB) | (1u << 15) | (1u << 16);
-    int g = 0;
-    for (int si = s_first; si < s_last; ++si) {
-      const int nk = bt.slab[si].chunks;
-      for (int kc = 0; kc < nk; ++kc, ++g) {
-        const int s = g % STAGES;
-        tc::mbar_wait(&full[s], (g / STAGES) & 1);
-        tc::fence_after_sync();
-        const uint32_t base = tc::smem_u32(smem + s * F::STAGE);
-#pragma unroll
-        for (int j = 0; j < BK / 16; ++j) {
-          const uint64_t b_hi = tc::smem_desc(base + 2 * F::A_PLANE + j * 2 * F::LBO_B, F::LBO_B, SBO);
-          const uint64_t b_lo = tc::smem_desc(base + 2 * F::A_PLANE + F::B_PLANE + j * 2 * F::LBO_B, F::LBO_B, SBO);
-#pragma unroll
-          for (int mt = 0; mt < F::MT; ++mt) {
-            const uint32_t ao = j * 2 * F::LBO_A + mt * 16 * SBO;
-            const uint64_t a_hi = tc::smem_desc(base + ao, F::LBO_A, SBO);
-            const uint64_t a_lo = tc::smem_desc(base + F::A_PLANE + ao, F::LBO_A, SBO);
-            const uint32_t d = tmem + (uint32_t)(mt * DB);
-            tc::mma_bf16_ss(d, a_lo, b_hi, IDESC, (kc | j) != 0);
-            tc::mma_bf16_ss(d, a_hi, b_lo, IDESC, 1);
-            tc::mma_bf16_ss(d, a_hi, b_hi, IDESC, 1);
-          }
-        }
-        tc::mma_commit(&empty[s]);
-      }
-      tc::mma_commit(accbar);
-    }
+    g += nk;
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == LOAD_WARPS) tc::tmem_dealloc(tmem, F::TMEM_COLS);
   // ---- all partial tiles are written: every CTA sums a share of every problem's output, slabs in order ----
   __threadfence();
   cooperative_groups::this_grid().sync();
   constexpr int64_t tile = (int64_t)DA * DB;
   constexpr int64_t tile4 = tile / 4;
   const int64_t items = (int64_t)bt.nprob * tile4;
-  for (int64_t it = (int64_t)cta * THREADS + tid; it < items; it += (int64_t)gridDim.x * THREADS) {
+  const int64_t rank = (int64_t)blockIdx.y * gridDim.x + cta, parts = (int64_t)gridDim.y * gridDim.x;
+  for (int64_t it = rank * THREADS + tid; it < items; it += parts * THREADS) {
     const int pi = (int)(it / tile4);
     const int64_t idx = (it - (int64_t)pi * tile4) * 4;
     const Problem& pr = bt.prob[pi];
@@ -450,11 +334,12 @@ wgrad_batch_kernel(const __grid_constant__ Batch bt, float* __restrict__ partial
 
 // Cut the problems into slabs: every CTA gets about the same cost, cost(slab) = its chunks + kSlabCost (the fixed price
 // of a slab: accumulator drain and a DA x DB partial tile to write and re-read, about the time of 6 chunks of rows).
-// The per-CTA budget starts at total / 148 and grows until the cut fits 148 CTAs (a problem cut in two pays the slab
-// price twice, so the first guess can be short).  Returns the number of slabs, or -1 if the batch does not fit the
+// The per-CTA budget starts at total / ctas and grows until the cut fits `ctas` CTA columns (kNumSMs / TILES: every
+// column is TILES CTAs, one per output block; a problem cut in two pays the slab price twice, so the first guess can be
+// short).  Returns the number of slabs, or -1 if the batch does not fit the
 // tables (the caller then splits the batch).
 constexpr int kSlabCost = 6;
-inline int cut_batch(const int64_t* K, int n, int64_t target, Batch* bt) {
+inline int cut_batch(const int64_t* K, int n, int64_t target, int ctas, Batch* bt) {
   int ns = 0, cta = 0;
   int64_t budget = target;
   if (bt) bt->cta_first[0] = 0;
@@ -463,7 +348,7 @@ inline int cut_batch(const int64_t* K, int n, int64_t target, Batch* bt) {
     const int first = ns;
     while (left > 0) {
       if (budget <= kSlabCost + 2) {                                  // not worth a slab here: next CTA
-        if (++cta >= kNumSMsWgrad) return -2;                         // budget too small for 148 CTAs
+        if (++cta >= ctas) return -2;                                  // budget too small for the CTAs
         budget = target;
         if (bt) bt->cta_first[cta] = ns;
       }
@@ -482,19 +367,19 @@ inline int cut_batch(const int64_t* K, int n, int64_t target, Batch* bt) {
   }
   return ns;
 }
-inline int plan_batch(const int64_t* K, int n, Batch* bt) {
+inline int plan_batch(const int64_t* K, int n, int ctas, Batch* bt) {
   if (n < 1 || n > kMaxProblems) return -1;
   int64_t total = 0;
   for (int p = 0; p < n; ++p) total += (K[p] + BK - 1) / BK + kSlabCost;
-  int64_t target = (total + kNumSMsWgrad - 1) / kNumSMsWgrad;
+  int64_t target = (total + ctas - 1) / ctas;
   if (target < 8 * kSlabCost) target = 8 * kSlabCost;                 // never spread a small batch thinner than this
   for (;;) {
-    const int ns = cut_batch(K, n, target, nullptr);
+    const int ns = cut_batch(K, n, target, ctas, nullptr);
     if (ns == -1) return -1;
     if (ns >= 0) break;
     target += (target + 31) / 32;                                     // +3 % and try again
   }
-  return cut_batch(K, n, target, bt);
+  return cut_batch(K, n, target, ctas, bt);
 }
 
 // out[g*DA + o][i] = sum_c partials[g][c][o][i]  (fixed order)
@@ -513,11 +398,11 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ partials, int ctas
   *reinterpret_cast<float4*>(out + ((int64_t)g * DA + o) * ld_out + i) = s;
 }
 
-inline int ctas_for(int64_t K, int groups) {
-  int per_group = kNumSMsWgrad / groups;
+inline int ctas_for(int64_t K, int groups, int tiles) {
+  int per_group = kNumSMsWgrad / (groups * tiles);
   if (per_group < 1) per_group = 1;
   const int64_t chunks = (K + BK - 1) / BK;
-  // every CTA writes (and the reduction re-reads) a full DA x DB partial tile -- 256 KB at D = 256 -- so a short
+  // every CTA column writes (and the reduction re-reads) a full DA x DB partial tile -- 256 KB at D = 256 -- so a short
   // reduction is not spread thinner than 4 pipeline chunks (128 rows) per CTA.
   const int64_t want = (chunks + 3) / 4;
   if (want < per_group) per_group = (int)(want < 1 ? 1 : want);
@@ -534,11 +419,11 @@ int launch(const float* A, int64_t lda, const float* B, int64_t ldb, int64_t K, 
     if (e != cudaSuccess) return record_cuda_error((int)e);
     configured.done(cfg_dev);
   }
-  const int ctas = ctas_for(K, groups);
+  const int ctas = ctas_for(K, groups, F::TILES);
   int64_t rows = (K + ctas - 1) / ctas;
   rows = (rows + BK - 1) / BK * BK;               // slabs start on a stage boundary
-  // cooperative launch: ctas * groups <= 148 CTAs of one per SM, so the in-kernel grid barrier before the split-K
-  // reduction is legal; if the device cannot co-schedule them (MPS slice, smaller part) fall back to two launches
+  // cooperative launch: ctas * groups * TILES <= kNumSMs CTAs of one per SM, so the in-kernel grid barrier before the
+  // split-K reduction is legal; if the device cannot co-schedule them (MPS slice, smaller part) fall back to two launches
   static int coop_ok = -1;
   if (coop_ok < 0) {
     int dev = 0, sms = 0, per_sm = 0, coop = 0;
@@ -552,12 +437,12 @@ int launch(const float* A, int64_t lda, const float* B, int64_t ldb, int64_t K, 
   if (coop_ok) {
     float* ws_p = ws;
     void* args[] = {(void*)&A, (void*)&lda, (void*)&B, (void*)&ldb, (void*)&K, (void*)&rows_i, (void*)&ws_p, (void*)&out, (void*)&ld_out};
-    cudaError_t e = cudaLaunchCooperativeKernel((const void*)wgrad_bf16x3_kernel<DA, DB>, dim3(ctas, groups), dim3(THREADS), args,
+    cudaError_t e = cudaLaunchCooperativeKernel((const void*)wgrad_bf16x3_kernel<DA, DB>, dim3(ctas, groups, F::TILES), dim3(THREADS), args,
                                                 (size_t)F::SMEM, st);
     if (e != cudaSuccess) return record_cuda_error((int)e);
     return check_launch();
   }
-  wgrad_bf16x3_kernel<DA, DB><<<dim3(ctas, groups), THREADS, F::SMEM, st>>>(A, lda, B, ldb, K, rows_i, ws, nullptr, 0);
+  wgrad_bf16x3_kernel<DA, DB><<<dim3(ctas, groups, F::TILES), THREADS, F::SMEM, st>>>(A, lda, B, ldb, K, rows_i, ws, nullptr, 0);
   int rc = check_launch();
   if (rc != ALIGNN_OK) return rc;
   const int64_t tile = (int64_t)DA * DB;
@@ -568,7 +453,7 @@ int launch(const float* A, int64_t lda, const float* B, int64_t ldb, int64_t K, 
 // supported (DA, DB): square conv shapes and the embedding-MLP shapes (inputs zero-padded to a multiple of 32)
 inline bool shape_ok(int DA, int DB) {
   if (DA == DB) return DA == 32 || DA == 64 || DA == 128 || DA == 256;
-  return (DA == 256 && (DB == 64 || DB == 96)) || (DA == 64 && (DB == 96 || DB == 32)) || (DA == 32 && DB == 64);
+  return (DA == 256 && (DB == 64 || DB == 96)) || (DA == 64 && (DB == 96 || DB == 32)) || (DA == 32 && (DB == 64 || DB == 96));
 }
 
 }  // namespace wgrad
@@ -587,9 +472,9 @@ static int launch_batch(const alignn::wgrad::Batch& bt, float* ws, cudaStream_t 
     configured.done(cfg_dev);
   }
   void* args[] = {(void*)&bt, (void*)&ws};
-  cudaError_t e = cudaLaunchCooperativeKernel((const void*)wgrad_batch_kernel<D, D>, dim3(kNumSMsWgrad), dim3(THREADS), args,
+  cudaError_t e = cudaLaunchCooperativeKernel((const void*)wgrad_batch_kernel<D, D>, dim3(kNumSMsWgrad / F::TILES, F::TILES), dim3(THREADS), args,
                                               (size_t)F::SMEM, st);
-  if (e == cudaErrorCooperativeLaunchTooLarge) {     // the device cannot co-schedule 148 CTAs right now (MPS slice, ...)
+  if (e == cudaErrorCooperativeLaunchTooLarge) {     // the device cannot co-schedule the grid right now (MPS slice, ...)
     (void)cudaGetLastError();
     return kBatchNeedsFallback;
   }
@@ -601,7 +486,7 @@ extern "C" {
 
 size_t alignn_b200_wgrad_workspace_bytes(int64_t K, int DA, int DB, int groups) {
   if (K < 0 || groups < 1 || !alignn::wgrad::shape_ok(DA, DB)) return 0;
-  return (size_t)alignn::wgrad::ctas_for(K, groups) * groups * DA * DB * sizeof(float);
+  return (size_t)alignn::wgrad::ctas_for(K, groups, alignn::wgrad::tiles_of(DA, DB)) * groups * DA * DB * sizeof(float);
 }
 
 size_t alignn_b200_wgrad_batch_workspace_bytes(const alignn_b200_wgrad_problem* problems, int n, int D) {
@@ -609,7 +494,7 @@ size_t alignn_b200_wgrad_batch_workspace_bytes(const alignn_b200_wgrad_problem* 
   if (!problems || n < 1 || n > kMaxProblems || !shape_ok(D, D)) return 0;
   int64_t K[kMaxProblems];
   for (int p = 0; p < n; ++p) { if (problems[p].K < 0) return 0; K[p] = problems[p].K; }
-  const int ns = plan_batch(K, n, nullptr);
+  const int ns = plan_batch(K, n, kNumSMsWgrad / tiles_of(D, D), nullptr);
   return ns < 0 ? 0 : (size_t)(ns > 0 ? ns : 1) * D * D * sizeof(float);
 }
 
@@ -631,7 +516,7 @@ int alignn_b200_wgrad_batch(const alignn_b200_wgrad_problem* problems, int n, in
     bt.prob[p].A = q.A; bt.prob[p].B = q.B; bt.prob[p].out = q.out;
     bt.prob[p].lda = q.lda; bt.prob[p].ldb = q.ldb; bt.prob[p].ld_out = q.ld_out; bt.prob[p].K = q.K;
   }
-  const int ns = plan_batch(K, n, &bt);
+  const int ns = plan_batch(K, n, kNumSMsWgrad / tiles_of(D, D), &bt);
   if (ns < 0) return ALIGNN_ERR_BAD_ARG;
   if (!workspace || workspace_bytes < (size_t)(ns > 0 ? ns : 1) * D * D * sizeof(float)) return ALIGNN_ERR_WORKSPACE;
   static int coop_ok = -1;
@@ -680,7 +565,7 @@ int alignn_b200_wgrad(const float* A, int64_t lda, const float* B, int64_t ldb, 
   float* ws = reinterpret_cast<float*>(workspace);
 #define WG(a, b) if (DA == a && DB == b) return launch<a, b>(A, lda, B, ldb, K, groups, out, ld_out, ws, st)
   WG(256, 256); WG(128, 128); WG(64, 64); WG(32, 32);
-  WG(256, 64); WG(256, 96); WG(64, 96); WG(64, 32); WG(32, 64);
+  WG(256, 64); WG(256, 96); WG(64, 96); WG(64, 32); WG(32, 64); WG(32, 96);
 #undef WG
   return ALIGNN_ERR_UNSUPPORTED_D;
 }

@@ -202,9 +202,8 @@ class BNLink:
         return bn_backward_finish(part, self.n, self.rstd)
 
 
-# Measured on B200 (batch 64, d = 256): the data-gradient GEMM with the two extra reductions in its epilogue takes 535 us
-# instead of 225 us -- the epilogue of the tensor-core kernels is already the saturated agent (shared-memory / L1 pipe,
-# DESIGN.md section 4) -- while the reduction pass it replaces costs 121 us.  Off by default; kept for A/B runs.
+# The data-gradient GEMM can also produce the two BatchNorm-backward reductions in its epilogue instead of a separate
+# reduction pass.  Off by default (not measured on H100); kept for A/B runs.
 USE_BN_LINKS = os.environ.get("ALIGNN_B200_BN_LINKS", "0") == "1"
 
 
@@ -355,7 +354,7 @@ def segment_mean_any_order(x: torch.Tensor, graph_ptr: torch.Tensor, second_orde
     return sums / counts.clamp_min(1).to(x.dtype).unsqueeze(1)
 
 
-# ---- tensor-core Linear (tcgen05, bf16x3) --------------------------------------------------------
+# ---- tensor-core Linear (wgmma, bf16x3) ----------------------------------------------------------
 class WeightImage:
     """bf16 hi/lo image of a weight matrix W[N,K] (or of W^T when transpose=True) in UMMA core-matrix
     order; valid until the weight changes (rebuilt every step in training)."""
@@ -508,7 +507,7 @@ def ptr_any(t: Optional[torch.Tensor]):
 @_on_tensor_device
 def gemm_nt(A: torch.Tensor, w: WeightImage, bias: Optional[torch.Tensor] = None,
             residual: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """out[M,N] = A[M,K] @ W^T (+ bias) (+ residual) on tcgen05.  A may be a column slice (row stride >= K)."""
+    """out[M,N] = A[M,K] @ W^T (+ bias) (+ residual) on wgmma.  A may be a column slice (row stride >= K)."""
     lib = _lib.load()
     if A.dim() != 2 or A.stride(1) != 1 or A.shape[1] != w.K:
         raise RuntimeError(f"gemm_nt: A must be [M,{w.K}] with unit column stride, got {tuple(A.shape)}/{A.stride()}")
@@ -532,7 +531,7 @@ def gemm_gather(A: torch.Tensor, w: WeightImage, bias: Optional[torch.Tensor] = 
                 add0: Optional[torch.Tensor] = None, idx0: Optional[torch.Tensor] = None,
                 add1: Optional[torch.Tensor] = None, idx1: Optional[torch.Tensor] = None,
                 stats: bool = False, out: Optional[torch.Tensor] = None, bn_aux=None):
-    """out[r] = A[r] @ W^T (+ bias) (+ add0[idx0[r]]) (+ add1[idx1[r]]) on tcgen05, A streamed by TMA tiles.
+    """out[r] = A[r] @ W^T (+ bias) (+ add0[idx0[r]]) (+ add1[idx1[r]]) on wgmma.
 
     add0 / add1 are 2-D fp32 views with unit column stride and w.N columns (column slices of a wider matrix are fine);
     idx None = identity (a residual).  stats=True also returns the per-CTA partial column sums [rows, 2, N] of out and
@@ -757,7 +756,7 @@ def _pad_cols(x: torch.Tensor, k_pad: int) -> torch.Tensor:
 
 
 class _TCLinearFn(torch.autograd.Function):
-    """y = x W^T + b on the tcgen05 bf16x3 GEMMs (forward, data gradient, weight gradient)."""
+    """y = x W^T + b on the wgmma bf16x3 GEMMs (forward, data gradient, weight gradient)."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, tbl):

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Benchmark of the ALIGNN edge-gated conv hot path on B200 (BASELINE.json metric).
+"""Benchmark of the ALIGNN edge-gated conv hot path on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--norm batchnorm|layernorm]
+                    [--dump-outputs DIR]
 
 A "step" is one forward + backward + optimizer update of ALIGNN (4 ALIGNN + 4 GCN layers, hidden
 256, the `ALIGNN` class of alignn/models/alignn.py, L1 loss as in train.py:240) on one synthetic
@@ -13,6 +14,9 @@ Prints ONE JSON line (rank 0).  Keys follow the driver contract; extra keys:
   step_hbm      whole-step compulsory bytes (SURVEY.md section 8d: 10.04 GB per batch fwd+bwd) / step time
   cpu_baseline  the oracle (torch-CPU restatement of the reference DGL path) on this box's cores
   e2e           same metric with the batch starting in pinned HOST memory every step and the loss read back
+--dump-outputs DIR writes what the last timed step (resident inputs) computed: DIR/loss.npy (float64), the flat
+gradient buffer DIR/grads.npy and the parameters after the optimizer update DIR/params.npy (float32).  The inputs
+and the initial model are seeded, so two builds run with the same arguments can be compared output for output.
 `--impl reference` times that CPU oracle alone (the reference's own implementation needs DGL, which
 cannot be installed offline; see DESIGN.md).
 """
@@ -48,6 +52,8 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true", help="launch every kernel eagerly instead of replaying CUDA graphs")
     ap.add_argument("--cpu-sample-graphs", type=int, default=0, help="0 = calibrate (~4 s of CPU work per step)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's loss, gradients and updated parameters as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -70,7 +76,7 @@ def peaks():
         with open(p) as fh:
             j = json.load(fh)
         return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3; not measured)"
 
 
 # ---------------------------------------------------------------------------------------------
@@ -219,7 +225,7 @@ def run_ours(args):
 
     rank, local, world = dp.init_from_env("nccl")
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a CUDA device (B200); there is no CPU path")
+        raise SystemExit("bench.py needs a CUDA device; there is no CPU path")
     if world != args.gpus:
         raise SystemExit(f"--gpus {args.gpus} but WORLD_SIZE={world}: launch with torch.distributed.run")
     torch.cuda.set_device(local)
@@ -303,22 +309,6 @@ def run_ours(args):
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         return ms.item()
 
-    def timed_repeats(fn, steps, budget_s=2.5, max_reps=10):
-        """Median of up to `max_reps` repetitions of exactly `steps` steps (the clock sampler needs seconds, a 20-step
-        region lasts ~0.2 s); every repetition is a full timed region as above."""
-        first = timed(fn, steps)
-        reps = int(max(1, min(max_reps, budget_s * 1e3 / max(first, 1e-3))))
-        if world > 1:
-            if cpu_group_ref[0] is not None:
-                t = torch.tensor([reps])
-                dist.broadcast(t, 0, group=cpu_group_ref[0])
-            else:
-                t = torch.tensor([reps], device=dev)
-                dist.broadcast(t, 0)
-            reps = int(t.item())
-        all_ms = [first] + [timed(fn, steps) for _ in range(reps - 1)]
-        return statistics.median(all_ms), all_ms
-
     # ---- warm-up (also builds the flat gradient buffer, the flat optimizer and the operand-image tables) ------------
     with torch.cuda.stream(work):
         g0, lg0, lat0, tgt0 = resident[0]
@@ -376,14 +366,17 @@ def run_ours(args):
             launches_per_step += _lib.launch_count() - l0         # the flat AdamW launch is one of the library's kernels
         barrier()
 
+    last = {}
+
     def run_resident(i):
         if use_graph:
             graphs_res[i % nb][0].replay()
+            last["loss"] = graphs_res[i % nb][1]
             if not nccl_in_graph:
                 reducer.reduce_flat()
                 graph_opt.replay()
         else:
-            step(resident[i % nb])
+            last["loss"] = step(resident[i % nb])
 
     # End to end = what a training loop with a prefetching loader does (train.py's DataLoader has pin_memory and
     # worker prefetch): while the GPU works on batch i, a copy stream moves batch i+1 from pinned host memory into the
@@ -441,14 +434,16 @@ def run_ours(args):
     if rank == 0:
         sampler.start()
     l0 = _lib.launch_count()
-    ms_total, reps_res = timed_repeats(run_resident, args.steps)
-    launches = (launches_per_step * args.steps) if use_graph else ((_lib.launch_count() - l0) // max(len(reps_res), 1))
+    ms_total = timed(run_resident, args.steps)
+    launches = (launches_per_step * args.steps) if use_graph else (_lib.launch_count() - l0)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["loss"], reducer.flat, model)
 
     # ---- timed: end to end from pinned host memory, loss read back every step ----------------
     with torch.cuda.stream(work):
         for i in range(2):
             run_e2e(i)
-    ms_e2e, reps_e2e = timed_repeats(run_e2e, args.steps)
+    ms_e2e = timed(run_e2e, args.steps)
     clocks = sampler.stop() if rank == 0 else None
 
     # ---- per-kernel table: CUDA events around every library call in an eager replay of the same steps (events inside
@@ -480,18 +475,11 @@ def run_ours(args):
     d = cfg.hidden_features
     sbytes = step_bytes(N, E, T, d, cfg.alignn_layers, cfg.gcn_layers)
     ms_step = ms_total / args.steps
-    traffic_tab = {}
-    tpath = os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")     # dram bytes per launch from `ncu --set full` captures
-    if os.path.exists(tpath) and args.norm == "batchnorm" and (N, E, T) == (1920, 23040, 276480):
-        with open(tpath) as fh:
-            traffic_tab = json.load(fh)
 
     def entry(name, k):
         # the kernel's L(g)-sized launches: algorithmic bytes / event time
         ach = k["big_bytes"] / (k["big_ms"] * 1e-3) / 1e9 if k["big_ms"] > 0 else 0.0
-        tr = traffic_tab.get(name)
         return {"kernel": name, "bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                "traffic": (tr or {}).get("dram_bytes_per_launch"), "traffic_source": (tr or {}).get("source"),
                 "share_of_eager_step": k["total_ms"] / ms_eager, "ms_per_step": k["total_ms"] / args.steps,
                 "launches_per_step": k["launches"] / args.steps, "big_launches_per_step": k["big_launches"] / args.steps,
                 "avg_big_launch_ms": k["big_ms"] / max(k["big_launches"], 1),
@@ -501,7 +489,7 @@ def run_ours(args):
     if table:
         roofline = dict(table[0])
         roofline["peak_source"] = peak_src
-        roofline["note"] = ("dominant kernel by total time in the step; achieved = algorithmic bytes (DESIGN.md section 4) of its "
+        roofline["note"] = ("dominant kernel by total time in the step; achieved = algorithmic bytes (BASELINE.md section 3) of its "
                             "L(g)-sized launches / CUDA-event time on the launching stream")
         roofline["extra"] = table[1:8]
     line = {
@@ -511,18 +499,17 @@ def run_ours(args):
         "config": {"workload": WORKLOAD, "norm": args.norm, "global_batch": graphs_per_step, "per_gpu_batch": args.batch,
                    "parallelism": f"dp{world}", "optimizer": "AdamW", "loss": "L1",
                    "l2": f"no explicit flush: per-step working set ~{sbytes / 1e9:.1f} GB >> 126 MB L2; 4 batches rotate"},
-        "run": {"device": "B200", "N": N, "E": E, "T": T,
+        "run": {"device": torch.cuda.get_device_name(dev), "N": N, "E": E, "T": T,
                 "optimizer_impl": "one launch over one flat parameter (alignn_b200.dp.FlatAdamW -> alignn_b200_adamw_flat)",
                 "cuda_graph": use_graph, "allreduce_in_graph": bool(nccl_in_graph), "eager_ms_per_step": ms_eager / args.steps,
-                "timing": f"median of {len(reps_res)} repetitions of exactly {args.steps} steps (each: events on the launching "
-                          f"stream, barrier + synchronize on both sides, max over ranks)",
-                "repetition_ms": [round(m, 3) for m in reps_res]},
+                "timing": f"exactly {args.steps} steps between events on the launching stream, barrier + synchronize on both "
+                          f"sides, max over ranks"},
         "roofline": roofline,
         "step_hbm": {"algorithmic_bytes_per_step": sbytes, "achieved": sbytes / (ms_step * 1e-3) / 1e9, "peak": peak,
                      "unit": "GB/s", "frac": sbytes / (ms_step * 1e-3) / 1e9 / peak,
                      "note": "conv-stack compulsory bytes per batch (SURVEY 8d) / whole step time incl. embeddings, GEMMs, optimizer"},
         "e2e": {"value": e2e_value, "unit": UNIT, "ms_per_step": ms_e2e / args.steps,
-                "h2d_bytes_per_step": int(h2d_bytes), "d2h_bytes_per_step": 4, "repetition_ms": [round(m, 3) for m in reps_e2e],
+                "h2d_bytes_per_step": int(h2d_bytes), "d2h_bytes_per_step": 4,
                 "how": ("every step: inputs pinned host -> device (copy stream, issued one step ahead so it overlaps the previous step's "
                         "kernels; the first step of a region copies its own inputs serially), CUDA-graph replay, loss device -> pinned "
                         "host, read by the host one step later") if use_graph else
@@ -541,6 +528,18 @@ def run_ours(args):
     print(json.dumps(line), flush=True)
     if world > 1:
         _finish(nccl_in_graph)
+
+
+def dump_outputs(out_dir, loss, flat_grads, model):
+    """What a caller of the timed training step receives: its loss, the gradients it reduced and the parameters the
+    optimizer left.  Under 64 MB for the default model (two float32 copies of ~4 M parameters)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray(loss.detach().double().cpu().numpy()))
+    np.save(os.path.join(out_dir, "grads.npy"), flat_grads.detach().float().cpu().numpy())
+    params = torch.cat([p.detach().reshape(-1).float().cpu() for p in model.parameters()])
+    np.save(os.path.join(out_dir, "params.npy"), params.numpy())
 
 
 def _finish(hard_exit):

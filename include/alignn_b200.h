@@ -1,5 +1,5 @@
 /*
- * alignn_b200.h -- C ABI of libalignn_b200.so: the B200 (sm_100a) edge-gated graph
+ * alignn_b200.h -- C ABI of libalignn_b200.so: the H100 (sm_90a) edge-gated graph
  * convolution hot path of ALIGNN.
  *
  * Drop-in boundary.  The reference (usnistgov/alignn, 100 % Python) reaches its device
@@ -235,8 +235,8 @@ int alignn_b200_gather_segment_sum(const float* Bh, const float* sigma, const in
                                    float* Sh, float* S, alignn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
- * Linear layers on the 5th-gen tensor cores (tcgen05.mma, bf16x3 split operands, fp32 accumulate in
- * TMEM; results agree with an fp32 GEMM to ~1e-5 relative):
+ * Linear layers on the Hopper tensor cores (wgmma, bf16x3 split operands, fp32 accumulate in
+ * registers; results agree with an fp32 GEMM to ~1e-5 relative):
  *     C[M,N] = A[M,K] * W[N,K]^T (+ bias[N]) (+ R[M,N])
  * Replaces the nn.Linear call sites alignn.py:98,99,101,104,110 (forward) and their data-gradient
  * GEMMs.  W is first converted once per step to a bf16 hi/lo image (`gemm_prepare_weights`;
@@ -267,7 +267,7 @@ int alignn_b200_gemm_nt(const float* A, int64_t lda, const void* w_image, int64_
                         const float* R, int64_t ldr, float* C, int64_t ldc, alignn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
- * Linear layer with a gather-add epilogue and optional column statistics (csrc/gemm_fused_tc.cu):
+ * Linear layer with a gather-add epilogue and optional column statistics (csrc/gemm_tc.cu):
  *     C[r, 0:N] = A[r, 0:K] * W^T (+ bias) (+ add0[i0(r), 0:N]) (+ add1[i1(r), 0:N]),   i(r) = idx ? idx[r] : r
  *     stats[blk][0][c] / stats[blk][1][c] = per-CTA partial sums of C[:, c] and C[:, c]^2  (optional; needs N in
  *     {32, 64, 128, 256}; rows = alignn_b200_gemm_gather_stat_rows(M, N); feed alignn_b200_bn_finalize, which = 0)
@@ -276,7 +276,7 @@ int alignn_b200_gemm_nt(const float* A, int64_t lda, const void* w_image, int64_
  * dst_gate bias by the caller) gives m = e_src[src] + e_dst[dst] + edge_gate(y) and the batch statistics of
  * BatchNorm1d(m) in one pass over y -- apply_edges(u_add_v) and the Linear fused, no [Ne,d] temporary.
  * With add0 = R, idx0 = NULL it is the data-gradient GEMM with its residual; without addends a plain Linear.
- * A is streamed by TMA tensor tiles (row stride lda floats, 16-byte aligned rows); W is an image from
+ * A is streamed row by row (row stride lda floats, 16-byte aligned rows); W is an image from
  * alignn_b200_gemm_prepare_weights.  Constraints: K % 32 == 0, N % 32 == 0, lda/ldc/ld0/ld1 % 4 == 0.
  * ---------------------------------------------------------------------------------------- */
 typedef struct {
@@ -305,7 +305,7 @@ int alignn_b200_gemm_gather_stat_rows(int64_t M, int N);
  *     out[g*DA + o, i] = sum_{r < K} A[r, g*DA + o] * B[r, i]        g < groups,  o < DA,  i < DB
  * i.e. dL/dW = GM^T y (groups = 1) and dL/dWcat = GP^T x (groups = 4) of SURVEY.md App. B, and the
  * rectangular weight gradients of the embedding MLPs (alignn.py:201-222).  Supported (DA, DB): DA == DB in
- * {32, 64, 128, 256}; (256,64), (256,96), (64,96), (64,32), (32,64).
+ * {32, 64, 128, 256}; (256,64), (256,96), (64,96), (64,32), (32,64), (32,96).
  * `workspace` holds the per-CTA partial tiles (size from alignn_b200_wgrad_workspace_bytes; 0 = unsupported). */
 size_t alignn_b200_wgrad_workspace_bytes(int64_t K, int DA, int DB, int groups);
 int alignn_b200_wgrad(const float* A, int64_t lda, const float* B, int64_t ldb, int64_t K, int DA, int DB, int groups,
@@ -317,7 +317,7 @@ int alignn_b200_wgrad(const float* A, int64_t lda, const float* B, int64_t ldb, 
  * ride along at the memory rate instead of paying a launch prologue and a grid barrier each.  `problems` is a HOST array
  * (copied into the kernel parameters: capturable in a CUDA graph); A, B, out are device pointers, 16-byte aligned,
  * leading dimensions multiples of 4.  Deterministic (fixed-order split-K).  The fallback on a device that cannot
- * co-schedule 148 CTAs runs the problems one by one through alignn_b200_wgrad and needs that function's workspace. */
+ * co-schedule one CTA per SM runs the problems one by one through alignn_b200_wgrad and needs that function's workspace. */
 typedef struct {
   const float* A; int64_t lda;     /* [K, >= D] output-gradient rows                                   */
   const float* B; int64_t ldb;     /* [K, >= D] input rows                                             */
@@ -418,10 +418,7 @@ int alignn_b200_segment_mean_backward(const float* g_out /*[B,d]*/, const int32_
 /* ------------------------------------------------------------------------------------------
  * Development aids (A/B switches and tracing used by tools/; not needed by a caller of the path).
  * ---------------------------------------------------------------------------------------- */
-void alignn_b200_debug_gemm_flags(int flags);               /* knock-out bits of the round-1 register-fed GEMM (gemm_nt) */
-void alignn_b200_debug_gemm_pair(int enabled);              /* route N = 256, K <= 256 gemm_gather calls to the two-CTA kernel */
 void alignn_b200_debug_egc_flags(int flags);                /* bit 0: register-staged pass 2 instead of the ring; bit 1: channel-half egc_backward_dst (d = 256, BatchNorm) instead of the full-row kernel */
-void alignn_b200_debug_gemm_trace(long long* device_buffer); /* per-role SM-clock timeline of CTA 0 of gemm_gather ([6][512]) */
 
 #ifdef __cplusplus
 }

@@ -1,4 +1,4 @@
-"""GPU (-m gpu): the tcgen05 bf16x3 Linear kernel against an fp64 matmul.
+"""GPU (-m gpu): the wgmma bf16x3 Linear kernel against an fp64 matmul.
 
 Tolerance 2e-5 relative to the output scale: the bf16x3 split drops terms of relative size
 <= 3*2^-18 per product (tc_common.cuh), ~4e-6 rms on a K=256 dot product."""
@@ -81,7 +81,8 @@ def test_wgrad_matches_fp64(K, D, groups):
     assert torch.equal(out, ops.wgrad(A, B, groups))          # deterministic split-K
 
 
-@pytest.mark.parametrize("K,DA,DB", [(276480, 256, 64), (23040, 256, 96), (5000, 64, 96), (777, 64, 32), (777, 32, 64)])
+@pytest.mark.parametrize("K,DA,DB", [(276480, 256, 64), (23040, 256, 96), (5000, 64, 96), (777, 64, 32), (777, 32, 64),
+                                     (5000, 32, 96)])
 def test_wgrad_rectangular_matches_fp64(K, DA, DB):
     """Embedding-MLP weight gradients: [out, in_padded] with out != in."""
     g = torch.Generator(device="cpu").manual_seed(K + DA + DB)
@@ -94,7 +95,7 @@ def test_wgrad_rectangular_matches_fp64(K, DA, DB):
     assert not ops.wgrad_supported(48, 64)
 
 
-# ---- gemm_gather: TMA-fed Linear with gather-add epilogue and column statistics (csrc/gemm_fused_tc.cu) -------------
+# ---- gemm_gather: Linear with gather-add epilogue and column statistics (csrc/gemm_tc.cu) ----------------------------
 @pytest.mark.parametrize("M,N,K", [(1, 32, 32), (127, 64, 64), (128, 256, 256), (129, 128, 96), (1000, 256, 256),
                                    (1920, 1024, 256), (23040, 256, 1024), (5000, 64, 96), (276480, 256, 256)])
 def test_gemm_gather_plain_matches_fp64_and_gemm_nt(M, N, K):

@@ -77,6 +77,7 @@ def test_conv_jvasp_vs_reference_golden(golden_dir, tag, norm, train):
     g = Graph(jv["src"], jv["dst"], 32)
     x, y = GI.features(11, 32, 64), GI.features(12, g.num_edges(), 64)
     out = _run_conv(_make_conv(norm, 64, 100, train), g, x, y, 100, 64)
+    out = {k: (v[::4] if k in ("y_out", "gy") else v) for k, v in out.items()}   # the fixture keeps every 4th edge row
     ref = {k: gold[f"{tag}.{k}"] for k in out}
     assert_dict_close(out, ref, what=tag)
 
@@ -89,9 +90,10 @@ def test_conv_linegraph_d256_vs_reference_golden(golden_dir, tag, norm, train):
     out = _run_conv(_make_conv(norm, 256, 200, train), lg, xm, z, 200, 256)
     for k in ("x_out", "gx", "g.edge_gate.weight", "g.src_gate.bias", "g.bn_edges.weight", "g.bn_nodes.bias",
               "g.dst_update.weight"):
-        assert_close(out[k], gold[f"{tag}.{k}"], what=f"{tag}.{k}")
-    assert_close(out["y_out"][::7], gold[f"{tag}.y_out_s"], what="y_out")
-    assert_close(out["gy"][::7], gold[f"{tag}.gy_s"], what="gy")
+        v = out[k][::8] if out[k].dim() == 2 else out[k]              # the fixture keeps every 8th row of matrices
+        assert_close(v, gold[f"{tag}.{k}"], what=f"{tag}.{k}")
+    assert_close(out["y_out"][::28], gold[f"{tag}.y_out_s"], what="y_out")
+    assert_close(out["gy"][::28], gold[f"{tag}.gy_s"], what="gy")
 
 
 @pytest.mark.parametrize("norm,train", [("batchnorm", True), ("layernorm", True), ("batchnorm", False)])

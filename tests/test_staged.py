@@ -3,9 +3,8 @@
 CPU part (always runs): the segment-aligned tile packer, and a numpy emulation of the kernel's tile / row-phase /
 column-phase data flow driven by the packer's descriptors, against the oracle's formulas -- this pins the tiling
 semantics the CUDA kernel implements.
-GPU part: the fully fused kernels (validated on B200 in round 2, bit-identical to the two-kernel path; measured 2x
-SLOWER than it -- their row-per-thread epilogue is bound by L2 gather latency, DESIGN.md -- and therefore not the
-shipped path) against the shipped gemm_nt + egc_forward pair.
+GPU part: the fully fused kernels (bit-identical to the two-kernel path; not the shipped path) against the shipped
+gemm_nt + egc_forward pair.
 """
 import os
 import sys
@@ -143,7 +142,7 @@ def test_tiled_dataflow_matches_oracle_formulas(staged):
 
 # ------------------------------------------------------------------------------------------------ GPU (opt-in)
 def needs_optin(f):
-    """(historical gate) the staged kernels ran and passed on B200 in round 2: their tests run with the GPU suite."""
+    """The staged kernels' tests run with the GPU suite (kept as a marker for them)."""
     return f
 
 

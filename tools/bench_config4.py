@@ -1,5 +1,5 @@
 """BASELINE config 4: ALIGNN-FF energy + per-atom forces on a ~1000-atom periodic supercell, 1 GPU.
-(Secondary config: reported in DESIGN.md / profiles, not the headline bench line.)
+(Secondary config, not the headline bench line.)
 Measures (a) the structure build -- periodic radius graph, sorted-CSR index, line graph, bond cosines -- on the host
 (native scan) and on the device (csrc/graph_device.cu), (b) one energy+forces evaluation launched eagerly and
 (c) replayed as ONE CUDA graph (forward, the autograd pass for the forces and the force reduction captured together)."""

@@ -1,4 +1,4 @@
-"""Secondary BASELINE.json configs (reported in DESIGN.md / profiles, not the headline bench line):
+"""Secondary BASELINE.json configs (not the headline bench line):
   config 2: full ALIGNN (4+4, d=256) inference, batch 64, eval-mode BatchNorm;
   config 5: gather/segment-sum primitive, 1e4..1e7 edges, d=256 (1288 algorithmic bytes per edge)."""
 import json

@@ -1,4 +1,4 @@
-"""A/B timing of the staged fused backward (node kernel + gm-producer/dgrad tcgen05 kernel) against the shipped
+"""A/B timing of the staged fused backward (node kernel + gm-producer/dgrad wgmma kernel) against the shipped
 `ops.egc_backward` (destination- AND source-keyed kernels) + data-gradient GEMM, train-mode BatchNorm, headline shapes.
 
     python tools/bench_fused_bwd.py [--iters 20] [--d 256] [--batch 64] [--graphs g,lg]

@@ -20,7 +20,7 @@ def build(force: bool = False) -> str:
         glob.glob(os.path.join(ROOT, "include", "*.h"))
     if force or not os.path.exists(LIB) or any(os.path.getmtime(s) > os.path.getmtime(LIB) for s in deps):
         nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-        cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+        cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
                "-shared", "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(STAGED, ".."), "-o", LIB] + sources
         print("[build_staged]", " ".join(cmd), flush=True)
         subprocess.check_call(cmd)
