@@ -18,9 +18,15 @@
 // mbarrier.
 //
 // Persistent, warp-specialised CTA (one per SM), 128 x BN output tiles, BN <= 128: the 128 x BN fp32 accumulator lives
-// in the registers of two consumer warpgroups (BN / 2 per thread), which also run the epilogue straight from registers.
+// in the registers of two consumer warpgroups (BN / 2 per thread).
 //   warps 0-7   : two consumer warpgroups, rows 0-63 / 64-127 of the tile: wgmma m64nBNk16, then the epilogue
 //   warps 8-15  : loaders / fp32->bf16x2 converters, up to STAGES chunks ahead of the MMAs
+// Mainloop: one wgmma group stays in flight; a stage is released once the MMAs of the next chunk have been issued.
+// Epilogue: the wgmma fragment of one consumer warp is 16 whole rows of the tile, so each warp stages its own rows
+// through a private shared-memory tile (no block barrier) and then works row by row: a row is BN / 4 lanes with one
+// float4 each, the addend rows of several rows are loaded before the first store, and C is written as contiguous row
+// segments.  The addend rows are read through __restrict__ pointers: C must not overlap A, add0, add1, the bias or
+// the BatchNorm vectors.
 #include "common.cuh"
 #include "tc_common.cuh"
 #include "api_common.h"
@@ -38,6 +44,7 @@ constexpr int THREADS = 32 * (MMA_WARPS + LOAD_WARPS);   // 512
 constexpr uint32_t LBO = 128;               // next 8-element K chunk
 constexpr uint32_t SBO = (BK / 8) * 128;    // next 8-row group (chunk-local image): 512 B
 constexpr int kMaxStatN = 256;              // widest output with column statistics
+constexpr int WARP_ROWS = 16;               // tile rows of one consumer warp's wgmma fragment
 
 template <int BN>
 struct Cfg {
@@ -45,10 +52,21 @@ struct Cfg {
   static constexpr int B_PLANE = BN * BK * 2;
   static constexpr int STAGE = 2 * A_PLANE + 2 * B_PLANE;
   static constexpr int PIPE_BYTES = STAGES * STAGE;
+  // accumulator staging, fp32, rows padded by 8 floats: the fragment stores (8 rows x 4 lane pairs per
+  // instruction) then fill all 32 banks twice, the minimum for 256 bytes
+  static constexpr int PITCH = BN + 8;
+  static constexpr int STG_BYTES = BM * PITCH * 4;
+  static constexpr int STAT_OFF = PIPE_BYTES + STG_BYTES;
   static constexpr int STAT_BYTES = MMA_WARPS * 2 * kMaxStatN * 4;   // per consumer warp: [2][N] column partials
-  static constexpr int BAR_OFF = PIPE_BYTES + STAT_BYTES;
+  static constexpr int BAR_OFF = STAT_OFF + STAT_BYTES;
   static constexpr int SMEM = BAR_OFF + 128;
   static_assert(SMEM <= 232448, "shared memory budget of one sm_90 CTA");
+  // row-oriented epilogue: LPR lanes per row (one float4 each), RPI rows per warp instruction, ITERS instructions
+  // for the warp's rows, G rows whose addends are in flight before the first store
+  static constexpr int LPR = BN / 4;
+  static constexpr int RPI = 32 / LPR;
+  static constexpr int ITERS = WARP_ROWS / RPI;
+  static constexpr int G = ITERS < 8 ? ITERS : 8;
 };
 
 struct Params {
@@ -82,6 +100,62 @@ __device__ __forceinline__ float dsilu_(float u) {          // d/du [u * sigmoid
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(u * -1.4426950408889634f));
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(sg) : "f"(1.f + e));
   return sg * (1.f + u * (1.f - sg));
+}
+
+__device__ __forceinline__ float4 ld4(const float* __restrict__ p) { return __ldg(reinterpret_cast<const float4*>(p)); }
+__device__ __forceinline__ float4 ld4s(const float* p) {          // 4 scalars: vectors of any 4-byte alignment
+  return p ? make_float4(__ldg(p), __ldg(p + 1), __ldg(p + 2), __ldg(p + 3)) : make_float4(0.f, 0.f, 0.f, 0.f);
+}
+
+// One consumer warp's WARP_ROWS rows of the tile, from its staged accumulator rows `stg` (row pitch Cfg::PITCH):
+//   C[r, col .. col + 3] = (acc + bias) + (add0[i0(r)] + add1[i1(r)]),   r = row0 + rw
+// i0 / i1 of row rw sit in lane rw (-1: no addend); col = n0 + 4 (lane % LPR).  s / q collect this lane's column
+// sums over its valid rows in row order (BatchNorm-backward mode: gu and gu (m - mean), see the kernel).
+template <int BN>
+__device__ __forceinline__ void epilogue_rows(const float* stg, float* __restrict__ C, int64_t ldc,
+                                              const float* __restrict__ add0, int64_t ld0,
+                                              const float* __restrict__ add1, int64_t ld1, int i0, int i1, int row0,
+                                              int M, int col, int lane, float4 b, bool bnmode, float4 sc, float4 sh,
+                                              float4 mu, float4& s, float4& q) {
+  using F = Cfg<BN>;
+  const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+  const int lr = lane / F::LPR, c = (lane % F::LPR) * 4;
+#pragma unroll
+  for (int g0 = 0; g0 < F::ITERS; g0 += F::G) {
+    float4 va[F::G], vb[F::G];
+#pragma unroll
+    for (int g = 0; g < F::G; ++g) {                         // every addend row of the group is requested first
+      const int rw = (g0 + g) * F::RPI + lr;
+      const int ia = __shfl_sync(0xffffffffu, i0, rw), ib = __shfl_sync(0xffffffffu, i1, rw);
+      va[g] = ia >= 0 ? ld4(add0 + (int64_t)ia * ld0 + col) : z4;
+      vb[g] = ib >= 0 ? ld4(add1 + (int64_t)ib * ld1 + col) : z4;
+    }
+#pragma unroll
+    for (int g = 0; g < F::G; ++g) {
+      const int rw = (g0 + g) * F::RPI + lr;
+      if (row0 + rw >= M) continue;
+      const float4 a = *reinterpret_cast<const float4*>(stg + rw * F::PITCH + c);
+      const float4 a0 = va[g], m = vb[g], a1 = bnmode ? z4 : m;
+      float4 o;
+      o.x = (a.x + b.x) + (a0.x + a1.x);
+      o.y = (a.y + b.y) + (a0.y + a1.y);
+      o.z = (a.z + b.z) + (a0.z + a1.z);
+      o.w = (a.w + b.w) + (a0.w + a1.w);
+      *reinterpret_cast<float4*>(C + (int64_t)(row0 + rw) * ldc + col) = o;
+      if (bnmode) {
+        // gu = o * silu'(m * scale + shift); sums of gu and gu * (m - mean): the two reductions of the train-mode
+        // BatchNorm backward for the layer that consumes this gradient
+        const float gx = o.x * dsilu_(fmaf(m.x, sc.x, sh.x)), gy = o.y * dsilu_(fmaf(m.y, sc.y, sh.y));
+        const float gz = o.z * dsilu_(fmaf(m.z, sc.z, sh.z)), gw = o.w * dsilu_(fmaf(m.w, sc.w, sh.w));
+        s.x += gx; s.y += gy; s.z += gz; s.w += gw;
+        q.x = fmaf(gx, m.x - mu.x, q.x); q.y = fmaf(gy, m.y - mu.y, q.y);
+        q.z = fmaf(gz, m.z - mu.z, q.z); q.w = fmaf(gw, m.w - mu.w, q.w);
+      } else {
+        s.x += o.x; s.y += o.y; s.z += o.z; s.w += o.w;
+        q.x = fmaf(o.x, o.x, q.x); q.y = fmaf(o.y, o.y, q.y); q.z = fmaf(o.z, o.z, q.z); q.w = fmaf(o.w, o.w, q.w);
+      }
+    }
+  }
 }
 
 template <int BN>
@@ -184,21 +258,31 @@ gemm_bf16x3_kernel(const Params p) {
 
   // ================= consumers: MMA + epilogue =================
   const int wg = warp >> 2;                                  // rows 64 wg .. 64 wg + 63 of the tile
-  const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's rows: r_lo, r_lo + 8
-  const int cq = 2 * (lane & 3);                             // and columns 8 j + cq, 8 j + cq + 1
+  const int wrow = wg * 64 + (warp & 3) * WARP_ROWS;         // this warp's fragment: tile rows wrow .. wrow + 15
   const bool bnmode = p.bn_scale != nullptr;
   const bool do_stats = p.stats != nullptr;
   const int N = p.N;
-  float* stat = reinterpret_cast<float*>(smem + F::PIPE_BYTES) + warp * 2 * N;   // this warp's column partials
+  float* stg = reinterpret_cast<float*>(smem + F::PIPE_BYTES) + wrow * F::PITCH;   // this warp's staged rows
+  float* stat = reinterpret_cast<float*>(smem + F::STAT_OFF) + warp * 2 * N;       // this warp's column partials
   if (do_stats)
     for (int i = lane; i < 2 * N; i += 32) stat[i] = 0.f;
   const uint32_t sbase = tc::smem_u32(smem);
   int s = 0, ph = 0;
   for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
     const int m0 = (tile / n_tiles) * BM, n0 = (tile % n_tiles) * BN;
+    // addend row indices of the warp's rows, one per lane, requested before the mainloop
+    int i0 = -1, i1 = -1;
+    {
+      const int gr = m0 + wrow + lane;
+      if (lane < WARP_ROWS && gr < M) {
+        if (p.add0) i0 = p.idx0 ? __ldg(p.idx0 + gr) : gr;
+        if (p.add1) i1 = p.idx1 ? __ldg(p.idx1 + gr) : gr;
+      }
+    }
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int prev = -1;
     for (int kc = 0; kc < nk; ++kc) {
       tc::mbar_wait(&full[s], ph);
       const uint32_t sa = sbase + s * F::STAGE;
@@ -214,74 +298,54 @@ gemm_bf16x3_kernel(const Params p) {
         tc::Wgmma<BN>::template mma<0, 0>(acc, dah, dbh, 1);
       }
       tc::wgmma_commit();
-      tc::wgmma_wait_all();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&empty[s]);             // this warp is done reading the stage
+      tc::wgmma_wait<1>();                                   // the MMAs of chunk kc - 1 are complete
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&empty[prev]);        // this warp is done reading that stage
+      }
+      prev = s;
       if (++s == STAGES) { s = 0; ph ^= 1; }
     }
-    // ---- epilogue from registers: (acc + bias) + (addend0 + addend1), row pieces of 8 bytes per lane ----
-    int ia[2], ib[2];
-    bool ok[2];
+    tc::wgmma_wait_all();
+    __syncwarp();
+    if (lane == 0 && prev >= 0) tc::mbar_arrive(&empty[prev]);
+    // ---- epilogue: stage the fragment (thread holds acc[4 j + 2 h + e] = row lane / 4 + 8 h, column 8 j + 2 (lane % 4)
+    //      + e of the warp's rows), then row by row: (acc + bias) + (addend0 + addend1) ----
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int gr = m0 + r_lo + 8 * h;
-      ok[h] = gr < M;
-      ia[h] = (p.add0 && ok[h]) ? (p.idx0 ? __ldg(p.idx0 + gr) : gr) : -1;
-      ib[h] = (p.add1 && ok[h]) ? (p.idx1 ? __ldg(p.idx1 + gr) : gr) : -1;
+    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        *reinterpret_cast<float2*>(stg + ((lane >> 2) + 8 * h) * F::PITCH + 8 * j + 2 * (lane & 3)) =
+            make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+    __syncwarp();
+    const int col = n0 + (lane % F::LPR) * 4;
+    const float4 b = ld4s(p.bias ? p.bias + col : nullptr);
+    float4 sc = make_float4(0.f, 0.f, 0.f, 0.f), sh = sc, mu = sc, s4 = sc, q4 = sc;
+    if (bnmode) {
+      sc = ld4s(p.bn_scale + col); sh = ld4s(p.bn_shift + col); mu = ld4s(p.bn_mean + col);
     }
-    const float2 z2 = make_float2(0.f, 0.f);
+    epilogue_rows<BN>(stg, p.C, p.ldc, p.add0, p.ld0, p.add1, p.ld1, i0, i1, m0 + wrow, M, col, lane, b, bnmode, sc, sh,
+                      mu, s4, q4);
+    if (do_stats) {
+      // lanes lane % LPR hold the same columns for different rows: fold them, fixed order
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int col = n0 + 8 * j + cq;
-      const float2 b2 = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : z2;
-      float2 sc = z2, sh = z2, mu = z2;
-      if (bnmode) {
-        sc = __ldg(reinterpret_cast<const float2*>(p.bn_scale + col));
-        sh = __ldg(reinterpret_cast<const float2*>(p.bn_shift + col));
-        mu = __ldg(reinterpret_cast<const float2*>(p.bn_mean + col));
+      for (int o = F::LPR; o < 32; o <<= 1) {
+        s4.x += __shfl_xor_sync(0xffffffffu, s4.x, o); s4.y += __shfl_xor_sync(0xffffffffu, s4.y, o);
+        s4.z += __shfl_xor_sync(0xffffffffu, s4.z, o); s4.w += __shfl_xor_sync(0xffffffffu, s4.w, o);
+        q4.x += __shfl_xor_sync(0xffffffffu, q4.x, o); q4.y += __shfl_xor_sync(0xffffffffu, q4.y, o);
+        q4.z += __shfl_xor_sync(0xffffffffu, q4.z, o); q4.w += __shfl_xor_sync(0xffffffffu, q4.w, o);
       }
-      float2 s2 = z2, q2 = z2;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const float2 a0 = ia[h] >= 0 ? __ldg(reinterpret_cast<const float2*>(p.add0 + (int64_t)ia[h] * p.ld0 + col)) : z2;
-        const float2 mrow = ib[h] >= 0 ? __ldg(reinterpret_cast<const float2*>(p.add1 + (int64_t)ib[h] * p.ld1 + col)) : z2;
-        const float2 a1 = bnmode ? z2 : mrow;
-        float2 o;
-        o.x = (acc[4 * j + 2 * h] + b2.x) + (a0.x + a1.x);
-        o.y = (acc[4 * j + 2 * h + 1] + b2.y) + (a0.y + a1.y);
-        if (ok[h]) {
-          *reinterpret_cast<float2*>(p.C + (int64_t)(m0 + r_lo + 8 * h) * p.ldc + col) = o;
-          if (bnmode) {
-            // gu = o * silu'(m * scale + shift); sums of gu and gu * (m - mean): the two reductions of the train-mode
-            // BatchNorm backward for the layer that consumes this gradient
-            const float gx = o.x * dsilu_(fmaf(mrow.x, sc.x, sh.x)), gy = o.y * dsilu_(fmaf(mrow.y, sc.y, sh.y));
-            s2.x += gx; s2.y += gy;
-            q2.x = fmaf(gx, mrow.x - mu.x, q2.x); q2.y = fmaf(gy, mrow.y - mu.y, q2.y);
-          } else {
-            s2.x += o.x; s2.y += o.y;
-            q2.x = fmaf(o.x, o.x, q2.x); q2.y = fmaf(o.y, o.y, q2.y);
-          }
-        }
-      }
-      if (do_stats) {
-        // lanes with equal (lane & 3) hold the same columns for the warp's 16 rows: fold them, fixed order
-#pragma unroll
-        for (int o = 4; o <= 16; o <<= 1) {
-          s2.x += __shfl_xor_sync(0xffffffffu, s2.x, o); s2.y += __shfl_xor_sync(0xffffffffu, s2.y, o);
-          q2.x += __shfl_xor_sync(0xffffffffu, q2.x, o); q2.y += __shfl_xor_sync(0xffffffffu, q2.y, o);
-        }
-        if (lane < 4) {
-          const int c = col;
-          stat[c] += s2.x; stat[c + 1] += s2.y;
-          stat[N + c] += q2.x; stat[N + c + 1] += q2.y;
-        }
+      if (lane < F::LPR) {
+        stat[col] += s4.x; stat[col + 1] += s4.y; stat[col + 2] += s4.z; stat[col + 3] += s4.w;
+        stat[N + col] += q4.x; stat[N + col + 1] += q4.y; stat[N + col + 2] += q4.z; stat[N + col + 3] += q4.w;
       }
     }
+    __syncwarp();                                            // staged rows read before the next tile overwrites them
   }
   if (do_stats) {
     // one partial row per CTA: the eight consumer warps' partials summed in a fixed order
     asm volatile("bar.sync 1, %0;" ::"n"(MMA_WARPS * 32) : "memory");
-    const float* all = reinterpret_cast<const float*>(smem + F::PIPE_BYTES);
+    const float* all = reinterpret_cast<const float*>(smem + F::STAT_OFF);
     float* out_row = p.stats + (int64_t)blockIdx.x * 2 * N;
     for (int i = tid; i < 2 * N; i += MMA_WARPS * 32) {
       float t = 0.f;
@@ -443,6 +507,7 @@ int alignn_b200_gemm_nt(const float* A, int64_t lda, const void* w_image, int64_
   if (M == 0) return ALIGNN_OK;
   if (!A || !w_image || !C || M > 0x7fffffff) return ALIGNN_ERR_BAD_ARG;
   if ((lda % 4) || (ldc % 4) || (R && (ldr % 4))) return ALIGNN_ERR_BAD_ARG;   // 16-byte row alignment
+  if (((uintptr_t)A & 15) || ((uintptr_t)C & 15) || ((uintptr_t)R & 15)) return ALIGNN_ERR_BAD_ARG;
   const int bn = pick_bn(N);
   if (bn == 0) return ALIGNN_ERR_UNSUPPORTED_D;
   Params p = {};

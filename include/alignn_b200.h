@@ -241,7 +241,8 @@ int alignn_b200_gather_segment_sum(const float* Bh, const float* sigma, const in
  * Replaces the nn.Linear call sites alignn.py:98,99,101,104,110 (forward) and their data-gradient
  * GEMMs.  W is first converted once per step to a bf16 hi/lo image (`gemm_prepare_weights`;
  * `transpose != 0` takes W^T of a [K,N] array, which is what the data-gradient GEMMs need).
- * Constraints: K % 32 == 0, N % 32 == 0, lda/ldc/ldr % 4 == 0 (16-byte rows).
+ * Constraints: K % 32 == 0, N % 32 == 0, lda/ldc/ldr % 4 == 0 and A, R, C 16-byte aligned (16-byte rows).
+ * C must not overlap A, R or bias: the epilogue reads the addends while other rows of C are being written.
  * ---------------------------------------------------------------------------------------- */
 size_t alignn_b200_gemm_weight_image_bytes(int N, int K);   /* 0 if the shape is unsupported */
 int alignn_b200_gemm_prepare_weights(const float* W, int N, int K, int64_t ldw, int transpose, void* image,
@@ -278,6 +279,8 @@ int alignn_b200_gemm_nt(const float* A, int64_t lda, const void* w_image, int64_
  * With add0 = R, idx0 = NULL it is the data-gradient GEMM with its residual; without addends a plain Linear.
  * A is streamed row by row (row stride lda floats, 16-byte aligned rows); W is an image from
  * alignn_b200_gemm_prepare_weights.  Constraints: K % 32 == 0, N % 32 == 0, lda/ldc/ld0/ld1 % 4 == 0.
+ * C must not overlap A, add0, add1, bias, the BatchNorm vectors or stats: the epilogue reads the addends while other
+ * rows of C are being written.
  * ---------------------------------------------------------------------------------------- */
 typedef struct {
   size_t struct_size;
