@@ -66,7 +66,6 @@ class GemmGatherArgs(C.Structure):
         ("add1", _fp), ("ld1", C.c_int64), ("idx1", _fp),
         ("C", _fp), ("ldc", C.c_int64),
         ("stats", _fp),
-        ("bn_scale", _fp), ("bn_shift", _fp), ("bn_mean", _fp),
         ("stream", _fp),
     ]
 
@@ -112,7 +111,6 @@ _SIGNATURES = {
     "alignn_b200_colsum_batch": (C.c_int, [C.POINTER(ColsumProblem), C.c_int, _fp]),
     "alignn_b200_gather_segment_sum": (C.c_int, [_fp, _fp, _fp, _fp, _fp, C.c_int64, C.c_int64, C.c_int, _fp, _fp, _fp]),
     "alignn_b200_gemm_weight_image_bytes": (C.c_size_t, [C.c_int, C.c_int]),
-    "alignn_b200_gemm_prepare_weights": (C.c_int, [_fp, C.c_int, C.c_int, C.c_int64, C.c_int, _fp, _fp]),
     "alignn_b200_gemm_prepare_table": (C.c_int, [_fp, C.c_int, C.c_int64, _fp, C.c_int, _fp]),
     "alignn_b200_gemm_nt": (C.c_int, [_fp, C.c_int64, _fp, C.c_int64, C.c_int, C.c_int, _fp, _fp, C.c_int64, _fp,
                                       C.c_int64, _fp]),
@@ -162,7 +160,7 @@ def load() -> C.CDLL:
     for name, (res, args) in _SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError if the .so does not export what the header declares
         fn.restype, fn.argtypes = res, args
-    if lib.alignn_b200_version() != 100:
+    if lib.alignn_b200_version() != 101:
         raise RuntimeError("libalignn_b200.so version mismatch; rebuild")
     _lib = lib
     return lib

@@ -16,8 +16,6 @@ it is reached through the C ABI (include/alignn_b200.h).
 """
 from __future__ import annotations
 
-import os
-
 import torch
 from torch import nn
 from torch.autograd.function import once_differentiable
@@ -27,13 +25,6 @@ from .graph import as_graph
 from .ops import NORM_AFFINE, NORM_LAYER, NORM_STATS
 
 GATE_EPS = 1e-6   # alignn.py:109
-# True: pass 1 = gather GEMM writes m and its batch statistics, pass 2 = segment reductions + edge tail.
-# False: the round-1 composition (plain GEMM writes G, the edge kernel forms m); kept for A/B runs and bit-identity tests.
-USE_GATHER_GEMM = os.environ.get("ALIGNN_B200_GATHER_GEMM", "1") != "0"
-# "1": independent kernels of a conv backward on parallel streams (see _Fork).  At batch 64 every one of these kernels
-# already fills the SMs (or is a cooperative launch), so the default is serial; the switch stays for small-graph
-# workloads.
-USE_SIDE_STREAMS = os.environ.get("ALIGNN_B200_SIDE_STREAMS", "0") != "0"
 
 
 class second_order:
@@ -74,46 +65,10 @@ def _torch_ops_forward(mod, ix, x, y, need_edge_out: bool):
     return x_out, y_out
 
 
-class _Fork:
-    """Fork / join of up to three side streams inside one autograd node, so that the independent kernels of a conv's
-    backward (node-side and edge-side reductions; the two data-gradient GEMMs and the two weight-gradient kernels) can
-    overlap: on the atom graph each of them keeps only a fraction of the SMs busy and is bound by its own pipeline
-    latency.  Results are joined on the calling stream before they are used or freed; the same pattern is legal inside
-    a CUDA-graph capture (parallel branches).  Memory: tensors allocated on a side stream are consumed on the main
-    stream after the join and the side stream re-synchronises with the main stream at the next fork, so the caching
-    allocator never hands a block to a kernel that can run before its previous reader."""
-    _pool = {}
-
-    def __init__(self, device, enabled=True):
-        self.enabled = enabled and USE_SIDE_STREAMS
-        self.main = torch.cuda.current_stream(device)
-        if self.enabled:
-            key = (device.index, self.main.cuda_stream)
-            if key not in _Fork._pool:
-                _Fork._pool[key] = [torch.cuda.Stream(device) for _ in range(3)]
-            self.side = _Fork._pool[key]
-            ev = torch.cuda.Event()
-            ev.record(self.main)
-            for s in self.side:
-                s.wait_event(ev)
-
-    def on(self, i, fn):
-        """Run `fn` on side stream i (0..2); on the calling stream when forking is disabled."""
-        if not self.enabled:
-            return fn()
-        with torch.cuda.stream(self.side[i]):
-            return fn()
-
-    def join(self):
-        if self.enabled:
-            for s in self.side:
-                self.main.wait_stream(s)
-
-
 class _Cfg:
     """Per-call, non-tensor configuration of the fused stage."""
     __slots__ = ("index", "norm_nodes", "norm_edges", "residual", "need_edge_out", "ln_eps",
-                 "bn_nodes", "bn_edges", "n_aux", "e_aux", "images", "legacy_w", "up_link", "e_link")
+                 "bn_nodes", "bn_edges", "n_aux", "e_aux", "images")
 
 
 def _bn_eval_vectors(bn: nn.BatchNorm1d):
@@ -156,72 +111,44 @@ class _EdgeGatedConvFn(torch.autograd.Function):
         bnn, bne = cfg.bn_nodes, cfg.bn_edges
 
         # node projections P = [e_src | Bh | e_dst | src_update] (include/alignn_b200.h); the edge-gate bias rides in
-        # the e_dst block, so the gate needs no bias of its own (weights are re-split every call: they change every step)
-        if USE_GATHER_GEMM:
-            img = cfg.images            # operand images, refreshed by one table-driven launch per step (ops.ImageTable)
-            P = ops.gemm_gather(x, img.images["cat"], img.vectors["bcat"])
-            # pass 1 over the edge rows (csrc/gemm_tc.cu): m = e_src[src] + e_dst[dst] + edge_gate(y) on wgmma,
-            # the P rows gathered in the epilogue, BatchNorm batch statistics of m on the way out
-            e_part = None
-            if Ne > 0:
-                res = ops.gemm_gather(y, img.images["eg"], None, add0=P[:, 0:d], idx0=ix.src,
-                                      add1=P[:, 2 * d:3 * d], idx1=ix.dst, stats=stats)
-                M, e_part = res if stats else (res, None)
-            else:
-                M = y.new_empty((0, d))
-            norm_e = cfg.norm_edges
-            if stats and Ne > 0:
-                # statistics (and running buffers) are updated even when the edge output is dead
-                # (SURVEY.md App. D-11): the reference always evaluates bn_edges(m).
-                track_e = bne.track_running_stats and bne.running_mean is not None
-                e_aux = ops.bn_finalize(e_part, 0, Ne, ew, eb, bne.eps, _momentum(bne),
-                                        bne.running_mean if track_e else None, bne.running_var if track_e else None)
-                e_w, e_b = e_aux[0], e_aux[1]
-            if stats:
-                norm_e = NORM_AFFINE
-            # pass 2 (csrc/egc_kernels.cu): sigmoid, both segment reductions by sorted-CSR index, y_out = y + silu(norm(m))
-            out = ops.egc_forward(ix, x, y, M, P, n_w, n_b, e_w, e_b, norm_nodes=cfg.norm_nodes, norm_edges=norm_e,
-                                  residual=cfg.residual, save=needs_grad, need_edge_out=cfg.need_edge_out and Ne > 0,
-                                  gate_eps=GATE_EPS, ln_eps=cfg.ln_eps, gate_is_m=True)
-            x_out, y_out = out["x_out"], out["y_out"]
-            if stats and needs_grad and y_out is not None and ops.USE_BN_LINKS:
-                cfg.e_link = ops.BNLink(M, e_aux[0], e_aux[1], e_aux[2], e_aux[3], Ne)
-            if stats:
-                track_n = bnn.track_running_stats and bnn.running_mean is not None
-                n_aux = ops.bn_finalize(out["partials"], 1, Nn, nw, nb, bnn.eps, _momentum(bnn),
-                                        bnn.running_mean if track_n else None, bnn.running_var if track_n else None)
-                x_out = ops.affine_silu_residual(out["XP"], x if cfg.residual else None, n_aux[0], n_aux[1])
+        # the e_dst block, so the gate needs no bias of its own
+        img = cfg.images            # operand images, refreshed by one table-driven launch per step (ops.ImageTable)
+        P = ops.gemm_gather(x, img.images["cat"], img.vectors["bcat"])
+        # pass 1 over the edge rows (csrc/gemm_tc.cu): m = e_src[src] + e_dst[dst] + edge_gate(y) on wgmma,
+        # the P rows gathered in the epilogue, BatchNorm batch statistics of m on the way out
+        e_part = None
+        if Ne > 0:
+            res = ops.gemm_gather(y, img.images["eg"], None, add0=P[:, 0:d], idx0=ix.src,
+                                  add1=P[:, 2 * d:3 * d], idx1=ix.dst, stats=stats)
+            M, e_part = res if stats else (res, None)
         else:
-            Wcat = torch.cat([W_sg, W_du, W_dg, W_su], 0)
-            bcat = torch.cat([b_sg, b_du, b_dg, b_su], 0)
-            P = ops.gemm_nt(x, ops.WeightImage(Wcat), bcat)
-            G = ops.gemm_nt(y, ops.WeightImage(W_eg.contiguous()), b_eg.contiguous())
-            out = ops.egc_forward(ix, x, y, G, P, n_w, n_b, e_w, e_b, norm_nodes=cfg.norm_nodes,
-                                  norm_edges=cfg.norm_edges, residual=cfg.residual, save=needs_grad,
-                                  need_edge_out=cfg.need_edge_out, gate_eps=GATE_EPS, ln_eps=cfg.ln_eps)
-            x_out, y_out = out["x_out"], out["y_out"]
-            if stats:
-                # BatchNorm1d train mode (alignn.py:122-123): batch statistics, running-stat update
-                track_n = bnn.track_running_stats and bnn.running_mean is not None
-                track_e = bne.track_running_stats and bne.running_mean is not None
-                n_aux = ops.bn_finalize(out["partials"], 1, Nn, nw, nb, bnn.eps, _momentum(bnn),
-                                        bnn.running_mean if track_n else None, bnn.running_var if track_n else None)
-                x_out = ops.affine_silu_residual(out["XP"], x if cfg.residual else None, n_aux[0], n_aux[1])
-                if Ne > 0:
-                    e_aux = ops.bn_finalize(out["partials"], 0, Ne, ew, eb, bne.eps, _momentum(bne),
-                                            bne.running_mean if track_e else None, bne.running_var if track_e else None)
-                    if cfg.need_edge_out:
-                        y_out = ops.affine_silu_residual(out["M"], y if cfg.residual else None, e_aux[0], e_aux[1])
+            M = y.new_empty((0, d))
+        norm_e = cfg.norm_edges
+        if stats and Ne > 0:
+            # statistics (and running buffers) are updated even when the edge output is dead
+            # (SURVEY.md App. D-11): the reference always evaluates bn_edges(m).
+            track_e = bne.track_running_stats and bne.running_mean is not None
+            e_aux = ops.bn_finalize(e_part, 0, Ne, ew, eb, bne.eps, _momentum(bne),
+                                    bne.running_mean if track_e else None, bne.running_var if track_e else None)
+            e_w, e_b = e_aux[0], e_aux[1]
         if stats:
+            norm_e = NORM_AFFINE
+        # pass 2 (csrc/egc_kernels.cu): sigmoid, both segment reductions by sorted-CSR index, y_out = y + silu(norm(m))
+        out = ops.egc_forward(ix, x, y, M, P, n_w, n_b, e_w, e_b, norm_nodes=cfg.norm_nodes, norm_edges=norm_e,
+                              residual=cfg.residual, save=needs_grad, need_edge_out=cfg.need_edge_out and Ne > 0,
+                              gate_eps=GATE_EPS, ln_eps=cfg.ln_eps, gate_is_m=True)
+        x_out, y_out = out["x_out"], out["y_out"]
+        if stats:
+            track_n = bnn.track_running_stats and bnn.running_mean is not None
+            n_aux = ops.bn_finalize(out["partials"], 1, Nn, nw, nb, bnn.eps, _momentum(bnn),
+                                    bnn.running_mean if track_n else None, bnn.running_var if track_n else None)
+            x_out = ops.affine_silu_residual(out["XP"], x if cfg.residual else None, n_aux[0], n_aux[1])
             for bn in (bnn, bne):
                 if bn.track_running_stats and bn.num_batches_tracked is not None:
                     bn.num_batches_tracked.add_(1)
         if needs_grad:
             ctx.cfg = cfg
             cfg.n_aux, cfg.e_aux = n_aux, e_aux
-            if not USE_GATHER_GEMM:
-                cfg.images = None
-                cfg.legacy_w = (Wcat, W_eg)
             ctx.save_for_backward(x, y, P, out["M"], out["XP"], out["S"], out["H"], nw, nb, ew, eb)
             ctx.weights = (W_sg, W_dg, W_eg, W_su, W_du)          # identities only: ops.WgradQueue maps them to destinations
             ctx.biases = (b_sg, b_dg, b_eg, b_su, b_du)
@@ -236,11 +163,7 @@ class _EdgeGatedConvFn(torch.autograd.Function):
     def backward(ctx, gx_out, gy_out):
         cfg = ctx.cfg
         x, y, P, M, XP, S, H, nw, nb, ew, eb = ctx.saved_tensors
-        if cfg.images is not None:
-            img_catT, img_egT = cfg.images.images["catT"], cfg.images.images["egT"]
-        else:
-            img_catT = ops.WeightImage(cfg.legacy_w[0], transpose=True)
-            img_egT = ops.WeightImage(cfg.legacy_w[1].contiguous(), transpose=True)
+        img_catT, img_egT = cfg.images.images["catT"], cfg.images.images["egT"]
         d = x.shape[1]
         gx_out = gx_out.contiguous()
         gy_out = None if (ctx.y_dead or gy_out is None) else gy_out.contiguous()
@@ -255,14 +178,9 @@ class _EdgeGatedConvFn(torch.autograd.Function):
                 sc, sh, mu, rs = cfg.e_aux
                 e = dict(w=sc, b=sh, mean=mu, rstd=rs)
             if cfg.norm_nodes == NORM_STATS:
-                fk = _Fork(x.device)
-                cn = fk.on(0, lambda: ops.bn_backward_reduce(XP, gx_out, n["w"], n["b"], n["mean"], n["rstd"]))
+                n["c1"], n["c2"] = ops.bn_backward_reduce(XP, gx_out, n["w"], n["b"], n["mean"], n["rstd"])
                 if gy_out is not None:
-                    got = cfg.e_link.take(gy_out) if cfg.e_link is not None else None   # sums from the consumer's GEMM epilogue
-                    e["c1"], e["c2"] = got if got is not None else \
-                        ops.bn_backward_reduce(M, gy_out, e["w"], e["b"], e["mean"], e["rstd"])
-                fk.join()
-                n["c1"], n["c2"] = cn
+                    e["c1"], e["c2"] = ops.bn_backward_reduce(M, gy_out, e["w"], e["b"], e["mean"], e["rstd"])
         # Parameter gradients are off the critical path of backward.  With a queue installed (FlatGradAllReducer.deferring())
         # the five weight-gradient GEMMs and the nine bias / norm-parameter reductions of this conv are only registered
         # here and computed by two batched launches at the end of backward, straight into the flat gradient buffer.
@@ -277,13 +195,11 @@ class _EdgeGatedConvFn(torch.autograd.Function):
                                           norm_nodes=cfg.norm_nodes, norm_edges=cfg.norm_edges,
                                           gate_eps=GATE_EPS, ln_eps=cfg.ln_eps)
         # GEMM halves of the backward on the tensor cores: data gradients (gemm_tc.cu, transposed weight images,
-        # residual added in the epilogue) and weight gradients (wgrad_tc.cu, split-K over rows); four independent
-        # kernels, forked over side streams
+        # residual added in the epilogue) and weight gradients (wgrad_tc.cu, split-K over rows)
         need = ctx.needs_input_grad
         gx = gy = None
-        fk = _Fork(x.device)
         if need[1]:
-            gx = fk.on(0, lambda: ops.gemm_gather(GP, img_catT, None, add0=gx_out if cfg.residual else None))
+            gx = ops.gemm_gather(GP, img_catT, None, add0=gx_out if cfg.residual else None)
         if deferred:
             for j, W in enumerate((W_sg, W_du, W_dg, W_su)):           # column blocks of GP: e_src | Bh | e_dst | src_update
                 queue.add(GP[:, j * d:(j + 1) * d], x, W)
@@ -300,19 +216,11 @@ class _EdgeGatedConvFn(torch.autograd.Function):
             queue.add_vec(vs, 0, d, b_sg)
             queue.add_vec(vs, 1, d, b_du)
         elif params:
-            gWcat = fk.on(1, lambda: ops.wgrad(GP, x, groups=4))      # [4d, d] rows: src_gate | dst_update | dst_gate | src_update
-            gW_eg = fk.on(2, lambda: ops.wgrad(GM, y, groups=1))
+            gWcat = ops.wgrad(GP, x, groups=4)      # [4d, d] rows: src_gate | dst_update | dst_gate | src_update
+            gW_eg = ops.wgrad(GM, y, groups=1)
         if need[2]:
             res = gy_out if (gy_out is not None and cfg.residual) else None
-            up = cfg.up_link
-            if up is not None and up.usable_for(y):
-                # the gradient leaving here feeds a train-mode BatchNorm + SiLU upstream: its two reductions ride on the
-                # epilogue of this GEMM (ops.BNLink)
-                gy, up.partials = ops.gemm_gather(GM, img_egT, None, add0=res, bn_aux=(up.rows, up.scale, up.shift, up.mean))
-                up.grad_ptr = gy.data_ptr()
-            else:
-                gy = ops.gemm_gather(GM, img_egT, None, add0=res)
-        fk.join()
+            gy = ops.gemm_gather(GM, img_egT, None, add0=res)
         if not params:
             return (None, gx, gy) + (None,) * 14
         if deferred:
@@ -400,13 +308,8 @@ class EdgeGatedGraphConvBase(nn.Module):
         cfg.need_edge_out = bool(_need_edge_out)
         cfg.bn_nodes, cfg.bn_edges = self.bn_nodes, self.bn_edges
         cfg.n_aux = cfg.e_aux = None
-        cfg.legacy_w = None
-        cfg.images = None
-        cfg.e_link = None
-        cfg.up_link = getattr(edge_feats, "_alignn_b200_bn_link", None) if (USE_GATHER_GEMM and ops.USE_BN_LINKS) else None
-        if USE_GATHER_GEMM:
-            cfg.images = self.image_table()
-            cfg.images.refresh()          # no launch if the model-level table already refreshed this step
+        cfg.images = self.image_table()
+        cfg.images.refresh()          # no launch if the model-level table already refreshed this step
         if self.norm_kind == "layernorm":
             cfg.norm_nodes = cfg.norm_edges = NORM_LAYER
             cfg.ln_eps = float(self.bn_nodes.eps)
@@ -416,8 +319,6 @@ class EdgeGatedGraphConvBase(nn.Module):
             cfg.ln_eps = 1e-5
         with torch.cuda.device(node_feats.device):     # kernels launch on the tensors' device, whatever the current one is
             x, y = self._run_kernels(cfg, node_feats, edge_feats)
-        if _need_edge_out and cfg.e_link is not None:
-            y._alignn_b200_bn_link = cfg.e_link         # see ops.BNLink
         return x, (y if _need_edge_out else None)
 
     def _run_kernels(self, cfg, node_feats, edge_feats):

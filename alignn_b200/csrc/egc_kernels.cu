@@ -589,161 +589,6 @@ egc_backward_dst_kernel(alignn_b200_egc_bwd_args a) {
   }
 }
 
-// ---- destination-keyed backward for the per-channel norms (BatchNorm train / eval), d = 256, one channel half at a time --
-// Same arithmetic per element as egc_backward_dst_kernel<256, NORM>.  That kernel sits at 80 % of the LSU data pipe: per
-// EDGE it reads six per-channel vectors and the node's two parked gradient rows from shared memory and does two
-// accumulator read-modify-writes there (12 KB of shared-memory traffic for 4 KB of HBM traffic), because 8 values per lane
-// of everything do not fit in registers.  With BatchNorm every quantity is per channel, so a warp can walk its segment
-// twice, 128 channels (one float4 per lane) at a time: the six vector halves (24 registers), the node's gradient halves and
-// the two accumulators then live in registers for the whole segment, and shared memory is touched once per (node, half)
-// instead of per edge.  Every global access is still a fully used 512-byte warp request.  (LayerNorm needs the whole row
-// for its statistics and keeps the full-row kernel.)  With 512-byte instead of 1 KB requests and the same
-// 16 warps per SM the bytes in flight halve, which made it slower than the full-row kernel where it was measured.  Kept opt-in (alignn_b200_debug_egc_flags bit 1).  The per-warp partial sums are accumulated per segment before they
-// are added to the running totals, so the parameter-gradient partials differ from the full-row kernel in the last bits;
-// GM and GP are bit-identical.
-template <int NORM>
-__global__ void __launch_bounds__(kThreads, 2)
-egc_backward_dst_half_kernel(alignn_b200_egc_bwd_args a) {
-  static_assert(NORM == ALIGNN_NORM_AFFINE || NORM == ALIGNN_NORM_STATS, "per-channel norms only");
-  constexpr int D = 256, HW = 128;                          // channels per half: one float4 per lane
-  extern __shared__ __align__(16) float dyn_smem[];
-  float* sacc = dyn_smem;                                   // [kWarpsPerBlock][6][D]
-  float* nvec = dyn_smem + kWarpsPerBlock * 6 * D;          // node norm vectors [6][D]: w, b, mean, rstd, c1, c2
-  float* evec = nvec + 6 * D;                               // edge norm vectors [6][D]
-  {
-    const float* srcs[12] = {a.n_w, a.n_b, a.n_mean, a.n_rstd, a.n_c1, a.n_c2, a.e_w, a.e_b, a.e_mean, a.e_rstd, a.e_c1, a.e_c2};
-#pragma unroll
-    for (int q = 0; q < 12; ++q)
-      for (int i = threadIdx.x; i < D; i += blockDim.x) nvec[q * D + i] = srcs[q] ? srcs[q][i] : 0.f;
-  }
-  __syncthreads();
-  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-  const int64_t warp0 = (int64_t)blockIdx.x * kWarpsPerBlock + wib;
-  const int64_t nwarps = (int64_t)gridDim.x * kWarpsPerBlock;
-  float* acc = sacc + wib * 6 * D;
-  for (int i = lane; i < 6 * D; i += 32) acc[i] = 0.f;
-  __syncwarp();
-  const bool edge_out = a.gy_out != nullptr;
-  auto ld4 = [](const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); };
-  auto ld4s = [](const float* p) { return __ldcs(reinterpret_cast<const float4*>(p)); };
-  auto lds4 = [](const float* p) { return *reinterpret_cast<const float4*>(p); };
-  auto acc4 = [](float* p, const float4& v) {               // this lane's four channels of a per-warp accumulator row
-    float4 t = *reinterpret_cast<float4*>(p);
-    t.x += v.x; t.y += v.y; t.z += v.z; t.w += v.w;
-    *reinterpret_cast<float4*>(p) = t;
-  };
-  // one element of a norm backward: gu = go * silu'(r w + b); xh = (r - mean) rstd; returns dL/dr
-  auto norm_bwd = [](float r, float go, float w, float b, float mu, float rs, float c1, float c2, float& gu, float& xh) {
-    gu = go * dsilu_(r * w + b);
-    xh = (r - mu) * rs;
-    float gr = w * gu;
-    if (NORM == ALIGNN_NORM_STATS) gr -= w * (c1 + xh * c2);
-    return gr;
-  };
-
-  for (int64_t v = warp0; v < a.Nn; v += nwarps) {
-    const int p0 = a.in_ptr[v], p1 = a.in_ptr[v + 1];
-    const bool one_chunk = p1 - p0 <= 32;
-    int my_e = 0, my_s = 0;
-    if (one_chunk && lane < p1 - p0) {                       // indices shared by both halves
-      my_e = a.in_eid ? a.in_eid[p0 + lane] : p0 + lane;
-      my_s = a.src[my_e];
-    }
-#pragma unroll 1
-    for (int h = 0; h < 2; ++h) {
-      const int co = h * HW + lane * 4;                      // this lane's channels of the half
-      // ---- node side ----
-      float4 gsh, gs;
-      {
-        const float4 xp = ld4(a.XP + v * D + co), go = ld4(a.gx_out + v * D + co);
-        const float4 w = lds4(nvec + co), b = lds4(nvec + D + co), mu = lds4(nvec + 2 * D + co), rs = lds4(nvec + 3 * D + co);
-        const float4 c1 = lds4(nvec + 4 * D + co), c2 = lds4(nvec + 5 * D + co);
-        float4 gu, xh, gxp;
-        gxp.x = norm_bwd(xp.x, go.x, w.x, b.x, mu.x, rs.x, c1.x, c2.x, gu.x, xh.x);
-        gxp.y = norm_bwd(xp.y, go.y, w.y, b.y, mu.y, rs.y, c1.y, c2.y, gu.y, xh.y);
-        gxp.z = norm_bwd(xp.z, go.z, w.z, b.z, mu.z, rs.z, c1.z, c2.z, gu.z, xh.z);
-        gxp.w = norm_bwd(xp.w, go.w, w.w, b.w, mu.w, rs.w, c1.w, c2.w, gu.w, xh.w);
-        acc4(acc + 2 * D + co, make_float4(gu.x * xh.x, gu.y * xh.y, gu.z * xh.z, gu.w * xh.w));
-        acc4(acc + 3 * D + co, gu);
-        acc4(acc + 4 * D + co, gxp);
-        *reinterpret_cast<float4*>(a.GP + v * 4 * D + 3 * D + co) = gxp;
-        const float4 sv = ld4(a.S + v * D + co), hv = ld4(a.H + v * D + co);
-        const float ix = 1.f / (sv.x + a.gate_eps), iy = 1.f / (sv.y + a.gate_eps), iz = 1.f / (sv.z + a.gate_eps),
-                    iw = 1.f / (sv.w + a.gate_eps);
-        gsh = make_float4(gxp.x * ix, gxp.y * iy, gxp.z * iz, gxp.w * iw);
-        gs = make_float4(-gxp.x * hv.x * ix, -gxp.y * hv.y * iy, -gxp.z * hv.z * iz, -gxp.w * hv.w * iw);
-        *reinterpret_cast<float4*>(a.GSh + v * D + co) = gsh;
-      }
-      // ---- edge side: vector halves and accumulators in registers for the whole segment ----
-      const float4 w = lds4(evec + co), b = lds4(evec + D + co), mu = lds4(evec + 2 * D + co), rs = lds4(evec + 3 * D + co);
-      const float4 c1 = lds4(evec + 4 * D + co), c2 = lds4(evec + 5 * D + co);
-      float4 accB = make_float4(0.f, 0.f, 0.f, 0.f), agw = accB, agb = accB;
-      for (int base = p0; base < p1; base += 32) {
-        const int cnt = min(32, p1 - base);
-        if (!one_chunk) {
-          my_e = 0; my_s = 0;
-          if (lane < cnt) {
-            my_e = a.in_eid ? a.in_eid[base + lane] : base + lane;
-            my_s = a.src[my_e];
-          }
-        }
-        // software pipeline: the rows of edge i+1 are requested before edge i is processed
-        float4 m = accB, go = accB, cv = accB;
-        {
-          const int64_t e = __shfl_sync(0xffffffffu, my_e, 0), sidx = __shfl_sync(0xffffffffu, my_s, 0);
-          m = ld4s(a.M + e * D + co);
-          if (edge_out) go = ld4s(a.gy_out + e * D + co);
-          cv = ld4(a.P + sidx * 4 * D + D + co);
-        }
-        for (int i = 0; i < cnt; ++i) {
-          const int64_t e = __shfl_sync(0xffffffffu, my_e, i);
-          float4 mn = m, gon = go, cvn = cv;
-          if (i + 1 < cnt) {
-            const int64_t en = __shfl_sync(0xffffffffu, my_e, i + 1), sn = __shfl_sync(0xffffffffu, my_s, i + 1);
-            mn = ld4s(a.M + en * D + co);
-            if (edge_out) gon = ld4s(a.gy_out + en * D + co);
-            cvn = ld4(a.P + sn * 4 * D + D + co);
-          }
-          float4 gm = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (edge_out) {
-            float4 gu, xh;
-            gm.x = norm_bwd(m.x, go.x, w.x, b.x, mu.x, rs.x, c1.x, c2.x, gu.x, xh.x);
-            gm.y = norm_bwd(m.y, go.y, w.y, b.y, mu.y, rs.y, c1.y, c2.y, gu.y, xh.y);
-            gm.z = norm_bwd(m.z, go.z, w.z, b.z, mu.z, rs.z, c1.z, c2.z, gu.z, xh.z);
-            gm.w = norm_bwd(m.w, go.w, w.w, b.w, mu.w, rs.w, c1.w, c2.w, gu.w, xh.w);
-            agw.x += gu.x * xh.x; agw.y += gu.y * xh.y; agw.z += gu.z * xh.z; agw.w += gu.w * xh.w;
-            agb.x += gu.x; agb.y += gu.y; agb.z += gu.z; agb.w += gu.w;
-          }
-          {
-            const float sx = sigmoidf_(m.x), sy = sigmoidf_(m.y), sz = sigmoidf_(m.z), sw = sigmoidf_(m.w);
-            gm.x += (gsh.x * cv.x + gs.x) * sx * (1.f - sx);
-            gm.y += (gsh.y * cv.y + gs.y) * sy * (1.f - sy);
-            gm.z += (gsh.z * cv.z + gs.z) * sz * (1.f - sz);
-            gm.w += (gsh.w * cv.w + gs.w) * sw * (1.f - sw);
-            accB.x += gm.x; accB.y += gm.y; accB.z += gm.z; accB.w += gm.w;
-          }
-          *reinterpret_cast<float4*>(a.GM + e * D + co) = gm;   // re-read by the src-keyed pass and the GEMMs
-          m = mn; go = gon; cv = cvn;
-        }
-      }
-      *reinterpret_cast<float4*>(a.GP + v * 4 * D + 2 * D + co) = accB;
-      acc4(acc + co, agw);
-      acc4(acc + D + co, agb);
-      acc4(acc + 5 * D + co, accB);
-    }
-  }
-  __syncthreads();
-  if (a.partials) {   // fixed-order sum over the block's warps -> one partial row
-    float* out_row = a.partials + (int64_t)blockIdx.x * 6 * D;
-    for (int i = threadIdx.x; i < 6 * D; i += blockDim.x) {
-      float t = 0.f;
-#pragma unroll
-      for (int w = 0; w < kWarpsPerBlock; ++w) t += sacc[w * 6 * D + i];
-      out_row[i] = t;
-    }
-  }
-}
-
 // =============================================================================================
 // Backward, source-keyed pass (out-CSR): GP[:, 0:d] = sum over out-edges of GM (dL/d e_src),
 // GP[:, d:2d] = sum over out-edges of GSh[dst] * sigma (dL/d Bh).
@@ -1180,8 +1025,7 @@ int one_wave_grid(const void* kernel, int threads, size_t dyn_smem, int wanted_b
 namespace {
 using alignn::check_launch;
 using alignn::g_launches;
-std::atomic<int> g_forward_ring{1};      // A/B switches (alignn_b200_debug_egc_flags: bit 0 selects the register-staged pass 2, bit 1 the channel-half backward)
-std::atomic<int> g_backward_half{0};     // channel-half egc_backward_dst: correct, measured slower (418 vs 370 us dst+src), opt-in
+std::atomic<int> g_forward_ring{1};      // alignn_b200_debug_egc_flags bit 0 selects the register-staged pass 2 instead
 using alignn::g_last_cuda_error;
 inline bool supported_d(int d) { return d == 32 || d == 64 || d == 128 || d == 256; }
 inline int grid_for_rows(int64_t n) {
@@ -1219,7 +1063,7 @@ const char* alignn_b200_strerror(int s) {
 }
 
 int alignn_b200_last_cuda_error(void) { return g_last_cuda_error.load(); }
-void alignn_b200_debug_egc_flags(int flags) { g_forward_ring.store((flags & 1) ? 0 : 1); g_backward_half.store((flags & 2) ? 1 : 0); }
+void alignn_b200_debug_egc_flags(int flags) { g_forward_ring.store((flags & 1) ? 0 : 1); }
 uint64_t alignn_b200_launch_count(void) { return g_launches.load(); }
 
 int alignn_b200_egc_partial_rows(int64_t Nn, int d) { (void)d; return grid_for_rows(Nn); }
@@ -1316,29 +1160,11 @@ int alignn_b200_egc_backward(const alignn_b200_egc_bwd_args* a) {
     }                                                                                                          \
     alignn::egc_backward_dst_kernel<D, NORM><<<grid, alignn::kThreads, smem_bytes, st>>>(*a);                  \
   })
-#define LAUNCH_BWD_DST_HALF(NORM)                                                                              \
-  {                                                                                                            \
-    const size_t smem_bytes = (size_t)(alignn::kWarpsPerBlock * 6 + 12) * 256 * sizeof(float);                 \
-    static alignn::DeviceOnce configured; int cfg_dev;                                                                            \
-    if (configured.needed(&cfg_dev)) {                                                                                         \
-      cudaError_t e = cudaFuncSetAttribute(alignn::egc_backward_dst_half_kernel<NORM>,                         \
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);      \
-      if (e != cudaSuccess) return alignn::record_cuda_error((int)e);                                          \
-      configured.done(cfg_dev);                                                                                       \
-    }                                                                                                          \
-    alignn::egc_backward_dst_half_kernel<NORM><<<grid, alignn::kThreads, smem_bytes, st>>>(*a);                \
-  }
-  const bool halves = a->d == 256 && a->norm_nodes != ALIGNN_NORM_LAYER && g_backward_half.load();   // per-channel norms, d = 256
   switch (a->norm_nodes) {
     case ALIGNN_NORM_LAYER: LAUNCH_BWD_DST(ALIGNN_NORM_LAYER); break;
-    case ALIGNN_NORM_AFFINE:
-      if (halves) LAUNCH_BWD_DST_HALF(ALIGNN_NORM_AFFINE) else LAUNCH_BWD_DST(ALIGNN_NORM_AFFINE);
-      break;
-    default:
-      if (halves) LAUNCH_BWD_DST_HALF(ALIGNN_NORM_STATS) else LAUNCH_BWD_DST(ALIGNN_NORM_STATS);
-      break;
+    case ALIGNN_NORM_AFFINE: LAUNCH_BWD_DST(ALIGNN_NORM_AFFINE); break;
+    default: LAUNCH_BWD_DST(ALIGNN_NORM_STATS); break;
   }
-#undef LAUNCH_BWD_DST_HALF
 #undef LAUNCH_BWD_DST
   int rc = check_launch();
   if (rc != ALIGNN_OK) return rc;

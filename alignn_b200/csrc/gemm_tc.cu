@@ -8,13 +8,12 @@
 // A = edge features y, add0 = P[src, 0:d] (e_src), add1 = P[dst, 2d:3d] (e_dst + both biases) it is the pre-activation
 // gate  m = e_src[src] + e_dst[dst] + edge_gate(y)  of alignn/models/alignn.py:98-101 in ONE pass over y, plus the
 // per-channel batch statistics BatchNorm1d(m) needs (alignn.py:123).  With add0 = the incoming gradient it is the
-// data-gradient GEMM of the backward (residual in the epilogue); with bn_scale set, add1 rows are the pre-norm rows m of
-// the BatchNorm + SiLU that produced this GEMM's input gradient, and the statistics are sum gu, sum gu (m - mean).
+// data-gradient GEMM of the backward (residual in the epilogue).
 //
 // A is the fp32 activation matrix, streamed from HBM once; it is converted to bf16 hi/lo planes by the loader warps on
 // its way into shared memory (software-pipelined: the global loads of chunk k+1 are in flight while chunk k is
 // converted).  W is pre-split once per step into an image that already has the GMMA core-matrix order
-// (gemm_prepare_weights), so a K-chunk of it is ONE contiguous bulk copy (cp.async.bulk) signalled on the stage's
+// (gemm_prepare_table), so a K-chunk of it is ONE contiguous bulk copy (cp.async.bulk) signalled on the stage's
 // mbarrier.
 //
 // Persistent, warp-specialised CTA (one per SM), 128 x BN output tiles, BN <= 128: the 128 x BN fp32 accumulator lives
@@ -25,8 +24,7 @@
 // Epilogue: the wgmma fragment of one consumer warp is 16 whole rows of the tile, so each warp stages its own rows
 // through a private shared-memory tile (no block barrier) and then works row by row: a row is BN / 4 lanes with one
 // float4 each, the addend rows of several rows are loaded before the first store, and C is written as contiguous row
-// segments.  The addend rows are read through __restrict__ pointers: C must not overlap A, add0, add1, the bias or
-// the BatchNorm vectors.
+// segments.  The addend rows are read through __restrict__ pointers: C must not overlap A, add0, add1 or the bias.
 #include "common.cuh"
 #include "tc_common.cuh"
 #include "api_common.h"
@@ -78,7 +76,6 @@ struct Params {
   const float* add1; int64_t ld1; const int32_t* idx1;
   float* C; int64_t ldc;
   float* stats;                                          // [gridDim.x][2][N] or NULL (requires N <= kMaxStatN)
-  const float* bn_scale; const float* bn_shift; const float* bn_mean;
 };
 
 // byte offset of element (r, k) inside one chunk plane (rows x BK, core-matrix order)
@@ -95,13 +92,6 @@ __device__ __forceinline__ void a_coord(int i, int lt, int& row, int& kq) {
   kq = (u & 1) * 4 + (lane >> 4) * 2 + (lane & 1);
 }
 
-__device__ __forceinline__ float dsilu_(float u) {          // d/du [u * sigmoid(u)], same formula as egc_kernels.cu
-  float e, sg;                                             // 4-instruction sigmoid, as common.cuh's sigmoidf_
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(u * -1.4426950408889634f));
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(sg) : "f"(1.f + e));
-  return sg * (1.f + u * (1.f - sg));
-}
-
 __device__ __forceinline__ float4 ld4(const float* __restrict__ p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 __device__ __forceinline__ float4 ld4s(const float* p) {          // 4 scalars: vectors of any 4-byte alignment
   return p ? make_float4(__ldg(p), __ldg(p + 1), __ldg(p + 2), __ldg(p + 3)) : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -110,17 +100,16 @@ __device__ __forceinline__ float4 ld4s(const float* p) {          // 4 scalars: 
 // One consumer warp's WARP_ROWS rows of the tile, from its staged accumulator rows `stg` (row pitch Cfg::PITCH):
 //   C[r, col .. col + 3] = (acc + bias) + (add0[i0(r)] + add1[i1(r)]),   r = row0 + rw
 // i0 / i1 of row rw sit in lane rw (-1: no addend); col = n0 + 4 (lane % LPR).  s / q collect this lane's column
-// sums over its valid rows in row order (BatchNorm-backward mode: gu and gu (m - mean), see the kernel).
+// sums of C and C^2 over its valid rows in row order.
 template <int BN>
 __device__ __forceinline__ void epilogue_rows(const float* stg, float* __restrict__ C, int64_t ldc,
                                               const float* __restrict__ add0, int64_t ld0,
                                               const float* __restrict__ add1, int64_t ld1, int i0, int i1, int row0,
-                                              int M, int col, int lane, float4 b, bool bnmode, float4 sc, float4 sh,
-                                              float4 mu, float4& s, float4& q) {
+                                              int M, int col, int lane, float4 b, float4& s, float4& q) {
   using F = Cfg<BN>;
   const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
   const int lr = lane / F::LPR, c = (lane % F::LPR) * 4;
-#pragma unroll
+#pragma unroll 1   // unrolled, the row groups of BN = 128 spill at the 128-register cap
   for (int g0 = 0; g0 < F::ITERS; g0 += F::G) {
     float4 va[F::G], vb[F::G];
 #pragma unroll
@@ -135,25 +124,15 @@ __device__ __forceinline__ void epilogue_rows(const float* stg, float* __restric
       const int rw = (g0 + g) * F::RPI + lr;
       if (row0 + rw >= M) continue;
       const float4 a = *reinterpret_cast<const float4*>(stg + rw * F::PITCH + c);
-      const float4 a0 = va[g], m = vb[g], a1 = bnmode ? z4 : m;
+      const float4 a0 = va[g], a1 = vb[g];
       float4 o;
       o.x = (a.x + b.x) + (a0.x + a1.x);
       o.y = (a.y + b.y) + (a0.y + a1.y);
       o.z = (a.z + b.z) + (a0.z + a1.z);
       o.w = (a.w + b.w) + (a0.w + a1.w);
       *reinterpret_cast<float4*>(C + (int64_t)(row0 + rw) * ldc + col) = o;
-      if (bnmode) {
-        // gu = o * silu'(m * scale + shift); sums of gu and gu * (m - mean): the two reductions of the train-mode
-        // BatchNorm backward for the layer that consumes this gradient
-        const float gx = o.x * dsilu_(fmaf(m.x, sc.x, sh.x)), gy = o.y * dsilu_(fmaf(m.y, sc.y, sh.y));
-        const float gz = o.z * dsilu_(fmaf(m.z, sc.z, sh.z)), gw = o.w * dsilu_(fmaf(m.w, sc.w, sh.w));
-        s.x += gx; s.y += gy; s.z += gz; s.w += gw;
-        q.x = fmaf(gx, m.x - mu.x, q.x); q.y = fmaf(gy, m.y - mu.y, q.y);
-        q.z = fmaf(gz, m.z - mu.z, q.z); q.w = fmaf(gw, m.w - mu.w, q.w);
-      } else {
-        s.x += o.x; s.y += o.y; s.z += o.z; s.w += o.w;
-        q.x = fmaf(o.x, o.x, q.x); q.y = fmaf(o.y, o.y, q.y); q.z = fmaf(o.z, o.z, q.z); q.w = fmaf(o.w, o.w, q.w);
-      }
+      s.x += o.x; s.y += o.y; s.z += o.z; s.w += o.w;
+      q.x = fmaf(o.x, o.x, q.x); q.y = fmaf(o.y, o.y, q.y); q.z = fmaf(o.z, o.z, q.z); q.w = fmaf(o.w, o.w, q.w);
     }
   }
 }
@@ -259,7 +238,6 @@ gemm_bf16x3_kernel(const Params p) {
   // ================= consumers: MMA + epilogue =================
   const int wg = warp >> 2;                                  // rows 64 wg .. 64 wg + 63 of the tile
   const int wrow = wg * 64 + (warp & 3) * WARP_ROWS;         // this warp's fragment: tile rows wrow .. wrow + 15
-  const bool bnmode = p.bn_scale != nullptr;
   const bool do_stats = p.stats != nullptr;
   const int N = p.N;
   float* stg = reinterpret_cast<float*>(smem + F::PIPE_BYTES) + wrow * F::PITCH;   // this warp's staged rows
@@ -320,12 +298,8 @@ gemm_bf16x3_kernel(const Params p) {
     __syncwarp();
     const int col = n0 + (lane % F::LPR) * 4;
     const float4 b = ld4s(p.bias ? p.bias + col : nullptr);
-    float4 sc = make_float4(0.f, 0.f, 0.f, 0.f), sh = sc, mu = sc, s4 = sc, q4 = sc;
-    if (bnmode) {
-      sc = ld4s(p.bn_scale + col); sh = ld4s(p.bn_shift + col); mu = ld4s(p.bn_mean + col);
-    }
-    epilogue_rows<BN>(stg, p.C, p.ldc, p.add0, p.ld0, p.add1, p.ld1, i0, i1, m0 + wrow, M, col, lane, b, bnmode, sc, sh,
-                      mu, s4, q4);
+    float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f), q4 = s4;
+    epilogue_rows<BN>(stg, p.C, p.ldc, p.add0, p.ld0, p.add1, p.ld1, i0, i1, m0 + wrow, M, col, lane, b, s4, q4);
     if (do_stats) {
       // lanes lane % LPR hold the same columns for different rows: fold them, fixed order
 #pragma unroll
@@ -356,33 +330,8 @@ gemm_bf16x3_kernel(const Params p) {
   }
 }
 
-// W[N,K] fp32 (row stride ldw; or, if transpose, the N x K matrix is W^T of a [K,N] array) ->
-// image [N/BN tiles][K/32 chunks][hi, lo][BN x 32 bf16 in core-matrix order]
-template <int BN>
-__global__ void prepare_weights_kernel(const float* __restrict__ W, int N, int K, int64_t ldw, int transpose,
-                                       uint8_t* __restrict__ img) {
-  using F = Cfg<BN>;
-  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;     // one 8-element K group of one row
-  const int k8n = K / 8;
-  if (t >= (int64_t)N * k8n) return;
-  const int n = (int)(t / k8n), k8 = (int)(t % k8n);
-  float v[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const int k = k8 * 8 + j;
-    v[j] = transpose ? W[(int64_t)k * ldw + n] : W[(int64_t)n * ldw + k];
-  }
-  uint2 h0, l0, h1, l1;
-  tc::split4(make_float4(v[0], v[1], v[2], v[3]), h0, l0);
-  tc::split4(make_float4(v[4], v[5], v[6], v[7]), h1, l1);
-  const int nt = n / BN, r = n % BN, kc = k8 / (BK / 8), kk = k8 % (BK / 8);
-  const int64_t chunk = ((int64_t)nt * (K / BK) + kc) * 2 * F::B_PLANE;
-  const int off = plane_off(r, kk * 8);
-  *reinterpret_cast<uint4*>(img + chunk + off) = make_uint4(h0.x, h0.y, h1.x, h1.y);
-  *reinterpret_cast<uint4*>(img + chunk + F::B_PLANE + off) = make_uint4(l0.x, l0.y, l1.x, l1.y);
-}
-
-// Table-driven variant: every entry converts one source block into its place inside a (possibly larger) image, so
+// Weight images: W[N,K] fp32 (or W^T of a [K,N] array) -> [N/BN tiles][K/32 chunks][hi, lo][BN x 32 bf16 in
+// core-matrix order].  Every table entry converts one source block into its place inside a (possibly larger) image, so
 // all operand images of a model -- [W_sg; W_du; W_dg; W_su] stacked along N, its transpose stacked along K, the
 // edge gate and its transpose, the embedding Linears (K zero-padded) -- are refreshed by ONE launch per step.
 // blockIdx.y = entry; thread = one 8-element K group of one image row inside the entry's block.
@@ -466,22 +415,6 @@ size_t alignn_b200_gemm_weight_image_bytes(int N, int K) {
   return (size_t)N * K * 2 * 2;   // two bf16 planes
 }
 
-int alignn_b200_gemm_prepare_weights(const float* W, int N, int K, int64_t ldw, int transpose, void* image,
-                                     alignn_stream_t stream) {
-  using namespace alignn::gemm;
-  if (!W || !image || N <= 0 || K <= 0 || K % BK != 0) return ALIGNN_ERR_BAD_ARG;
-  const int bn = pick_bn(N);
-  if (bn == 0) return ALIGNN_ERR_UNSUPPORTED_D;
-  const int64_t total = (int64_t)N * (K / 8);
-  const int blocks = (int)((total + 255) / 256);
-  cudaStream_t st = (cudaStream_t)stream;
-  uint8_t* img = reinterpret_cast<uint8_t*>(image);
-  if (bn == 128) prepare_weights_kernel<128><<<blocks, 256, 0, st>>>(W, N, K, ldw, transpose, img);
-  else if (bn == 64) prepare_weights_kernel<64><<<blocks, 256, 0, st>>>(W, N, K, ldw, transpose, img);
-  else prepare_weights_kernel<32><<<blocks, 256, 0, st>>>(W, N, K, ldw, transpose, img);
-  return alignn::check_launch();
-}
-
 int alignn_b200_gemm_prepare_table(const alignn_b200_image_entry* entries, int n_entries, int64_t max_units,
                                    const alignn_b200_bias_entry* bias_entries, int n_bias, alignn_stream_t stream) {
   if (n_entries < 0 || n_bias < 0 || (n_entries > 0 && (!entries || max_units <= 0)) || (n_bias > 0 && !bias_entries))
@@ -544,7 +477,6 @@ int alignn_b200_gemm_gather(const alignn_b200_gemm_gather_args* a) {
   const int bn = pick_bn(a->N);
   if (bn == 0) return ALIGNN_ERR_UNSUPPORTED_D;
   if (a->stats && a->N > kMaxStatN) return ALIGNN_ERR_BAD_ARG;   // column partials of every warp live in shared memory
-  if (a->bn_scale && (!a->bn_shift || !a->bn_mean || !a->add1 || !a->stats)) return ALIGNN_ERR_BAD_ARG;
   Params p;
   p.A = a->A; p.lda = a->lda;
   p.M = (int)a->M; p.N = a->N; p.K = a->K;
@@ -553,7 +485,6 @@ int alignn_b200_gemm_gather(const alignn_b200_gemm_gather_args* a) {
   p.add0 = a->add0; p.ld0 = a->ld0; p.idx0 = a->idx0;
   p.add1 = a->add1; p.ld1 = a->ld1; p.idx1 = a->idx1;
   p.C = a->C; p.ldc = a->ldc; p.stats = a->stats;
-  p.bn_scale = a->bn_scale; p.bn_shift = a->bn_shift; p.bn_mean = a->bn_mean;
   const int total = ((p.M + BM - 1) / BM) * (p.N / bn);
   int grid = total < num_sms() ? total : num_sms();
   if (p.stats) grid = alignn_b200_gemm_gather_stat_rows(p.M, p.N);   // the caller sized `stats` for this many CTAs

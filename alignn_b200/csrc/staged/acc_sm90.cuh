@@ -94,7 +94,7 @@ __device__ __forceinline__ void mma_warpgroup(uint8_t* smem, uint64_t* full, uin
   }
 }
 
-// weight chunk kc of an image with D columns (gemm_prepare_weights layout, column tiles of BN) -> the stage's B region
+// weight chunk kc of an image with D columns (gemm_prepare_table layout, column tiles of BN) -> the stage's B region
 template <int D, int NK>
 __device__ __forceinline__ void copy_weight_chunk(uint8_t* dst, const uint8_t* wimg, int kc, uint64_t* bar) {
   constexpr int BN = D < 128 ? D : 128, WBP = BN * 32 * 2;

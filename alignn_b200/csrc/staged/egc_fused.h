@@ -36,7 +36,7 @@ typedef struct {
                               16-column chunks (row phase of one overlaps the column phase of the other) */
   float gate_eps, ln_eps;
   const float* y;        /* [Ne,d] edge features = A operand of the gate GEMM */
-  const void* w_image;   /* alignn_b200_gemm_prepare_weights(W_eg, N=d, K=d) */
+  const void* w_image;   /* image of W_eg (alignn_b200_gemm_prepare_table, N=d, K=d) */
   const float* bias;     /* [d] edge_gate.bias */
   const float* P;        /* [Nn,4d] node projections [e_src | Bh | e_dst | src_update] */
   const int32_t* src; const int32_t* dst;
@@ -84,7 +84,7 @@ typedef struct {
   int32_t residual;
   const float* M; const float* gy_out;
   const float* P; const float* GSh; const float* GS;
-  const void* w_image;   /* alignn_b200_gemm_prepare_weights(W_eg, N=d, K=d, transpose=1) */
+  const void* w_image;   /* image of W_eg^T (alignn_b200_gemm_prepare_table, N=d, K=d, transpose=1) */
   const int32_t* src; const int32_t* dst; const int32_t* in_ptr; const int32_t* in_eid;
   const int32_t* tiles; int32_t num_tiles;
   const float* e_w; const float* e_b; const float* e_mean; const float* e_rstd; const float* e_c1; const float* e_c2;

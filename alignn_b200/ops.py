@@ -7,7 +7,6 @@ from __future__ import annotations
 
 import ctypes as C
 import functools
-import os
 import weakref
 from typing import Optional, Tuple
 
@@ -177,44 +176,6 @@ def colsum(a: torch.Tensor, alpha: float = 1.0) -> torch.Tensor:
     return out
 
 
-class BNLink:
-    """Travels (as a Python attribute) on the OUTPUT tensor of a train-mode `BatchNorm1d -> SiLU (+ residual)` stage to
-    the Linear that consumes it.  That Linear's data-gradient GEMM produces exactly the gradient the BatchNorm backward
-    has to reduce first (c1 = mean gu, c2 = mean gu*xhat), so its epilogue accumulates those sums on the way out
-    (`gemm_gather(bn_aux=...)`) and leaves them here; the producing stage's backward then skips its own reduction pass
-    over the two [rows, d] tensors.  The producer only trusts the sums if the gradient it receives is the very tensor
-    that GEMM wrote (`grad_ptr`): if autograd summed several consumers it falls back to `bn_backward_reduce`."""
-    __slots__ = ("rows", "scale", "shift", "mean", "rstd", "n", "partials", "grad_ptr")
-
-    def __init__(self, rows, scale, shift, mean, rstd, n):
-        self.rows, self.scale, self.shift, self.mean, self.rstd, self.n = rows, scale, shift, mean, rstd, int(n)
-        self.partials = None
-        self.grad_ptr = None
-
-    def usable_for(self, x: torch.Tensor) -> bool:
-        return self.rows is not None and tuple(self.rows.shape) == tuple(x.shape) and self.rows.device == x.device
-
-    def take(self, g_out: torch.Tensor):
-        """(c1, c2) if the consumer's GEMM left sums for exactly this gradient tensor, else None."""
-        part, self.partials = self.partials, None
-        if part is None or g_out is None or g_out.data_ptr() != self.grad_ptr:
-            return None
-        return bn_backward_finish(part, self.n, self.rstd)
-
-
-# The data-gradient GEMM can also produce the two BatchNorm-backward reductions in its epilogue instead of a separate
-# reduction pass.  Off by default (not measured on H100); kept for A/B runs.
-USE_BN_LINKS = os.environ.get("ALIGNN_B200_BN_LINKS", "0") == "1"
-
-
-def bn_backward_finish(partials: torch.Tensor, n: int, rstd: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
-    """(c1, c2) from the partial sums a `gemm_gather(..., bn_aux=...)` epilogue produced:
-    c1 = sum(gu) / n,  c2 = rstd * sum(gu * (m - mean)) / n."""
-    rows, two, d = partials.shape
-    c = colsum(partials.view(rows, 2 * d), 1.0 / n)
-    return c[:d], c[d:] * rstd
-
-
 @_on_tensor_device
 def bn_backward_reduce(R, g_out, scale, shift, mean, rstd) -> Tuple[torch.Tensor, torch.Tensor]:
     """c1 = mean(gu), c2 = mean(gu*xhat) per channel (BatchNorm train-mode backward, pass 1)."""
@@ -362,17 +323,14 @@ class WeightImage:
     __slots__ = ("buf", "N", "K")
 
     def __init__(self, W: torch.Tensor, transpose: bool = False):
-        lib = _lib.load()
         require_cuda(W)
         if W.dim() != 2:
             raise RuntimeError("WeightImage needs a 2-D weight")
         self.N, self.K = (W.shape[1], W.shape[0]) if transpose else (W.shape[0], W.shape[1])
-        nbytes = int(lib.alignn_b200_gemm_weight_image_bytes(self.N, self.K))
-        if nbytes == 0:
-            raise RuntimeError(f"alignn_b200 GEMM: unsupported weight shape N={self.N}, K={self.K} (need multiples of 32)")
-        self.buf = torch.empty(nbytes, device=W.device, dtype=torch.uint8)
-        _lib.check(lib.alignn_b200_gemm_prepare_weights(ptr(W), self.N, self.K, W.stride(0), int(transpose), ptr_any(self.buf),
-                                                        stream_ptr()), "alignn_b200_gemm_prepare_weights")
+        tbl = ImageTable()
+        tbl.add_image("w", self.N, self.K, [(W, transpose, 0, 0)], W.device)
+        tbl.refresh()
+        self.buf = tbl.images["w"].buf
 
 
 class _Img:
@@ -530,15 +488,12 @@ def gemm_nt(A: torch.Tensor, w: WeightImage, bias: Optional[torch.Tensor] = None
 def gemm_gather(A: torch.Tensor, w: WeightImage, bias: Optional[torch.Tensor] = None, *,
                 add0: Optional[torch.Tensor] = None, idx0: Optional[torch.Tensor] = None,
                 add1: Optional[torch.Tensor] = None, idx1: Optional[torch.Tensor] = None,
-                stats: bool = False, out: Optional[torch.Tensor] = None, bn_aux=None):
+                stats: bool = False, out: Optional[torch.Tensor] = None):
     """out[r] = A[r] @ W^T (+ bias) (+ add0[idx0[r]]) (+ add1[idx1[r]]) on wgmma.
 
     add0 / add1 are 2-D fp32 views with unit column stride and w.N columns (column slices of a wider matrix are fine);
     idx None = identity (a residual).  stats=True also returns the per-CTA partial column sums [rows, 2, N] of out and
-    out^2 (alignn.py:123 batch statistics; feed `bn_finalize(partials, 0, M, ...)`).
-    bn_aux = (m_rows [M,N], scale, shift, mean): `out` is the gradient w.r.t. the output of a train-mode
-    BatchNorm1d + SiLU whose pre-norm rows are m_rows; returns (out, partials [rows,2,N]) with the partial sums of
-    gu = out * silu'(m*scale+shift) and gu * (m - mean) (feed `bn_backward_finish`)."""
+    out^2 (alignn.py:123 batch statistics; feed `bn_finalize(partials, 0, M, ...)`)."""
     lib = _lib.load()
     if A.dim() != 2 or A.stride(1) != 1 or A.shape[1] != w.K:
         raise RuntimeError(f"gemm_gather: A must be [M,{w.K}] with unit column stride, got {tuple(A.shape)}/{A.stride()}")
@@ -560,16 +515,6 @@ def gemm_gather(A: torch.Tensor, w: WeightImage, bias: Optional[torch.Tensor] = 
     if out is None:
         out = torch.empty(M, w.N, device=A.device, dtype=torch.float32)
     part = None
-    bn_ptrs = (None, None, None)
-    if bn_aux is not None:
-        if add1 is not None or stats:
-            raise RuntimeError("gemm_gather: bn_aux excludes add1 / stats")
-        add1, sc, sh, mu = bn_aux
-        if add1.shape != (M, w.N) or add1.stride(1) != 1:
-            raise RuntimeError("gemm_gather: bn_aux rows must be [M, N]")
-        require_cuda(sc, sh, mu)
-        bn_ptrs = (ptr(sc), ptr(sh), ptr(mu))
-        stats = True
     if stats:
         rows = int(lib.alignn_b200_gemm_gather_stat_rows(M, w.N))
         part = torch.empty(max(rows, 1), 2, w.N, device=A.device, dtype=torch.float32)
@@ -578,12 +523,9 @@ def gemm_gather(A: torch.Tensor, w: WeightImage, bias: Optional[torch.Tensor] = 
         w_image=ptr_any(w.buf), bias=ptr_any(bias),
         add0=ptr_any(add0), ld0=add0.stride(0) if add0 is not None else 0, idx0=ptr_any(idx0),
         add1=ptr_any(add1), ld1=add1.stride(0) if add1 is not None else 0, idx1=ptr_any(idx1),
-        C=ptr_any(out), ldc=out.stride(0), stats=ptr_any(part), bn_scale=bn_ptrs[0], bn_shift=bn_ptrs[1], bn_mean=bn_ptrs[2],
-        stream=stream_ptr())
-    nb = 4 * M * (w.K + w.N) + (8 * M if idx0 is not None else 0) + (4 * M * w.N if bn_aux is not None else 0) + (4 * M * w.N if (add0 is not None and idx0 is None) else 0)
+        C=ptr_any(out), ldc=out.stride(0), stats=ptr_any(part), stream=stream_ptr())
+    nb = 4 * M * (w.K + w.N) + (8 * M if idx0 is not None else 0) + (4 * M * w.N if (add0 is not None and idx0 is None) else 0)
     kind = "+gather" if idx0 is not None else ("+residual" if add0 is not None else "")
-    if bn_aux is not None:
-        kind += "+bn_bwd"
     with _span(f"gemm_gather<{min(w.N, 256)}>" + kind + ("+stats" if stats else ""), nb):
         _lib.check(lib.alignn_b200_gemm_gather(C.byref(a)), "alignn_b200_gemm_gather")
     return (out, part) if stats else out
@@ -812,7 +754,6 @@ class _MLPBNTrainFn(torch.autograd.Function):
             bn.num_batches_tracked.add_(1)
         out = affine_silu_residual(R, None, scale, shift)
         ctx.save_for_backward(x, R, scale, shift, mean, rstd)
-        ctx.link = BNLink(R, scale, shift, mean, rstd, n) if USE_BN_LINKS else None
         ctx.tbl = tbl
         ctx.k_in = weight.shape[1]
         return out
@@ -824,8 +765,7 @@ class _MLPBNTrainFn(torch.autograd.Function):
         x, R, scale, shift, mean, rstd = ctx.saved_tensors
         go = go.contiguous()
         n, d = R.shape
-        got = ctx.link.take(go) if ctx.link is not None else None     # sums left by the consumer's data-gradient GEMM
-        c1, c2 = got if got is not None else bn_backward_reduce(R, go, scale, shift, mean, rstd)
+        c1, c2 = bn_backward_reduce(R, go, scale, shift, mean, rstd)
         gR = torch.empty_like(R)
         with _span("bn_backward_apply", 12 * n * d):
             _lib.check(lib.alignn_b200_bn_backward_apply(ptr(R), ptr(go), ptr(scale), ptr(shift), ptr(mean), ptr(rstd),
@@ -901,7 +841,4 @@ def mlp_ln(x, lin, ln):
 def mlp_bn_train(x, lin, bn):
     tbl = linear_table(lin)
     tbl.refresh()
-    out = _MLPBNTrainFn.apply(x, lin.weight, lin.bias, bn.weight, bn.bias, bn, tbl)
-    if out.grad_fn is not None and getattr(out.grad_fn, "link", None) is not None:
-        out._alignn_b200_bn_link = out.grad_fn.link
-    return out
+    return _MLPBNTrainFn.apply(x, lin.weight, lin.bias, bn.weight, bn.bias, bn, tbl)

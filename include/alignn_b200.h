@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define ALIGNN_B200_VERSION 100
+#define ALIGNN_B200_VERSION 101
 
 typedef enum {
   ALIGNN_OK = 0,
@@ -239,14 +239,12 @@ int alignn_b200_gather_segment_sum(const float* Bh, const float* sigma, const in
  * registers; results agree with an fp32 GEMM to ~1e-5 relative):
  *     C[M,N] = A[M,K] * W[N,K]^T (+ bias[N]) (+ R[M,N])
  * Replaces the nn.Linear call sites alignn.py:98,99,101,104,110 (forward) and their data-gradient
- * GEMMs.  W is first converted once per step to a bf16 hi/lo image (`gemm_prepare_weights`;
+ * GEMMs.  W is first converted once per step to a bf16 hi/lo image (`gemm_prepare_table`;
  * `transpose != 0` takes W^T of a [K,N] array, which is what the data-gradient GEMMs need).
  * Constraints: K % 32 == 0, N % 32 == 0, lda/ldc/ldr % 4 == 0 and A, R, C 16-byte aligned (16-byte rows).
  * C must not overlap A, R or bias: the epilogue reads the addends while other rows of C are being written.
  * ---------------------------------------------------------------------------------------- */
 size_t alignn_b200_gemm_weight_image_bytes(int N, int K);   /* 0 if the shape is unsupported */
-int alignn_b200_gemm_prepare_weights(const float* W, int N, int K, int64_t ldw, int transpose, void* image,
-                                     alignn_stream_t stream);
 /* Table-driven refresh of many operand images in one launch (+ one for the bias vectors).  Every entry converts one
  * source block W[rows, cols] (row stride ldw; transpose != 0: the block enters as its transpose) into the image of an
  * [N, K] operand at row offset n_off / column offset k_off (k_off % 8 == 0; blocks narrower than a multiple of 8 are
@@ -278,9 +276,9 @@ int alignn_b200_gemm_nt(const float* A, int64_t lda, const void* w_image, int64_
  * BatchNorm1d(m) in one pass over y -- apply_edges(u_add_v) and the Linear fused, no [Ne,d] temporary.
  * With add0 = R, idx0 = NULL it is the data-gradient GEMM with its residual; without addends a plain Linear.
  * A is streamed row by row (row stride lda floats, 16-byte aligned rows); W is an image from
- * alignn_b200_gemm_prepare_weights.  Constraints: K % 32 == 0, N % 32 == 0, lda/ldc/ld0/ld1 % 4 == 0.
- * C must not overlap A, add0, add1, bias, the BatchNorm vectors or stats: the epilogue reads the addends while other
- * rows of C are being written.
+ * alignn_b200_gemm_prepare_table.  Constraints: K % 32 == 0, N % 32 == 0, lda/ldc/ld0/ld1 % 4 == 0.
+ * C must not overlap A, add0, add1, bias or stats: the epilogue reads the addends while other rows of C are being
+ * written.
  * ---------------------------------------------------------------------------------------- */
 typedef struct {
   size_t struct_size;
@@ -292,12 +290,6 @@ typedef struct {
   const float* add1; int64_t ld1; const int32_t* idx1;
   float* C; int64_t ldc;
   float* stats;                                             /* [stat_rows][2][N] or NULL */
-  /* BatchNorm-backward mode (all three != NULL; needs add1 and stats): the rows add1[i1(r)] are NOT added -- they are
-   * the pre-norm rows m of the train-mode BatchNorm1d + SiLU whose output gradient this GEMM produces (C = dL/d(out)),
-   * bn_scale / bn_shift / bn_mean [N] its batch scale, shift and mean; stats then holds the partial sums of
-   * gu = C * silu'(m * scale + shift) and gu * (m - mean): the two reductions of that BatchNorm's backward
-   * (alignn_b200_bn_backward_reduce) without another pass over C and m. */
-  const float* bn_scale; const float* bn_shift; const float* bn_mean;
   alignn_stream_t stream;
 } alignn_b200_gemm_gather_args;
 
@@ -421,7 +413,7 @@ int alignn_b200_segment_mean_backward(const float* g_out /*[B,d]*/, const int32_
 /* ------------------------------------------------------------------------------------------
  * Development aids (A/B switches and tracing used by tools/; not needed by a caller of the path).
  * ---------------------------------------------------------------------------------------- */
-void alignn_b200_debug_egc_flags(int flags);                /* bit 0: register-staged pass 2 instead of the ring; bit 1: channel-half egc_backward_dst (d = 256, BatchNorm) instead of the full-row kernel */
+void alignn_b200_debug_egc_flags(int flags);                /* bit 0: register-staged pass 2 instead of the ring */
 
 #ifdef __cplusplus
 }

@@ -480,35 +480,3 @@ def test_force_reduction_properties_on_the_cuda_path():
         by_bond[d[e]] += pf[e]
         by_bond[s[e]] -= pf[e]
     assert float((f - by_bond).abs().max()) <= 1e-5 * scale
-
-
-def test_bn_links_move_the_batchnorm_backward_reductions_into_the_gemm_epilogue():
-    """(Optional path, off by default: measured slower, see ops.USE_BN_LINKS.)  With ops.BNLink the T-sized reductions of the train-mode BatchNorm backward (one per L(g) conv that has a
-    consumer, plus the angle embedding's last layer) ride on the consumer's data-gradient GEMM; results equal the
-    explicit reduction pass to fp32 round-off."""
-    g, lg, lat, tgt = synthetic.make_batch(batch_size=4, atoms=10, k=12, seed=9)
-    gd, lgd, latd, tgtd = g.to(DEV), lg.to(DEV), lat.to(DEV), tgt.to(DEV)
-
-    def run(use_links):
-        ops.USE_BN_LINKS = use_links
-        m = ALIGNN(ALIGNNConfig(name="alignn", alignn_layers=3, gcn_layers=1, hidden_features=64, embedding_features=32))
-        GI.fill_state_dict(m, 21)
-        m.to(DEV).train()
-        ops.TIMER = ops.KernelTimer()
-        (m((gd, lgd, latd)) - tgtd).abs().mean().backward()
-        torch.cuda.synchronize()
-        names = {k: len(v) for k, v in ops.TIMER.records.items()}
-        ops.TIMER = None
-        return {n: p.grad.clone() for n, p in m.named_parameters() if p.grad is not None}, names
-    try:
-        g_on, n_on = run(True)
-        g_off, n_off = run(False)
-    finally:
-        ops.USE_BN_LINKS = False
-        ops.TIMER = None
-    fused = sum(v for k, v in n_on.items() if "bn_bwd" in k)
-    assert fused >= 3                                   # L(g) convs 1, 2 -> 0, 1 and layer 0 -> angle embedding (+ g-side links)
-    assert n_on.get("bn_backward_reduce", 0) <= n_off["bn_backward_reduce"] - fused
-    for k in g_off:
-        scale = max(g_off[k].abs().max().item(), 1e-12)
-        assert (g_on[k] - g_off[k]).abs().max().item() <= 2e-5 * scale + 1e-7, k

@@ -222,47 +222,3 @@ def test_kernels_follow_the_tensors_device_not_the_current_device():
         torch.cuda.synchronize(dev)
         outs.append(red.flat.cpu())
     assert torch.equal(outs[0], outs[1])
-
-
-@pytest.mark.parametrize("mode", ["bn_train", "bn_eval"])
-@pytest.mark.parametrize("edge_out", [True, False])
-def test_channel_half_backward_matches_full_row_backward(mode, edge_out):
-    """egc_backward_dst_half_kernel (d = 256, per-channel norms) against egc_backward_dst_kernel: GM and GP bit-identical,
-    the parameter-gradient sums equal up to the order of the per-warp additions."""
-    from alignn_b200._lib import NORM_AFFINE, NORM_STATS
-    from alignn_b200.graph import Graph
-    lib = _lib.load()
-    d = 256
-    gen = torch.Generator(device="cpu").manual_seed(11)
-    Nn = 700
-    deg = torch.randint(0, 14, (Nn,), generator=gen)
-    deg[3] = 75                                                   # more than one 32-edge chunk
-    deg[0] = 0
-    dst = torch.repeat_interleave(torch.arange(Nn), deg)
-    for sort in (True, False):
-        if not sort:
-            dst = dst[torch.randperm(dst.numel(), generator=gen)]
-        src = torch.randint(0, Nn, (dst.numel(),), generator=gen)
-        gr = Graph(src.numpy(), dst.numpy(), Nn).to(DEV)
-        ix = gr.index
-        Ne = dst.numel()
-        rnd = lambda *s: torch.randn(*s, generator=gen).to(DEV)  # noqa: E731
-        P, M, XP, H = rnd(Nn, 4 * d), rnd(Ne, d), rnd(Nn, d), rnd(Nn, d)
-        S = (torch.rand(Nn, d, generator=gen) * 5).to(DEV)
-        gx_out, gy_out = rnd(Nn, d), (rnd(Ne, d) if edge_out else None)
-        vec = lambda: {"w": (torch.rand(d, generator=gen) + 0.5).to(DEV), "b": rnd(d), "mean": rnd(d),  # noqa: E731
-                       "rstd": (torch.rand(d, generator=gen) + 0.5).to(DEV), "c1": rnd(d) * 0.1, "c2": rnd(d) * 0.1}
-        n, e = vec(), vec()
-        norm = NORM_STATS if mode == "bn_train" else NORM_AFFINE
-        res = {}
-        try:
-            for flag in (0, 2):                                     # 0: full-row kernel (default), 2: channel halves (opt-in)
-                lib.alignn_b200_debug_egc_flags(flag)
-                res[flag] = ops.egc_backward(ix, P, M, XP, S, H, gx_out, gy_out, n, e, norm_nodes=norm, norm_edges=norm)
-        finally:
-            lib.alignn_b200_debug_egc_flags(0)
-        (GM0, GP0, vd0, vs0), (GM1, GP1, vd1, vs1) = res[0], res[2]
-        assert torch.equal(GM0, GM1) and torch.equal(GP0, GP1)
-        assert torch.equal(vs0, vs1)
-        scale = vd0.abs().max().item()
-        assert (vd0 - vd1).abs().max().item() <= 2e-6 * scale

@@ -113,7 +113,7 @@ def test_library_exports_every_declared_symbol():
     nm = subprocess.check_output(["nm", "-D", "--defined-only", _lib.LIB_PATH], text=True)
     exported = {ln.split()[-1] for ln in nm.splitlines() if ln.split() and ln.split()[-1].startswith("alignn_b200_")}
     assert exported == declared, exported ^ declared
-    assert lib.alignn_b200_version() == 100
+    assert lib.alignn_b200_version() == 101
     assert lib.alignn_b200_strerror(-2).decode().startswith("unsupported feature width")
     assert lib.alignn_b200_egc_partial_rows(1920, 256) == 240
     assert lib.alignn_b200_egc_partial_rows(10 ** 7, 256) == 132 * 4

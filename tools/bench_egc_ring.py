@@ -53,21 +53,5 @@ for name, nn_, ne_, save in (("bn_train", NORM_STATS, NORM_AFFINE, True), ("laye
     same = all((res["ring"][1][k] is None and res["registers"][1][k] is None) or torch.equal(res["ring"][1][k], res["registers"][1][k])
                for k in ("x_out", "y_out", "XP", "S", "H", "partials"))
     out["forward_" + name] = {"us_registers": res["registers"][0], "us_ring": res["ring"][0], "bit_identical": bool(same)}
-# backward, destination-keyed + source-keyed pass: full-row kernel vs channel-half kernel (per-channel norms only)
-M, XP, H = rnd(Ne, d), rnd(Nn, d), rnd(Nn, d)
-S = (torch.rand(Nn, d, generator=gen) * 5).to(dev)
-gx_out, gy_out = rnd(Nn, d), rnd(Ne, d)
-mk = lambda: {"w": vec[0], "b": vec[1], "mean": vec[2], "rstd": vec[3], "c1": vec[0] * 0.01, "c2": vec[1] * 0.01}  # noqa: E731
-for name, norm in (("bn_train", NORM_STATS), ("bn_eval", NORM_AFFINE)):
-    def bwd():
-        return ops.egc_backward(ix, P, M, XP, S, H, gx_out, gy_out, mk(), mk(), norm_nodes=norm, norm_edges=norm)
-    res = {}
-    for flag, tag in ((0, "full_row"), (2, "channel_half")):
-        lib.alignn_b200_debug_egc_flags(flag)
-        r = bwd()
-        res[tag] = (timeit(bwd), r)
-    same = torch.equal(res["full_row"][1][0], res["channel_half"][1][0]) and torch.equal(res["full_row"][1][1], res["channel_half"][1][1])
-    out["backward_dst_plus_src_" + name] = {"us_full_row": res["full_row"][0], "us_channel_half": res["channel_half"][0],
-                                             "GM_GP_bit_identical": bool(same)}
 lib.alignn_b200_debug_egc_flags(0)
 print(json.dumps(out))

@@ -8,7 +8,7 @@ runs with ops.gemm_nt / ops.gemm_gather wrapped, and every distinct call (kernel
 M, N, K, addends) is kept with its real arguments.  Each is then replayed from a CUDA graph of back-to-back launches
 (no host launch cost in the window) for at least --seconds of GPU time, timed with CUDA events.
 
-Per shape it prints ms per launch; compulsory bytes (A, C, identity addends and the bn_aux rows once each, gathered
+Per shape it prints ms per launch; compulsory bytes (A, C and identity addends once each, gathered
 tables and their indices once, the weight image) and GB/s; bf16 work (three bf16 products per fp32 product) and
 TFLOP/s; and the share of the larger of the two floors at the H100 SXM data-sheet rates (3.35 TB/s HBM3, 989 TFLOP/s
 dense BF16), with which floor it is.  The device name, power limit and SM clock limit are read in the same run.
@@ -62,7 +62,7 @@ def record_calls(args):
                 kind = ("+gather" if kw.get("idx0") is not None else ("+residual" if kw.get("add0") is not None else ""))
                 if kw.get("add1") is not None:
                     kind += "+add1" + ("[idx]" if kw.get("idx1") is not None else "")
-                kind += ("+bn_bwd" if kw.get("bn_aux") is not None else "") + ("+stats" if kw.get("stats") else "")
+                kind += "+stats" if kw.get("stats") else ""
             key = (f"{name}<{min(w.N, 256)}>{kind}", A.shape[0], w.N, w.K)
             if key in calls:
                 calls[key][4] += 1
@@ -95,8 +95,6 @@ def compulsory_bytes(fn_name, call_args, kw, M, N, K):
         if t is None:
             continue
         b += 4 * M * N if ix is None else 4 * t.shape[0] * N + 4 * M   # a gathered table is read once, plus its index
-    if kw.get("bn_aux") is not None:
-        b += 4 * M * N + 3 * 4 * N
     return b
 
 
