@@ -56,6 +56,23 @@ class EgcBwdArgs(C.Structure):
     ]
 
 
+class EgcBwdVjpArgs(C.Structure):
+    _fields_ = [
+        ("struct_size", C.c_size_t),
+        ("Nn", C.c_int64), ("Ne", C.c_int64),
+        ("d", C.c_int32), ("norm", C.c_int32),
+        ("gate_eps", C.c_float), ("ln_eps", C.c_float),
+        ("P", _fp), ("M", _fp), ("XP", _fp), ("S", _fp), ("H", _fp),
+        ("src", _fp), ("dst", _fp), ("in_ptr", _fp), ("in_eid", _fp), ("out_ptr", _fp), ("out_eid", _fp),
+        ("n_w", _fp), ("n_b", _fp), ("e_w", _fp), ("e_b", _fp),
+        ("gx_out", _fp), ("gy_out", _fp), ("GSh", _fp),
+        ("GPbar", _fp), ("GMbar", _fp), ("gx_bar_res", _fp), ("gy_bar_res", _fp),
+        ("Pbar", _fp), ("Mbar", _fp), ("gx_out_bar", _fp), ("gy_out_bar", _fp), ("Gamma", _fp), ("Shbar", _fp),
+        ("partials", _fp), ("partials_src", _fp),
+        ("stream", _fp),
+    ]
+
+
 class GemmGatherArgs(C.Structure):
     _fields_ = [
         ("struct_size", C.c_size_t),
@@ -99,6 +116,7 @@ _SIGNATURES = {
                                           C.c_float, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
     "alignn_b200_affine_silu_residual": (C.c_int, [_fp, _fp, _fp, _fp, _fp, C.c_int64, C.c_int, _fp]),
     "alignn_b200_egc_backward": (C.c_int, [C.POINTER(EgcBwdArgs)]),
+    "alignn_b200_egc_backward_vjp": (C.c_int, [C.POINTER(EgcBwdVjpArgs)]),
     "alignn_b200_bn_backward_reduce": (C.c_int, [_fp, _fp, _fp, _fp, _fp, _fp, C.c_int64, C.c_int, _fp, C.c_int, _fp]),
     "alignn_b200_rowstats_partials": (C.c_int, [_fp, C.c_int64, C.c_int, _fp, C.c_int, _fp]),
     "alignn_b200_bn_backward_apply": (C.c_int, [_fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, C.c_int64, C.c_int, _fp, _fp]),

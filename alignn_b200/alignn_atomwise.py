@@ -5,8 +5,6 @@
 """
 from __future__ import annotations
 
-import contextlib
-
 from torch import nn
 
 from .conv import ALIGNNConvBase, EdgeGatedGraphConvBase, second_order
@@ -128,8 +126,9 @@ class ALIGNNAtomWise(nn.Module):
     (alignn/models/alignn_atomwise.py:249-660, BASELINE config 4).
 
     Same constructor/`forward((g, lg, lat))`/result-dict surface and state_dict names as the reference.
-    Forces use first-order autograd only (`create_graph=False`): the conv's autograd Function is
-    once-differentiable, so FF *training* on forces (double backward, :536) is not available.
+    Forces come from autograd through the conv stack.  In training with a force or stress loss the force pass keeps the
+    graph (`create_graph=True`, :530-539) and the loss's backward runs the convs' double backward on the CUDA kernels
+    (alignn_b200_egc_backward_vjp); the embedding MLPs, pooling and force / virial reductions are torch operators there.
     Stress: the batched virial of :610-638 (`batch_stress=True`, the default) from the same pair forces.
     Cutoff envelope on the bond lengths (`use_cutoff_function`, both `multiply_cutoff` settings, :434-451).
     Not built (SURVEY.md section 8f): `batch_stress=False` (:573-590), include_pos_deriv.
@@ -170,9 +169,10 @@ class ALIGNNAtomWise(nn.Module):
 
     def forward(self, g):
         c = self.config
-        # Force / stress TRAINING differentiates through the force computation (create_graph=True, :530-539): the convs
-        # then run as differentiable torch-operator compositions (conv.second_order); inference, MD and property-only
-        # training use the once-differentiable CUDA kernels.
+        # Force / stress TRAINING differentiates through the force computation (create_graph=True, :530-539): the MLP
+        # embeddings and the pooling then run as differentiable torch operators (conv.second_order) while the LayerNorm
+        # convs keep the CUDA kernels, whose backward is differentiable once more; inference, MD and property-only
+        # training use the first-order kernels throughout.
         second = bool(self.training and torch.is_grad_enabled() and c.calculate_gradient
                       and (c.gradwise_weight != 0 or c.stresswise_weight != 0))
         if second:
@@ -237,8 +237,9 @@ class ALIGNNAtomWise(nn.Module):
                 # lands in result["out"] (SURVEY App. D-12); reproduced, not fixed
                 out = en_out
         if c.calculate_gradient:
-            # first order: only d energy / d r leaves this call, so the kernels skip every parameter gradient
-            with (contextlib.nullcontext() if second else ops.input_grads_only()):
+            # only d energy / d r leaves this call, so the kernels skip every parameter gradient (in force training the
+            # parameter gradients come from the loss's backward through this graph)
+            with ops.input_grads_only():
                 (dr,) = torch.autograd.grad(en_out, r, grad_outputs=torch.ones_like(en_out),
                                             create_graph=second, retain_graph=second or self.training)
             pair_forces = c.grad_multiplier * dr                         # (:530-539)

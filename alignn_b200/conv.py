@@ -28,11 +28,11 @@ GATE_EPS = 1e-6   # alignn.py:109
 
 
 class second_order:
-    """Context manager: run the convs as a composition of differentiable torch operators (ATen kernels on the same
-    device) instead of the once-differentiable CUDA Function.  Needed only where the reference differentiates through
-    its own backward -- force / stress training, `torch.autograd.grad(..., create_graph=True)` at
-    alignn/models/alignn_atomwise.py:530-539 (SURVEY.md section 8b "autograd contract").  Slower: every
-    intermediate is materialised, as in the reference."""
+    """Context manager for code that differentiates through its own backward -- force / stress training,
+    `torch.autograd.grad(..., create_graph=True)` at alignn/models/alignn_atomwise.py:530-539 (SURVEY.md section 8b
+    "autograd contract").  BatchNorm convs (and the embedding MLPs, alignn.mlp_forward) then run as compositions of
+    differentiable torch operators; LayerNorm convs keep the CUDA Function, whose backward is differentiable once more
+    (_EdgeGatedConvBackwardFn)."""
     active = False
 
     def __enter__(self):
@@ -159,80 +159,160 @@ class _EdgeGatedConvFn(torch.autograd.Function):
         return x_out, y_out
 
     @staticmethod
-    @once_differentiable
     def backward(ctx, gx_out, gy_out):
-        cfg = ctx.cfg
-        x, y, P, M, XP, S, H, nw, nb, ew, eb = ctx.saved_tensors
-        img_catT, img_egT = cfg.images.images["catT"], cfg.images.images["egT"]
-        d = x.shape[1]
-        gx_out = gx_out.contiguous()
-        gy_out = None if (ctx.y_dead or gy_out is None) else gy_out.contiguous()
-        if cfg.norm_nodes == NORM_LAYER:
-            n = dict(w=nw.contiguous(), b=nb.contiguous())
-            e = dict(w=ew.contiguous(), b=eb.contiguous())
-        else:
-            sc, sh, mu, rs = cfg.n_aux
-            n = dict(w=sc, b=sh, mean=mu, rstd=rs)
-            e = {}
-            if cfg.e_aux is not None:
-                sc, sh, mu, rs = cfg.e_aux
-                e = dict(w=sc, b=sh, mean=mu, rstd=rs)
-            if cfg.norm_nodes == NORM_STATS:
-                n["c1"], n["c2"] = ops.bn_backward_reduce(XP, gx_out, n["w"], n["b"], n["mean"], n["rstd"])
-                if gy_out is not None:
-                    e["c1"], e["c2"] = ops.bn_backward_reduce(M, gy_out, e["w"], e["b"], e["mean"], e["rstd"])
-        # Parameter gradients are off the critical path of backward.  With a queue installed (FlatGradAllReducer.deferring())
-        # the five weight-gradient GEMMs and the nine bias / norm-parameter reductions of this conv are only registered
-        # here and computed by two batched launches at the end of backward, straight into the flat gradient buffer.
-        params = not ops.input_grads_only.active                # a forces-only backward discards every parameter gradient
-        queue = ops.WgradQueue.current
-        W_sg, W_dg, W_eg, W_su, W_du = ctx.weights
-        b_sg, b_dg, b_eg, b_su, b_du = ctx.biases
-        vec_needed = [b_sg, b_dg, b_eg, b_su, b_du, nw, nb] + ([ew, eb] if gy_out is not None else [])
-        deferred = params and queue is not None and ops.wgrad_supported(d, d) and queue.wants(W_sg, W_du, W_dg, W_su, W_eg) \
-            and queue.wants_vecs(*vec_needed)
-        GM, GP, vd, vs = ops.egc_backward(cfg.index, P, M, XP, S, H, gx_out, gy_out, n, e, reduce=params and not deferred,
-                                          norm_nodes=cfg.norm_nodes, norm_edges=cfg.norm_edges,
-                                          gate_eps=GATE_EPS, ln_eps=cfg.ln_eps)
-        # GEMM halves of the backward on the tensor cores: data gradients (gemm_tc.cu, transposed weight images,
-        # residual added in the epilogue) and weight gradients (wgrad_tc.cu, split-K over rows)
-        need = ctx.needs_input_grad
-        gx = gy = None
-        if need[1]:
-            gx = ops.gemm_gather(GP, img_catT, None, add0=gx_out if cfg.residual else None)
-        if deferred:
-            for j, W in enumerate((W_sg, W_du, W_dg, W_su)):           # column blocks of GP: e_src | Bh | e_dst | src_update
-                queue.add(GP[:, j * d:(j + 1) * d], x, W)
-            queue.add(GM, y, W_eg)
-            # partial rows of the destination pass: {g_ew, g_eb, g_nw, g_nb, gb_su, gb_dg}; of the source pass: {gb_sg, gb_du}
+        if torch.is_grad_enabled() and ctx.cfg.norm_nodes == NORM_LAYER:
+            # create_graph=True (force training): the first backward becomes a differentiable function of x, y, the
+            # incoming gradients and the parameters, whose own backward runs on the library kernels
+            x, y, P, M, XP, S, H, nw, nb, ew, eb = ctx.saved_tensors
+            W_sg, W_dg, W_eg, W_su, W_du = ctx.weights
+            b_sg, b_dg, b_eg, b_su, b_du = ctx.biases
+            gy_live = None if (ctx.y_dead or gy_out is None) else gy_out
+            grads = _EdgeGatedConvBackwardFn.apply(ctx, (P, M, XP, S, H), x, y, gx_out, gy_live, W_sg, b_sg, W_dg, b_dg,
+                                                   W_eg, b_eg, W_su, b_su, W_du, b_du, nw, nb, ew, eb)
+            return (None,) + tuple(grads)
+        return _first_backward_once(ctx, gx_out, gy_out)
+
+
+def _first_backward(ctx, gx_out, gy_out, saved=None, create_graph=False):
+    """The conv's backward on the library kernels.  Returns the 17 gradients of _EdgeGatedConvFn.forward's inputs;
+    with create_graph=True also (GP, GM, GSh) for the double backward, and weight gradients are never deferred."""
+    cfg = ctx.cfg
+    x, y, P, M, XP, S, H, nw, nb, ew, eb = saved if saved is not None else ctx.saved_tensors
+    img_catT, img_egT = cfg.images.images["catT"], cfg.images.images["egT"]
+    d = x.shape[1]
+    gx_out = gx_out.contiguous()
+    gy_out = None if (ctx.y_dead or gy_out is None) else gy_out.contiguous()
+    if cfg.norm_nodes == NORM_LAYER:
+        n = dict(w=nw.contiguous(), b=nb.contiguous())
+        e = dict(w=ew.contiguous(), b=eb.contiguous())
+    else:
+        sc, sh, mu, rs = cfg.n_aux
+        n = dict(w=sc, b=sh, mean=mu, rstd=rs)
+        e = {}
+        if cfg.e_aux is not None:
+            sc, sh, mu, rs = cfg.e_aux
+            e = dict(w=sc, b=sh, mean=mu, rstd=rs)
+        if cfg.norm_nodes == NORM_STATS:
+            n["c1"], n["c2"] = ops.bn_backward_reduce(XP, gx_out, n["w"], n["b"], n["mean"], n["rstd"])
             if gy_out is not None:
-                queue.add_vec(vd, 0, d, ew)
-                queue.add_vec(vd, 1, d, eb)
-            queue.add_vec(vd, 2, d, nw)
-            queue.add_vec(vd, 3, d, nb)
-            queue.add_vec(vd, 4, d, b_su)
-            queue.add_vec(vd, 5, d, b_dg)
-            queue.add_vec(vd, 5, d, b_eg)                            # sum_e gm_e == sum_v sum_{e->v} gm_e
-            queue.add_vec(vs, 0, d, b_sg)
-            queue.add_vec(vs, 1, d, b_du)
-        elif params:
-            gWcat = ops.wgrad(GP, x, groups=4)      # [4d, d] rows: src_gate | dst_update | dst_gate | src_update
-            gW_eg = ops.wgrad(GM, y, groups=1)
-        if need[2]:
-            res = gy_out if (gy_out is not None and cfg.residual) else None
-            gy = ops.gemm_gather(GM, img_egT, None, add0=res)
-        if not params:
-            return (None, gx, gy) + (None,) * 14
-        if deferred:
-            return (None, gx, gy) + (None,) * 14
+                e["c1"], e["c2"] = ops.bn_backward_reduce(M, gy_out, e["w"], e["b"], e["mean"], e["rstd"])
+    # Parameter gradients are off the critical path of backward.  With a queue installed (FlatGradAllReducer.deferring())
+    # the five weight-gradient GEMMs and the nine bias / norm-parameter reductions of this conv are only registered
+    # here and computed by two batched launches at the end of backward, straight into the flat gradient buffer.
+    params = not ops.input_grads_only.active                # a forces-only backward discards every parameter gradient
+    queue = None if create_graph else ops.WgradQueue.current
+    W_sg, W_dg, W_eg, W_su, W_du = ctx.weights
+    b_sg, b_dg, b_eg, b_su, b_du = ctx.biases
+    vec_needed = [b_sg, b_dg, b_eg, b_su, b_du, nw, nb] + ([ew, eb] if gy_out is not None else [])
+    deferred = params and queue is not None and ops.wgrad_supported(d, d) and queue.wants(W_sg, W_du, W_dg, W_su, W_eg) \
+        and queue.wants_vecs(*vec_needed)
+    res = ops.egc_backward(cfg.index, P, M, XP, S, H, gx_out, gy_out, n, e, reduce=params and not deferred,
+                           norm_nodes=cfg.norm_nodes, norm_edges=cfg.norm_edges,
+                           gate_eps=GATE_EPS, ln_eps=cfg.ln_eps, keep_gsh=create_graph)
+    GM, GP, vd, vs = res[:4]
+    # GEMM halves of the backward on the tensor cores: data gradients (gemm_tc.cu, transposed weight images,
+    # residual added in the epilogue) and weight gradients (wgrad_tc.cu, split-K over rows)
+    need = ctx.needs_input_grad
+    gx = gy = None
+    if need[1]:
+        gx = ops.gemm_gather(GP, img_catT, None, add0=gx_out if cfg.residual else None)
+    if deferred:
+        for j, W in enumerate((W_sg, W_du, W_dg, W_su)):           # column blocks of GP: e_src | Bh | e_dst | src_update
+            queue.add(GP[:, j * d:(j + 1) * d], x, W)
+        queue.add(GM, y, W_eg)
+        # partial rows of the destination pass: {g_ew, g_eb, g_nw, g_nb, gb_su, gb_dg}; of the source pass: {gb_sg, gb_du}
+        if gy_out is not None:
+            queue.add_vec(vd, 0, d, ew)
+            queue.add_vec(vd, 1, d, eb)
+        queue.add_vec(vd, 2, d, nw)
+        queue.add_vec(vd, 3, d, nb)
+        queue.add_vec(vd, 4, d, b_su)
+        queue.add_vec(vd, 5, d, b_dg)
+        queue.add_vec(vd, 5, d, b_eg)                            # sum_e gm_e == sum_v sum_{e->v} gm_e
+        queue.add_vec(vs, 0, d, b_sg)
+        queue.add_vec(vs, 1, d, b_du)
+    elif params:
+        gWcat = ops.wgrad(GP, x, groups=4)      # [4d, d] rows: src_gate | dst_update | dst_gate | src_update
+        gW_eg = ops.wgrad(GM, y, groups=1)
+    if need[2]:
+        res_y = gy_out if (gy_out is not None and cfg.residual) else None
+        gy = ops.gemm_gather(GM, img_egT, None, add0=res_y)
+    if not params or deferred:
+        grads = (None, gx, gy) + (None,) * 14
+        return (grads, GP, GM, res[4]) if create_graph else grads
+    gW_sg, gW_du, gW_dg, gW_su = gWcat[0:d], gWcat[d:2 * d], gWcat[2 * d:3 * d], gWcat[3 * d:4 * d]
+    gb_sg, gb_du = vs[0], vs[1]
+    gb_su, gb_dg = vd[4], vd[5]
+    gb_eg = gb_dg                           # sum_e gm_e == sum_v sum_{e->v} gm_e
+    g_nw, g_nb = vd[2], vd[3]
+    g_ew, g_eb = (vd[0], vd[1]) if gy_out is not None else (None, None)
+    grads = (None, gx, gy, gW_sg, gb_sg, gW_dg, gb_dg, gW_eg, gb_eg, gW_su, gb_su, gW_du, gb_du, g_nw, g_nb, g_ew, g_eb)
+    return (grads, GP, GM, res[4]) if create_graph else grads
+
+
+# today's first-order backward: no grad mode inside, and a create_graph backward through it (BatchNorm convs) fails
+# loudly when differentiated again
+_first_backward_once = once_differentiable(_first_backward)
+
+
+class _EdgeGatedConvBackwardFn(torch.autograd.Function):
+    """The first backward of a LayerNorm conv as a function of (x, y, gx_out, gy_out, parameters) -> (gx, gy, parameter
+    gradients).  Its forward is the first backward on the library kernels; its backward (the double backward) projects
+    the cotangents of gx, gy through the weight images, runs alignn_b200_egc_backward_vjp, and finishes through the
+    forward GEMMs.  The parameter gradients it returns are values only: differentiating through them raises."""
+
+    @staticmethod
+    def forward(ctx, fctx, saved, x, y, gx_out, gy_out, W_sg, b_sg, W_dg, b_dg, W_eg, b_eg, W_su, b_su, W_du, b_du,
+                nw, nb, ew, eb):
+        ctx.set_materialize_grads(False)
+        P, M, XP, S, H = saved
+        grads, GP, GM, GSh = _first_backward(fctx, gx_out, gy_out, (x, y) + saved + (nw, nb, ew, eb), create_graph=True)
+        ctx.cfg, ctx.residual = fctx.cfg, fctx.cfg.residual
+        ctx.save_for_backward(x, y, P, M, XP, S, H, nw, nb, ew, eb, gx_out.contiguous(),
+                              None if gy_out is None else gy_out.contiguous(), GP, GM, GSh)
+        return grads[1:]
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gx_bar, gy_bar, *gparam_bar):
+        if any(g is not None for g in gparam_bar):
+            raise NotImplementedError(
+                "alignn_b200.EdgeGatedGraphConv: the parameter gradients of a create_graph=True backward cannot be "
+                "differentiated again (the double backward covers the input gradients gx, gy); wrap the first "
+                "autograd.grad in alignn_b200.ops.input_grads_only() if only input gradients are needed")
+        cfg = ctx.cfg
+        x, y, P, M, XP, S, H, nw, nb, ew, eb, gx_out, gy_out, GP, GM, GSh = ctx.saved_tensors
+        img = cfg.images.images
+        d = x.shape[1]
+        Ne = y.shape[0]
+        gx_bar = torch.zeros_like(x) if gx_bar is None else gx_bar.contiguous()
+        gy_bar = None if (gy_bar is None or Ne == 0) else gy_bar.contiguous()
+        # through the GEMMs of the first backward: gx = GP Wcat (+ gx_out), gy = GM W_eg (+ gy_out)
+        GPbar = ops.gemm_gather(gx_bar, img["cat"])
+        GMbar = ops.gemm_gather(gy_bar, img["eg"]) if gy_bar is not None else None
+        Pbar, Mbar, gxo_bar, gyo_bar, vd, vs = ops.egc_backward_vjp(
+            cfg.index, P, M, XP, S, H, gx_out, gy_out, GSh, GPbar, GMbar,
+            gx_bar if ctx.residual else None, gy_bar if (ctx.residual and gy_out is not None) else None,
+            nw.contiguous(), nb.contiguous(), ew.contiguous(), eb.contiguous(), gate_eps=GATE_EPS, ln_eps=cfg.ln_eps)
+        # through the forward GEMMs: P = x Wcat^T + bcat, M = y W_eg^T + e_src[src] + e_dst[dst]
+        need = ctx.needs_input_grad
+        x_bar = ops.gemm_gather(Pbar, img["catT"]) if need[2] else None
+        y_bar = ops.gemm_gather(Mbar, img["egT"]) if need[3] else None
+        if ops.input_grads_only.active:
+            return (None, None, x_bar, y_bar, gxo_bar, gyo_bar) + (None,) * 14
+        gWcat = ops.wgrad(Pbar, x, groups=4)
+        gWcat.add_(ops.wgrad(GP, gx_bar, groups=4))
+        gW_eg = ops.wgrad(Mbar, y, groups=1)
+        if gy_bar is not None:
+            gW_eg.add_(ops.wgrad(GM, gy_bar, groups=1))
         gW_sg, gW_du, gW_dg, gW_su = gWcat[0:d], gWcat[d:2 * d], gWcat[2 * d:3 * d], gWcat[3 * d:4 * d]
         gb_sg, gb_du = vs[0], vs[1]
         gb_su, gb_dg = vd[4], vd[5]
-        gb_eg = gb_dg                           # sum_e gm_e == sum_v sum_{e->v} gm_e
+        gb_eg = gb_dg                           # sum_e Mbar_e == sum_v sum_{e->v} Mbar_e
         g_nw, g_nb = vd[2], vd[3]
         g_ew, g_eb = (vd[0], vd[1]) if gy_out is not None else (None, None)
-        return (None, gx, gy, gW_sg, gb_sg, gW_dg, gb_dg, gW_eg, gb_eg, gW_su, gb_su, gW_du, gb_du,
-                g_nw, g_nb, g_ew, g_eb)
+        return (None, None, x_bar, y_bar, gxo_bar, gyo_bar, gW_sg, gb_sg, gW_dg, gb_dg, gW_eg, gb_eg, gW_su, gb_su,
+                gW_du, gb_du, g_nw, g_nb, g_ew, g_eb)
 
 
 def _momentum(bn: nn.BatchNorm1d) -> float:
@@ -300,7 +380,8 @@ class EdgeGatedGraphConvBase(nn.Module):
             raise RuntimeError("feature rows do not match the graph: "
                                f"{tuple(node_feats.shape)} nodes vs {g.num_nodes()}, "
                                f"{tuple(edge_feats.shape)} edges vs {g.num_edges()}")
-        if second_order.active:
+        if second_order.active and self.norm_kind != "layernorm":
+            # BatchNorm convs have no double backward on the kernels: differentiable torch operators instead
             return _torch_ops_forward(self, g.index, node_feats, edge_feats, _need_edge_out)
         cfg = _Cfg()
         cfg.index = g.index
@@ -322,8 +403,10 @@ class EdgeGatedGraphConvBase(nn.Module):
         return x, (y if _need_edge_out else None)
 
     def _run_kernels(self, cfg, node_feats, edge_feats):
+        # contiguous HERE, outside the Function: its saved x, y must be the autograd inputs themselves, or the double
+        # backward would see a detached copy and drop the x / y terms
         return _EdgeGatedConvFn.apply(
-            cfg, node_feats, edge_feats,
+            cfg, node_feats.contiguous(), edge_feats.contiguous(),
             self.src_gate.weight, self.src_gate.bias, self.dst_gate.weight, self.dst_gate.bias,
             self.edge_gate.weight, self.edge_gate.bias, self.src_update.weight, self.src_update.bias,
             self.dst_update.weight, self.dst_update.bias,

@@ -194,11 +194,12 @@ def bn_backward_reduce(R, g_out, scale, shift, mean, rstd) -> Tuple[torch.Tensor
 
 @_on_tensor_device
 def egc_backward(ix: EdgeIndex, P, M, XP, S, H, gx_out, gy_out, n, e, *, reduce: bool = True, norm_nodes: int, norm_edges: int,
-                 gate_eps: float = 1e-6, ln_eps: float = 1e-5):
+                 gate_eps: float = 1e-6, ln_eps: float = 1e-5, keep_gsh: bool = False):
     """n / e: dicts with keys w, b, mean, rstd, c1, c2 (entries may be None).
 
     Returns GM [Ne,d], GP [Nn,4d], vec_dst [6,d], vec_src [2,d] (column sums of the partials); with reduce=False the
-    per-block partial rows [rows, 6d] and [rows, 2d] themselves."""
+    per-block partial rows [rows, 6d] and [rows, 2d] themselves.  keep_gsh=True appends the workspace GSh = dL/dSh
+    [Nn,d], which the double backward (`egc_backward_vjp`) reads."""
     lib = _lib.load()
     Nn, d = XP.shape
     Ne = M.shape[0]
@@ -225,9 +226,56 @@ def egc_backward(ix: EdgeIndex, P, M, XP, S, H, gx_out, gy_out, n, e, *, reduce:
     nb = 4 * d * (Ne * (2 + (gy_out is not None)) + 9 * Nn) + 12 * Ne + 4 * d * 2 * Ne
     with _span("egc_backward(dst+src)", nb):
         _lib.check(lib.alignn_b200_egc_backward(C.byref(a)), "alignn_b200_egc_backward")
+    extra = (GSh,) if keep_gsh else ()
     if not reduce:              # the caller sums the per-block partial rows itself (WgradQueue: one batched launch per backward)
-        return GM, GP, part, part_src
-    return GM, GP, colsum(part).view(6, d), colsum(part_src).view(2, d)
+        return (GM, GP, part, part_src) + extra
+    return (GM, GP, colsum(part).view(6, d), colsum(part_src).view(2, d)) + extra
+
+
+@_on_tensor_device
+def egc_backward_vjp(ix: EdgeIndex, P, M, XP, S, H, gx_out, gy_out, GSh, GPbar, GMbar, gx_bar_res, gy_bar_res,
+                     n_w, n_b, e_w, e_b, *, gate_eps: float = 1e-6, ln_eps: float = 1e-5):
+    """Double backward of a LayerNorm conv (include/alignn_b200.h, alignn_b200_egc_backward_vjp): the cotangents of
+    the first backward's inputs, given GPbar = gx_bar Wcat^T and GMbar = gy_bar W_eg^T (None: zero).  gx_bar_res /
+    gy_bar_res are added to the gx_out / gy_out cotangents (the residual), None to skip.
+
+    Returns Pbar [Nn,4d], Mbar [Ne,d], gx_out_bar [Nn,d], gy_out_bar [Ne,d] (None when gy_out is None), and the column
+    sums vec_dst [6,d] = {e_w, e_b, n_w, n_b cotangents, sum Pbar_D, sum Pbar_B}, vec_src [2,d] = {sum Pbar_A,
+    sum Pbar_C}."""
+    lib = _lib.load()
+    Nn, d = XP.shape
+    Ne = M.shape[0]
+    _check_d(d)
+    require_cuda(P, M, XP, S, H, gx_out, gy_out, GSh, GPbar, GMbar, gx_bar_res, gy_bar_res, n_w, n_b, e_w, e_b,
+                 ix.src, ix.dst, ix.in_ptr, ix.in_eid, ix.out_ptr, ix.out_eid)
+    dev = XP.device
+    new = lambda *s: torch.empty(*s, device=dev, dtype=torch.float32)  # noqa: E731
+    Pbar, Mbar, gxo_bar = new(Nn, 4 * d), new(Ne, d), new(Nn, d)
+    gyo_bar = new(Ne, d) if gy_out is not None else None
+    Gamma, Shbar = new(Ne, d), new(Nn, d)
+    rows = partial_rows(Nn, d)
+    part, part_src = new(rows, 6 * d), new(rows, 2 * d)
+    a = _lib.EgcBwdVjpArgs(
+        struct_size=C.sizeof(_lib.EgcBwdVjpArgs), Nn=Nn, Ne=Ne, d=d, norm=NORM_LAYER, gate_eps=gate_eps, ln_eps=ln_eps,
+        P=ptr(P), M=ptr(M), XP=ptr(XP), S=ptr(S), H=ptr(H),
+        src=ptr(ix.src), dst=ptr(ix.dst), in_ptr=ptr(ix.in_ptr), in_eid=None if ix.dst_sorted else ptr(ix.in_eid),
+        out_ptr=ptr(ix.out_ptr), out_eid=ptr(ix.out_eid),
+        n_w=ptr(n_w), n_b=ptr(n_b), e_w=ptr(e_w), e_b=ptr(e_b),
+        gx_out=ptr(gx_out), gy_out=ptr(gy_out), GSh=ptr(GSh),
+        GPbar=ptr(GPbar), GMbar=ptr(GMbar), gx_bar_res=ptr(gx_bar_res), gy_bar_res=ptr(gy_bar_res),
+        Pbar=ptr(Pbar), Mbar=ptr(Mbar), gx_out_bar=ptr(gxo_bar), gy_out_bar=ptr(gyo_bar), Gamma=ptr(Gamma),
+        Shbar=ptr(Shbar), partials=ptr(part), partials_src=ptr(part_src), stream=stream_ptr())
+    # compulsory bytes: every input row read once and every output row written once; gathered node rows (C, GPbar_A,
+    # GPbar_C) count once per node.  node rows: read XP, gx_out, S, H, GSh, the C block of P, GPbar (4 blocks) and
+    # gx_bar_res; write Pbar (4 blocks) and gx_out_bar.  edge rows: read M, GMbar, gy_out, gy_bar_res; write Mbar,
+    # gy_out_bar; plus the src / dst / eid indices and both pointer arrays.  The workspaces Gamma and Shbar and the
+    # re-reads of M and Mbar in the second sweep and the source pass are not compulsory.
+    live = gy_out is not None
+    nb = 4 * d * Nn * (6 + 4 + (gx_bar_res is not None) + 4 + 1)
+    nb += 4 * d * Ne * (1 + (GMbar is not None) + live + (gy_bar_res is not None) + 1 + live) + 12 * Ne + 8 * (Nn + 1)
+    with _span("egc_backward_vjp", nb):
+        _lib.check(lib.alignn_b200_egc_backward_vjp(C.byref(a)), "alignn_b200_egc_backward_vjp")
+    return Pbar, Mbar, gxo_bar, gyo_bar, colsum(part).view(6, d), colsum(part_src).view(2, d)
 
 
 @_on_tensor_device

@@ -169,6 +169,58 @@ typedef struct {
 
 int alignn_b200_egc_backward(const alignn_b200_egc_bwd_args* args);
 
+/* ------------------------------------------------------------------------------------------
+ * Double backward of the same stage, LayerNorm only: the vector-Jacobian product of the first
+ * backward, which `torch.autograd.grad(..., create_graph=True)` differentiates in force training
+ * (alignn/models/alignn_atomwise.py:530-539).  The first backward maps (x, y, gx_out, gy_out) to
+ *   gx = GP Wcat (+ gx_out),  gy = GM W_eg (+ gy_out);
+ * given cotangents gx_bar, gy_bar of gx, gy, the caller first projects them through the same
+ * weights (GPbar = gx_bar Wcat^T, GMbar = gy_bar W_eg^T) and this call produces
+ *   Pbar [Nn,4d] = dL/dP (layout of P),  Mbar [Ne,d] = dL/dm,
+ *   gx_out_bar, gy_out_bar (with the residual's gx_bar / gy_bar added when given),
+ *   LayerNorm parameter cotangents and bias sums as per-block partials.
+ * The caller finishes with x_bar = Pbar Wcat, y_bar = Mbar W_eg and the weight cotangents
+ * Pbar^T x + GP^T gx_bar, Mbar^T y + GM^T gy_bar.  norm must be ALIGNN_NORM_LAYER (ALIGNN_ERR_BAD_ARG
+ * otherwise; checked right after struct_size and d, before the graph sizes and pointers).
+ * ---------------------------------------------------------------------------------------- */
+typedef struct {
+  size_t struct_size;
+  int64_t Nn, Ne;
+  int32_t d;
+  int32_t norm;                   /* ALIGNN_NORM_LAYER (both norms of the conv) */
+  float gate_eps, ln_eps;
+  /* saved from forward */
+  const float* P; const float* M; const float* XP; const float* S; const float* H;
+  const int32_t* src; const int32_t* dst;
+  const int32_t* in_ptr; const int32_t* in_eid;   /* in_eid NULL = identity */
+  const int32_t* out_ptr; const int32_t* out_eid;
+  const float* n_w; const float* n_b; const float* e_w; const float* e_b;   /* LayerNorm gamma, beta [d] */
+  /* inputs of the first backward and its workspace */
+  const float* gx_out;      /* [Nn,d] */
+  const float* gy_out;      /* [Ne,d] or NULL (edge output unused) */
+  const float* GSh;         /* [Nn,d] dL/d(sum_sigma_h) as alignn_b200_egc_backward wrote it */
+  /* cotangents */
+  const float* GPbar;       /* [Nn,4d] gx_bar Wcat^T */
+  const float* GMbar;       /* [Ne,d] gy_bar W_eg^T, or NULL (zero) */
+  const float* gx_bar_res;  /* [Nn,d] gx_bar, added to gx_out_bar (residual), or NULL */
+  const float* gy_bar_res;  /* [Ne,d] gy_bar, added to gy_out_bar (residual), or NULL */
+  /* outputs */
+  float* Pbar;              /* [Nn,4d] */
+  float* Mbar;              /* [Ne,d] */
+  float* gx_out_bar;        /* [Nn,d] */
+  float* gy_out_bar;        /* [Ne,d]; required when gy_out != NULL */
+  float* Gamma;             /* [Ne,d] workspace: cotangent of GM */
+  float* Shbar;             /* [Nn,d] workspace: dL/d(sum_sigma_h) of the forward */
+  /* per-block partials, rows = alignn_b200_egc_partial_rows(Nn, d):
+     destination pass [rows, 6, d] = {sum e_w_bar, sum e_b_bar, sum n_w_bar, sum n_b_bar, sum Pbar_D, sum Pbar_B};
+     source pass      [rows, 2, d] = {sum Pbar_A, sum Pbar_C} */
+  float* partials;
+  float* partials_src;
+  alignn_stream_t stream;
+} alignn_b200_egc_bwd_vjp_args;
+
+int alignn_b200_egc_backward_vjp(const alignn_b200_egc_bwd_vjp_args* args);
+
 /* BatchNorm train-mode backward, pass 1: per-block partials of sum(gu) and sum(gu*xhat) over rows,
  * gu = g_out * silu'(R*scale+shift), xhat = (R-mean)*rstd.  partials: [rows_out, 2, d]. */
 int alignn_b200_bn_backward_reduce(const float* R, const float* g_out, const float* scale, const float* shift,
