@@ -77,6 +77,17 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
                : "memory");
 }
 
+// 16-byte global -> shared copy of this thread (LDGSTS, L2 only), tracked by cp.async commit / wait groups.  With
+// `valid` false nothing is read and the 16 bytes are zero-filled (src must still be a mapped address).
+__device__ __forceinline__ void cp_async16_zfill(void* dst_smem, const void* src_gmem, bool valid) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(valid ? 16 : 0)
+               : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+// wait until at most N committed cp.async groups of this thread are still in flight
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
 // Asynchronous bulk prefetch of a contiguous global region into L2 (no destination, no completion).
 __device__ __forceinline__ void bulk_prefetch_l2(const void* src_gmem, uint32_t bytes) {
   asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src_gmem), "r"(bytes) : "memory");

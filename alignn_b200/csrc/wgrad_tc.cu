@@ -7,6 +7,11 @@
 // SWIZZLE_NONE GMMA layout:  addr(mn, k) = (mn/8)*SBO + (k/8)*LBO + (k%8)*16 + (mn%8)*2,
 // SBO = 128 (next 8 channels), LBO = (rows_of_plane/8)*128 (next 8 rows of the contraction).
 //
+// Mainloop, per CTA: the fp32 rows travel global -> shared by cp.async into a ring of FSTAGES fp32 stages (the bytes
+// in flight are set by shared memory, not by registers); the loader warps split each fp32 stage into a bf16 hi/lo
+// plane stage (ring of STAGES); the two consumer warpgroups keep one wgmma group in flight and release a plane stage
+// once the next chunk's MMAs are issued.
+//
 // Output tiles: a CTA owns a 128 x TN block of the DA x DB output (TN = min(DB, 128)), held in the registers of two
 // consumer warpgroups (rows 0-63 / 64-127, TN / 2 floats per thread); DA = 256 or DB = 256 take 2 or 4 CTAs per row
 // slab, each reading only its channels.  Split-K: CTA c of group g reduces a contiguous slab of rows into its block
@@ -22,7 +27,10 @@ namespace alignn {
 namespace wgrad {
 
 constexpr int BK = 32;          // contraction rows per stage (2 MMA K=16 steps)
-constexpr int STAGES = 4;
+// Shared memory at TA = TN = 128: 2 plane stages of 32 KB, 3 fp32 stages of 32 KB and the 64 KB of running sums, 224 KB.
+// (3 plane stages with 2 fp32 stages measured 6 % slower on the bench's weight-gradient launch on H100.)
+constexpr int STAGES = 2;       // bf16 hi/lo plane stages (loaders -> MMAs)
+constexpr int FSTAGES = 3;      // fp32 stages (cp.async -> loaders): up to 64 KB in flight per CTA while it converts
 constexpr int LOAD_WARPS = 8;
 constexpr int MMA_WARPS = 8;    // two consumer warpgroups
 constexpr int THREADS = 32 * (MMA_WARPS + LOAD_WARPS);
@@ -46,9 +54,15 @@ struct Cfg {
   static constexpr uint32_t LBO_B = (TN / 8) * 128;
   static constexpr int STAGE = 2 * A_PLANE + 2 * B_PLANE;
   static constexpr int PIPE = STAGES * STAGE;
+  static constexpr int NBA = TA / 32, NBB = TN / 32;         // 32-channel blocks of A and B: one loader warp each
+  static constexpr int FSTAGE = LOAD_WARPS * BK * 128;        // fp32 stage: 4 KB (32 rows x 32 channels) per loader warp
+  static constexpr int ACC_OFF = PIPE + FSTAGES * FSTAGE;
   static constexpr int ACC = MMA_WARPS * 32 * (TN / 2) * 4;   // running sums, one column per consumer thread
-  static constexpr int SMEM = PIPE + ACC + 128;
+  static constexpr int BAR_OFF = ACC_OFF + ACC;
+  static constexpr int SMEM = BAR_OFF + 128;
   static_assert(TILES * TA * TN == DA * DB, "output blocks cover the output");
+  static_assert(SMEM <= 232448, "shared memory budget of one sm_90 CTA");
+  static_assert(TA % 32 == 0 && TN % 32 == 0 && NBA + NBB <= LOAD_WARPS, "one loader warp per 32-channel block");
 };
 
 // The pipeline of one CTA over consecutive chunks of contraction rows, shared by the single-problem and the batch
@@ -61,51 +75,54 @@ struct Pipe {
   uint64_t* empty;
 
   // loader warps: rows [r_begin, r_end) of A (channels a0 .. a0 + TA) and B (channels b0 .. b0 + TN), chunks numbered
-  // from g0 in the ring.  Work split with compile-time structure: slot (eg, j) of warp w covers the 16-channel group
-  // og = w + 8*j of 8-row group eg; a half-warp = 8 contraction rows x 2 adjacent float4 -> one 128-byte core matrix.
+  // from g0 in the plane ring.  Loader warp w < NBA + NBB owns one 32-channel block of the chunk (A's blocks first, then
+  // B's), all 32 rows: it copies the block into its own 4 KB of the fp32 stage (one cp.async instruction = 4 rows x
+  // 128 bytes) and converts it into the planes (a half-warp = 8 contraction rows x 2 adjacent float4 -> one 128-byte
+  // core matrix).  Float4 f of row r sits at r * 128 + ((f + 2 r) % 8) * 16 of the warp's block: the copies and the
+  // converting reads are both free of bank conflicts.  Only the warp touches its block, so the lanes' own
+  // cp.async.wait_group and a __syncwarp order the copies before the reads, and the reads before the next copy into
+  // the stage.  Rows at or beyond r_end are not read; their copies zero-fill the slot.
   __device__ __forceinline__ void load(const float* __restrict__ Ag, int64_t lda, const float* __restrict__ Bg, int64_t ldb,
                                        int64_t r_begin, int64_t r_end, int nk, int g0, int warp, int lane) {
-    const int e_l = (lane >> 1) & 7, oq = (lane >> 4) * 2 + (lane & 1);
-    constexpr int JA = (F::TA / 16 + LOAD_WARPS - 1) / LOAD_WARPS, JB = (F::TN / 16 + LOAD_WARPS - 1) / LOAD_WARPS;
-    constexpr int NT = 4 * (JA + JB);
-    auto load_chunk = [&](float4 (&v)[NT], int kc) {
-      const int64_t r0 = r_begin + (int64_t)kc * BK + e_l;
+    const bool isA = warp < F::NBA, active = warp < F::NBA + F::NBB;
+    const int cb = isA ? warp : warp - F::NBA;                         // 32-channel block of the operand
+    const float* __restrict__ src = (isA ? Ag : Bg) + cb * 32 + (lane & 7) * 4;
+    const int64_t ld = isA ? lda : ldb;
+    uint8_t* blk = smem + F::PIPE + warp * BK * 128;
+    auto fetch = [&](int kc) {                 // chunk kc into fp32 stage kc % FSTAGES; one commit group per call
+      if (active && kc < nk) {
+        uint8_t* fs = blk + (kc % FSTAGES) * F::FSTAGE;
 #pragma unroll
-      for (int eg = 0; eg < 4; ++eg) {
-        const int64_t r = r0 + eg * 8;
-        const bool rv = r < r_end;
-#pragma unroll
-        for (int j = 0; j < JA; ++j) {
-          const int og = warp + LOAD_WARPS * j;
-          v[eg * (JA + JB) + j] = (rv && og < F::TA / 16) ? __ldcs(reinterpret_cast<const float4*>(Ag + r * lda + (og * 4 + oq) * 4))
-                                                          : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-#pragma unroll
-        for (int j = 0; j < JB; ++j) {
-          const int og = warp + LOAD_WARPS * j;
-          v[eg * (JA + JB) + JA + j] = (rv && og < F::TN / 16) ? __ldcs(reinterpret_cast<const float4*>(Bg + r * ldb + (og * 4 + oq) * 4))
-                                                               : make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int i = 0; i < BK / 4; ++i) {
+          const int row = i * 4 + (lane >> 3);
+          const int64_t r = r_begin + (int64_t)kc * BK + row;
+          const bool rv = r < r_end;
+          tc::cp_async16_zfill(fs + row * 128 + (((lane & 7) + 2 * row) & 7) * 16, src + (rv ? r : r_begin) * ld, rv);
         }
       }
+      tc::cp_async_commit();
     };
-    auto store_chunk = [&](const float4 (&v)[NT], int gc) {
-      const int s = gc % STAGES;
+    const int e_l = (lane >> 1) & 7, oq = (lane >> 4) * 2 + (lane & 1);
+    const int lbo = isA ? (int)F::LBO_A : (int)F::LBO_B, plane = isA ? F::A_PLANE : F::B_PLANE;
+#pragma unroll
+    for (int kc = 0; kc < FSTAGES - 1; ++kc) fetch(kc);
+    for (int kc = 0; kc < nk; ++kc) {
+      fetch(kc + FSTAGES - 1);                 // into the stage this warp converted from in iteration kc - 1
+      tc::cp_async_wait<FSTAGES - 1>();        // this lane's copies of chunk kc have landed
+      __syncwarp();                            // ... and every lane's
+      const int gc = g0 + kc, s = gc % STAGES;
       if (gc >= STAGES) tc::mbar_wait(&empty[s], ((gc / STAGES) - 1) & 1);
-      uint8_t* st = smem + s * F::STAGE;
+      if (active) {
+        const uint8_t* fs = blk + (kc % FSTAGES) * F::FSTAGE;
+        uint8_t* base = smem + s * F::STAGE + (isA ? 0 : 2 * F::A_PLANE);
 #pragma unroll
-      for (int eg = 0; eg < 4; ++eg) {
-        const int edge = eg * 8 + e_l;
+        for (int eg = 0; eg < 4; ++eg) {
+          const int edge = eg * 8 + e_l;
 #pragma unroll
-        for (int j = 0; j < JA + JB; ++j) {
-          const bool isA = j < JA;
-          const int og = warp + LOAD_WARPS * (isA ? j : j - JA);
-          if (og < (isA ? F::TA : F::TN) / 16) {
-            const int o4 = og * 4 + oq;
+          for (int h = 0; h < 2; ++h) {
+            const int f = h * 4 + oq, o4 = cb * 8 + f;
             uint2 hi, lo;
-            tc::split4(v[eg * (JA + JB) + j], hi, lo);
-            const int lbo = isA ? (int)F::LBO_A : (int)F::LBO_B;
-            const int plane = isA ? F::A_PLANE : F::B_PLANE;
-            uint8_t* base = st + (isA ? 0 : 2 * F::A_PLANE);
+            tc::split4(*reinterpret_cast<const float4*>(fs + edge * 128 + ((f + 2 * edge) & 7) * 16), hi, lo);
             const int off = (o4 >> 1) * (int)SBO + (edge >> 3) * lbo + (edge & 7) * 16 + (o4 & 1) * 8;
             *reinterpret_cast<uint2*>(base + off) = hi;
             *reinterpret_cast<uint2*>(base + plane + off) = lo;
@@ -115,50 +132,49 @@ struct Pipe {
       tc::fence_async_smem();
       __syncwarp();
       if (lane == 0) tc::mbar_arrive(&full[s]);          // one arrival per warp
-    };
-    // double-buffered in registers: the loads of chunk k+1 are in flight while chunk k is converted
-    float4 b0[NT], b1[NT];
-    if (nk > 0) load_chunk(b0, 0);
-    for (int kc = 0; kc < nk; kc += 2) {
-      if (kc + 1 < nk) load_chunk(b1, kc + 1);
-      store_chunk(b0, g0 + kc);
-      if (kc + 1 < nk) {
-        if (kc + 2 < nk) load_chunk(b0, kc + 2);
-        store_chunk(b1, g0 + kc + 1);
-      }
     }
   }
 
-  // consumer warpgroup wg: acc = its 64 rows of the block summed over nk chunks numbered from g0
+  // consumer warpgroup wg: acc = its 64 rows of the block summed over nk chunks numbered from g0.  One wgmma group
+  // stays in flight: the stage of chunk kc - 1 is released once the MMAs of chunk kc are issued and kc - 1's are
+  // complete; the queue drains only where the accumulator is read (promotion into the running sum).
   __device__ __forceinline__ void mma(float (&acc)[F::TN / 2], int nk, int g0, int wg, int lane) {
     const uint32_t base0 = tc::smem_u32(smem);
-    float* run = reinterpret_cast<float*>(smem + F::PIPE) + wg * 128 + (threadIdx.x & 127);
+    float* run = reinterpret_cast<float*>(smem + F::ACC_OFF) + wg * 128 + (threadIdx.x & 127);
 #pragma unroll
     for (int i = 0; i < F::TN / 2; ++i) { run[i * MMA_WARPS * 32] = 0.f; acc[i] = 0.f; }
-    for (int kc = 0; kc < nk; ++kc) {
-      const int g = g0 + kc, s = g % STAGES;
-      tc::mbar_wait(&full[s], (g / STAGES) & 1);
-      const uint32_t base = base0 + s * F::STAGE;
-      tc::wgmma_fence();
+    // The chunks go in runs of PROMOTE_CHUNKS: the full drain sits after a run's loop, never on a branch inside it (a
+    // wgmma wait on a branch makes ptxas serialize every wgmma of the kernel).
+    for (int k0 = 0; k0 < nk; k0 += PROMOTE_CHUNKS) {
+      const int k1 = k0 + PROMOTE_CHUNKS < nk ? k0 + PROMOTE_CHUNKS : nk;
+      int prev = -1;                                     // stage whose MMAs may still be in flight
+      for (int kc = k0; kc < k1; ++kc) {
+        const int g = g0 + kc, s = g % STAGES;
+        tc::mbar_wait(&full[s], (g / STAGES) & 1);
+        const uint32_t base = base0 + s * F::STAGE;
+        tc::wgmma_fence();
 #pragma unroll
-      for (int j = 0; j < BK / 16; ++j) {
-        const uint64_t b_hi = tc::smem_desc(base + 2 * F::A_PLANE + j * 2 * F::LBO_B, F::LBO_B, SBO);
-        const uint64_t b_lo = tc::smem_desc(base + 2 * F::A_PLANE + F::B_PLANE + j * 2 * F::LBO_B, F::LBO_B, SBO);
-        const uint32_t ao = j * 2 * F::LBO_A + wg * 8 * SBO;
-        const uint64_t a_hi = tc::smem_desc(base + ao, F::LBO_A, SBO);
-        const uint64_t a_lo = tc::smem_desc(base + F::A_PLANE + ao, F::LBO_A, SBO);
-        tc::Wgmma<F::TN>::template mma<1, 1>(acc, a_lo, b_hi, 1);
-        tc::Wgmma<F::TN>::template mma<1, 1>(acc, a_hi, b_lo, 1);
-        tc::Wgmma<F::TN>::template mma<1, 1>(acc, a_hi, b_hi, 1);
+        for (int j = 0; j < BK / 16; ++j) {
+          const uint64_t b_hi = tc::smem_desc(base + 2 * F::A_PLANE + j * 2 * F::LBO_B, F::LBO_B, SBO);
+          const uint64_t b_lo = tc::smem_desc(base + 2 * F::A_PLANE + F::B_PLANE + j * 2 * F::LBO_B, F::LBO_B, SBO);
+          const uint32_t ao = j * 2 * F::LBO_A + wg * 8 * SBO;
+          const uint64_t a_hi = tc::smem_desc(base + ao, F::LBO_A, SBO);
+          const uint64_t a_lo = tc::smem_desc(base + F::A_PLANE + ao, F::LBO_A, SBO);
+          tc::Wgmma<F::TN>::template mma<1, 1>(acc, a_lo, b_hi, 1);
+          tc::Wgmma<F::TN>::template mma<1, 1>(acc, a_hi, b_lo, 1);
+          tc::Wgmma<F::TN>::template mma<1, 1>(acc, a_hi, b_hi, 1);
+        }
+        tc::wgmma_commit();
+        tc::wgmma_wait<1>();                             // the MMAs of chunk kc - 1 are complete
+        __syncwarp();
+        if (lane == 0 && prev >= 0) tc::mbar_arrive(&empty[prev]);
+        prev = s;
       }
-      tc::wgmma_commit();
       tc::wgmma_wait_all();
       __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&empty[s]);
-      if ((kc + 1) % PROMOTE_CHUNKS == 0 || kc + 1 == nk) {
+      if (lane == 0) tc::mbar_arrive(&empty[prev]);
 #pragma unroll
-        for (int i = 0; i < F::TN / 2; ++i) { run[i * MMA_WARPS * 32] += acc[i]; acc[i] = 0.f; }
-      }
+      for (int i = 0; i < F::TN / 2; ++i) { run[i * MMA_WARPS * 32] += acc[i]; acc[i] = 0.f; }
     }
 #pragma unroll
     for (int i = 0; i < F::TN / 2; ++i) acc[i] = run[i * MMA_WARPS * 32];
@@ -202,7 +218,7 @@ wgrad_bf16x3_kernel(const float* __restrict__ A, int64_t lda, const float* __res
                     int rows_per_cta, float* __restrict__ partials, float* __restrict__ out, int64_t ld_out) {
   using F = Cfg<DA, DB>;
   extern __shared__ __align__(128) uint8_t smem[];
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + F::PIPE + F::ACC);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + F::BAR_OFF);
   Pipe<DA, DB> pipe{smem, full, full + STAGES};
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int cta = blockIdx.x, group = blockIdx.y, mt = blockIdx.z / F::NT, nt = blockIdx.z % F::NT;
@@ -278,7 +294,7 @@ __global__ void __launch_bounds__(THREADS, 1)
 wgrad_batch_kernel(const __grid_constant__ Batch bt, float* __restrict__ partials) {
   using F = Cfg<DA, DB>;
   extern __shared__ __align__(128) uint8_t smem[];
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + F::PIPE + F::ACC);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + F::BAR_OFF);
   Pipe<DA, DB> pipe{smem, full, full + STAGES};
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int cta = blockIdx.x, mt = blockIdx.y / F::NT, nt = blockIdx.y % F::NT;
@@ -558,7 +574,9 @@ int alignn_b200_wgrad(const float* A, int64_t lda, const float* B, int64_t ldb, 
   using namespace alignn::wgrad;
   if (K < 0 || groups < 1 || !out || ld_out < DB || (ld_out % 4)) return ALIGNN_ERR_BAD_ARG;
   if (!shape_ok(DA, DB)) return ALIGNN_ERR_UNSUPPORTED_D;
-  if (K > 0 && (!A || !B || lda < (int64_t)groups * DA || ldb < DB || (lda % 4) || (ldb % 4))) return ALIGNN_ERR_BAD_ARG;
+  if (K > 0 && (!A || !B || lda < (int64_t)groups * DA || ldb < DB || (lda % 4) || (ldb % 4) || ((uintptr_t)A & 15) ||
+                ((uintptr_t)B & 15)))
+    return ALIGNN_ERR_BAD_ARG;
   if (K >= ((int64_t)1 << 31) * BK) return ALIGNN_ERR_BAD_ARG;
   if (!workspace || workspace_bytes < alignn_b200_wgrad_workspace_bytes(K, DA, DB, groups)) return ALIGNN_ERR_WORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
