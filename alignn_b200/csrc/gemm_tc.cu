@@ -10,21 +10,27 @@
 // per-channel batch statistics BatchNorm1d(m) needs (alignn.py:123).  With add0 = the incoming gradient it is the
 // data-gradient GEMM of the backward (residual in the epilogue).
 //
-// A is the fp32 activation matrix, streamed from HBM once; it is converted to bf16 hi/lo planes by the loader warps on
-// its way into shared memory (software-pipelined: the global loads of chunk k+1 are in flight while chunk k is
-// converted).  W is pre-split once per step into an image that already has the GMMA core-matrix order
-// (gemm_prepare_table), so a K-chunk of it is ONE contiguous bulk copy (cp.async.bulk) signalled on the stage's
-// mbarrier.
+// A is the fp32 activation matrix, read once per column tile: the producer warps copy its K-chunks global -> shared with
+// cp.async into a ring of fp32 stages (the bytes in flight are set by shared memory, not by registers) and split them
+// into the bf16 hi/lo planes of a ring of plane stages.  W is pre-split once per step into an image that already has the
+// GMMA core-matrix order (gemm_prepare_table), so a K-chunk of it is ONE contiguous bulk copy (cp.async.bulk) signalled
+// on the plane stage's mbarrier.
 //
-// Persistent, warp-specialised CTA (one per SM), 128 x BN output tiles, BN <= 128: the 128 x BN fp32 accumulator lives
-// in the registers of two consumer warpgroups (BN / 2 per thread).
-//   warps 0-7   : two consumer warpgroups, rows 0-63 / 64-127 of the tile: wgmma m64nBNk16, then the epilogue
-//   warps 8-15  : loaders / fp32->bf16x2 converters, up to STAGES chunks ahead of the MMAs
+// Persistent, warp-specialised CTA (one per SM), 128 x BN output tiles, BN <= 128, three warpgroups:
+//   warps 0-3, 4-7 : two consumer warpgroups, ping-pong: local tile i of the CTA belongs to warpgroup i % 2, which runs
+//                    both m64 row halves of it (wgmma m64nBNk16, BN accumulator registers per thread) and then its
+//                    epilogue -- while one warpgroup is in its epilogue the other runs the MMAs of the next tile
+//   warps 8-11     : producer: cp.async of A, fp32 -> bf16 hi/lo split, bulk copy of W
+// setmaxnreg moves registers from the producer to the consumers.  The chunks of consecutive tiles pass through the
+// stage ring in tile order, and a consumer starts the mainloop of local tile i only once the other one has issued the
+// MMAs of tile i - 1's last chunk: the MMAs of the two warpgroups do not interleave, and a consumer never waits on a
+// stage barrier more than one phase ahead of it (an mbarrier parity wait cannot tell phase k from phase k + 2).
 // Mainloop: one wgmma group stays in flight; a stage is released once the MMAs of the next chunk have been issued.
-// Epilogue: the wgmma fragment of one consumer warp is 16 whole rows of the tile, so each warp stages its own rows
-// through a private shared-memory tile (no block barrier) and then works row by row: a row is BN / 4 lanes with one
-// float4 each, the addend rows of several rows are loaded before the first store, and C is written as contiguous row
-// segments.  The addend rows are read through __restrict__ pointers: C must not overlap A, add0, add1 or the bias.
+// Epilogue: the wgmma fragment of one consumer warp is 16 whole rows of each row half, so each warp stages its own rows
+// through a private shared-memory tile (no block barrier), one half after the other, and then works row by row: a row is
+// BN / 4 lanes with one float4 each, the addend rows of several rows are loaded before the first store, and C is written
+// as contiguous row segments.  The addend rows are read through __restrict__ pointers: C must not overlap A, add0, add1
+// or the bias.
 #include "common.cuh"
 #include "tc_common.cuh"
 #include "api_common.h"
@@ -35,14 +41,18 @@ namespace gemm {
 
 constexpr int BM = 128;       // rows per tile (two m64 warpgroup MMAs)
 constexpr int BK = 32;        // K per pipeline stage (2 MMA K=16 steps)
-constexpr int STAGES = 4;
-constexpr int MMA_WARPS = 8;
-constexpr int LOAD_WARPS = 8;
-constexpr int THREADS = 32 * (MMA_WARPS + LOAD_WARPS);   // 512
+constexpr int STAGES = 2;     // bf16 hi/lo plane stages (producer -> MMAs)
+constexpr int FSTAGES = 4;    // fp32 stages of A (cp.async -> producer): up to 64 KB in flight per CTA
+constexpr int MMA_WARPS = 8;  // two consumer warpgroups
+constexpr int LOAD_WARPS = 4; // one producer warpgroup
+constexpr int THREADS = 32 * (MMA_WARPS + LOAD_WARPS);   // 384
+constexpr int LOAD_REGS = 40, MMA_REGS = 232;            // setmaxnreg: 128 x 40 + 256 x 232 <= 64 K registers
+static_assert(128 * LOAD_REGS + 256 * MMA_REGS <= 65536, "register file of one SM");
 constexpr uint32_t LBO = 128;               // next 8-element K chunk
 constexpr uint32_t SBO = (BK / 8) * 128;    // next 8-row group (chunk-local image): 512 B
 constexpr int kMaxStatN = 256;              // widest output with column statistics
-constexpr int WARP_ROWS = 16;               // tile rows of one consumer warp's wgmma fragment
+constexpr int WARP_ROWS = 16;               // tile rows of one consumer warp's wgmma fragment (per row half)
+constexpr int STAT_ROWS = 8;                // column partials: one per (row half, warp of the warpgroup)
 
 template <int BN>
 struct Cfg {
@@ -50,12 +60,16 @@ struct Cfg {
   static constexpr int B_PLANE = BN * BK * 2;
   static constexpr int STAGE = 2 * A_PLANE + 2 * B_PLANE;
   static constexpr int PIPE_BYTES = STAGES * STAGE;
-  // accumulator staging, fp32, rows padded by 8 floats: the fragment stores (8 rows x 4 lane pairs per
-  // instruction) then fill all 32 banks twice, the minimum for 256 bytes
+  // fp32 stage: 128 rows x 128 bytes, 32 rows (4 KB) per producer warp
+  static constexpr int FSTAGE = BM * BK * 4;
+  static constexpr int FP_OFF = PIPE_BYTES;
+  // accumulator staging, fp32, 16 rows per consumer warp, rows padded by 8 floats: the fragment stores (8 rows x 4 lane
+  // pairs per instruction) then fill all 32 banks twice, the minimum for 256 bytes
   static constexpr int PITCH = BN + 8;
-  static constexpr int STG_BYTES = BM * PITCH * 4;
-  static constexpr int STAT_OFF = PIPE_BYTES + STG_BYTES;
-  static constexpr int STAT_BYTES = MMA_WARPS * 2 * kMaxStatN * 4;   // per consumer warp: [2][N] column partials
+  static constexpr int STG_OFF = FP_OFF + FSTAGES * FSTAGE;
+  static constexpr int STG_BYTES = MMA_WARPS * WARP_ROWS * PITCH * 4;
+  static constexpr int STAT_OFF = STG_OFF + STG_BYTES;
+  static constexpr int STAT_BYTES = STAT_ROWS * 2 * kMaxStatN * 4;   // [STAT_ROWS][2][N] column partials
   static constexpr int BAR_OFF = STAT_OFF + STAT_BYTES;
   static constexpr int SMEM = BAR_OFF + 128;
   static_assert(SMEM <= 232448, "shared memory budget of one sm_90 CTA");
@@ -80,17 +94,6 @@ struct Params {
 
 // byte offset of element (r, k) inside one chunk plane (rows x BK, core-matrix order)
 __host__ __device__ constexpr int plane_off(int r, int k) { return (r >> 3) * (int)SBO + (k >> 3) * 128 + (r & 7) * 16 + (k & 7) * 2; }
-
-// Loader thread -> (row, float4 index along K) of the 128 x 32 fp32 chunk for its i-th load.
-// A half-warp (what one 64-bit shared store wavefront serves) covers 8 rows x 2 adjacent float4, i.e. one
-// K-core-matrix column of 8 rows = 128 contiguous bytes of the plane: bank-conflict-free stores, and
-// every lane pair still reads a full 32-byte sector from HBM.
-__device__ __forceinline__ void a_coord(int i, int lt, int& row, int& kq) {
-  const int w = lt >> 5, lane = lt & 31;
-  const int u = i * LOAD_WARPS + w;                      // 32 units of (8 rows x 4 float4)
-  row = (u >> 1) * 8 + ((lane >> 1) & 7);
-  kq = (u & 1) * 4 + (lane >> 4) * 2 + (lane & 1);
-}
 
 __device__ __forceinline__ float4 ld4(const float* __restrict__ p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 __device__ __forceinline__ float4 ld4s(const float* p) {          // 4 scalars: vectors of any 4-byte alignment
@@ -144,122 +147,132 @@ gemm_bf16x3_kernel(const Params p) {
   extern __shared__ __align__(128) uint8_t smem[];
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + F::BAR_OFF);
   uint64_t* empty = full + STAGES;
+  uint64_t* stat_bar = empty + STAGES;                       // [4]: tile order of the column-partial updates
+  uint64_t* mma_turn = stat_bar + 4;                         // [4]: tile order of the consumers' mainloops
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int M = p.M, nk = p.K / BK;
-  const int n_tiles = p.N / BN;
+  const int M = p.M, N = p.N, nk = p.K / BK;
+  const int n_tiles = N / BN;
   const int m_tiles = (M + BM - 1) / BM;
   const int total = m_tiles * n_tiles;
+  const bool do_stats = p.stats != nullptr;
 
   if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full[s], LOAD_WARPS + 1); tc::mbar_init(&empty[s], MMA_WARPS); }
+    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full[s], LOAD_WARPS + 1); tc::mbar_init(&empty[s], MMA_WARPS / 2); }
+    for (int w = 0; w < 4; ++w) { tc::mbar_init(&stat_bar[w], 1); tc::mbar_init(&mma_turn[w], 1); }
     tc::mbar_fence_init();
+  }
+  if (do_stats) {
+    float* stat = reinterpret_cast<float*>(smem + F::STAT_OFF);
+    for (int i = tid; i < STAT_ROWS * 2 * N; i += THREADS) stat[i] = 0.f;
   }
   __syncthreads();
 
   if (warp >= MMA_WARPS) {
-    // ================= loaders / converters =================
-    const int lt = tid - 32 * MMA_WARPS;                 // 0..255
-    // The CTA's work is the stream of chunks c = (local tile, kc).  PF chunks of A are kept in flight in
-    // registers; every per-chunk address is an incremented pointer, not recomputed index math.
-    constexpr int PF = 3;
-    float4 buf[PF][4];
-    int soff[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      int row, kq;
-      a_coord(i, lt, row, kq);
-      soff[i] = plane_off(row, kq * 4);
-    }
+    // ================= producer =================
+    tc::setmaxnreg_dec<LOAD_REGS>();
+    // The CTA's work is the stream of chunks c = (local tile, kc).  Producer warp pw owns rows 32 pw .. 32 pw + 31 of
+    // every chunk: it copies them into its own 4 KB of the fp32 stage (one cp.async instruction = 4 rows x 128 bytes)
+    // and splits them into the planes (a half-warp = 8 rows x 2 adjacent float4 -> one 128-byte core matrix).  Float4
+    // f of row r sits at r * 128 + ((f + 2 r) % 8) * 16 of the warp's block: the copies and the converting reads are
+    // both free of bank conflicts.  Only the warp touches its block, so the lanes' own cp.async.wait_group and a
+    // __syncwarp order the copies before the reads, and the reads before the next copy into the stage.  Rows at or
+    // beyond M are not read; their copies zero-fill the slot.
+    const int pw = warp - MMA_WARPS;
     const int my_tiles = (total - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
     const int nchunks = my_tiles * nk;
-    int l_tile = blockIdx.x, l_kc = 0;
-    const float* lp[4];
-    bool lval[4];
-    auto set_tile_ptrs = [&](int tile) {
-      const int m0 = (tile / n_tiles) * BM;
+    uint8_t* blk = smem + F::FP_OFF + pw * 32 * 128;
+    int f_tile = blockIdx.x, f_kc = 0;                       // next chunk to fetch
+    auto fetch = [&](int c) {                                // chunk c into fp32 stage c % FSTAGES; one commit group
+      if (c < nchunks) {
+        uint8_t* fs = blk + (c % FSTAGES) * F::FSTAGE;
+        const int r0 = (f_tile / n_tiles) * BM + pw * 32 + (lane >> 3);
+        const float* src = p.A + (int64_t)r0 * p.lda + f_kc * BK + (lane & 7) * 4;
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        int r_, kq;
-        a_coord(i, lt, r_, kq);
-        const int gr = m0 + r_;
-        lval[i] = gr < M;
-        lp[i] = p.A + (int64_t)(lval[i] ? gr : 0) * p.lda + kq * 4;
+        for (int i = 0; i < 8; ++i) {
+          const int row = i * 4 + (lane >> 3);
+          const bool rv = r0 + i * 4 < M;
+          tc::cp_async16_zfill(fs + row * 128 + (((lane & 7) + 2 * row) & 7) * 16, rv ? src : p.A, rv);
+          src += 4 * p.lda;
+        }
+        if (++f_kc == nk) { f_kc = 0; f_tile += gridDim.x; }
       }
+      tc::cp_async_commit();
     };
-    auto load_next = [&](float4 (&v)[4]) {
+    const int e_l = (lane >> 1) & 7, oq = (lane >> 4) * 2 + (lane & 1);
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        v[i] = lval[i] ? __ldcs(reinterpret_cast<const float4*>(lp[i])) : make_float4(0.f, 0.f, 0.f, 0.f);
-        lp[i] += BK;
+    for (int c = 0; c < FSTAGES - 1; ++c) fetch(c);
+    int s = 0, ph = 0, w_kc = 0, w_tile = blockIdx.x;
+    const uint8_t* wsrc = p.w_image + (int64_t)(w_tile % n_tiles) * nk * 2 * F::B_PLANE;
+    for (int c = 0; c < nchunks; ++c) {
+      fetch(c + FSTAGES - 1);                                // into the fp32 stage this warp read in iteration c - 1
+      tc::cp_async_wait<FSTAGES - 1>();                      // this lane's copies of chunk c have landed
+      __syncwarp();                                          // ... and every lane's
+      if (c >= STAGES) tc::mbar_wait(&empty[s], ph ^ 1);
+      uint8_t* st = smem + s * F::STAGE;
+      if (pw == 0 && lane == 0) {   // W chunk: one contiguous bulk copy (both planes), counted in bytes on full[s]
+        tc::mbar_arrive_expect_tx(&full[s], 2 * F::B_PLANE);
+        tc::bulk_g2s(st + 2 * F::A_PLANE, wsrc, 2 * F::B_PLANE, &full[s]);
       }
-      if (++l_kc == nk) { l_kc = 0; l_tile += gridDim.x; if (l_tile < total) set_tile_ptrs(l_tile); }
-    };
-    if (nchunks > 0) set_tile_ptrs(l_tile);
+      const uint8_t* fs = blk + (c % FSTAGES) * F::FSTAGE;
 #pragma unroll
-    for (int j = 0; j < PF; ++j)
-      if (j < nchunks) load_next(buf[j]);
-    int s = 0, ph = 0, s_kc = 0, s_tile = blockIdx.x;
-    const uint8_t* wsrc = p.w_image + (int64_t)(s_tile % n_tiles) * nk * 2 * F::B_PLANE;
-    for (int c0 = 0; c0 < nchunks; c0 += PF) {
+      for (int eg = 0; eg < 4; ++eg) {
+        const int row = eg * 8 + e_l;
 #pragma unroll
-      for (int j = 0; j < PF; ++j) {
-        const int c = c0 + j;
-        if (c < nchunks) {
-          if (c >= STAGES) tc::mbar_wait(&empty[s], ph ^ 1);
-          uint8_t* st = smem + s * F::STAGE;
-          if (lt == 0) {   // W chunk: one contiguous bulk copy (both planes), counted in bytes on full[s]
-            tc::mbar_arrive_expect_tx(&full[s], 2 * F::B_PLANE);
-            tc::bulk_g2s(st + 2 * F::A_PLANE, wsrc, 2 * F::B_PLANE, &full[s]);
-          }
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            uint2 hi, lo;
-            tc::split4(buf[j][i], hi, lo);
-            *reinterpret_cast<uint2*>(st + soff[i]) = hi;
-            *reinterpret_cast<uint2*>(st + F::A_PLANE + soff[i]) = lo;
-          }
-          if (c + PF < nchunks) load_next(buf[j]);           // refill this register slot
-          tc::fence_async_smem();
-          __syncwarp();
-          if ((lt & 31) == 0) tc::mbar_arrive(&full[s]);     // one arrival per warp
-          wsrc += 2 * F::B_PLANE;
-          if (++s_kc == nk) {
-            s_kc = 0; s_tile += gridDim.x;
-            wsrc = p.w_image + (int64_t)(s_tile % n_tiles) * nk * 2 * F::B_PLANE;
-          }
-          if (++s == STAGES) { s = 0; ph ^= 1; }
+        for (int h = 0; h < 2; ++h) {
+          const int f = h * 4 + oq;
+          uint2 hi, lo;
+          tc::split4(*reinterpret_cast<const float4*>(fs + row * 128 + ((f + 2 * row) & 7) * 16), hi, lo);
+          const int off = plane_off(pw * 32 + row, f * 4);
+          *reinterpret_cast<uint2*>(st + off) = hi;
+          *reinterpret_cast<uint2*>(st + F::A_PLANE + off) = lo;
         }
       }
+      tc::fence_async_smem();
+      __syncwarp();
+      if (lane == 0) tc::mbar_arrive(&full[s]);              // one arrival per warp
+      wsrc += 2 * F::B_PLANE;
+      if (++w_kc == nk) {
+        w_kc = 0; w_tile += gridDim.x;
+        wsrc = p.w_image + (int64_t)(w_tile % n_tiles) * nk * 2 * F::B_PLANE;
+      }
+      if (++s == STAGES) { s = 0; ph ^= 1; }
     }
     return;   // no block-wide barrier follows
   }
 
-  // ================= consumers: MMA + epilogue =================
-  const int wg = warp >> 2;                                  // rows 64 wg .. 64 wg + 63 of the tile
-  const int wrow = wg * 64 + (warp & 3) * WARP_ROWS;         // this warp's fragment: tile rows wrow .. wrow + 15
-  const bool do_stats = p.stats != nullptr;
-  const int N = p.N;
-  float* stg = reinterpret_cast<float*>(smem + F::PIPE_BYTES) + wrow * F::PITCH;   // this warp's staged rows
-  float* stat = reinterpret_cast<float*>(smem + F::STAT_OFF) + warp * 2 * N;       // this warp's column partials
-  if (do_stats)
-    for (int i = lane; i < 2 * N; i += 32) stat[i] = 0.f;
+  // ================= consumers: MMA + epilogue, local tiles wg, wg + 2, ... =================
+  tc::setmaxnreg_inc<MMA_REGS>();
+  const int wg = warp >> 2, wq = warp & 3;
+  const int wrow = wq * WARP_ROWS;                           // this warp's fragment: rows wrow .. wrow + 15 of each half
+  float* stg = reinterpret_cast<float*>(smem + F::STG_OFF) + warp * WARP_ROWS * F::PITCH;   // this warp's staged rows
+  // Column partials: row h * 4 + wq sums rows 64 h + wrow .. + 15 of every tile of the CTA, tile after tile in tile
+  // order.  The two warpgroups' warps wq share the rows and take turns: stat_bar[wq] completes one phase per tile.
+  float* stat = reinterpret_cast<float*>(smem + F::STAT_OFF);
   const uint32_t sbase = tc::smem_u32(smem);
-  int s = 0, ph = 0;
-  for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+  int li = wg;                                               // local tile index
+  for (int tile = blockIdx.x + wg * gridDim.x; tile < total; tile += 2 * gridDim.x, li += 2) {
     const int m0 = (tile / n_tiles) * BM, n0 = (tile % n_tiles) * BN;
-    // addend row indices of the warp's rows, one per lane, requested before the mainloop
-    int i0 = -1, i1 = -1;
-    {
-      const int gr = m0 + wrow + lane;
+    // addend row indices of the warp's rows, one per lane and half, requested before the mainloop
+    int i0[2] = {-1, -1}, i1[2] = {-1, -1};
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int gr = m0 + h * 64 + wrow + lane;
       if (lane < WARP_ROWS && gr < M) {
-        if (p.add0) i0 = p.idx0 ? __ldg(p.idx0 + gr) : gr;
-        if (p.add1) i1 = p.idx1 ? __ldg(p.idx1 + gr) : gr;
+        if (p.add0) i0[h] = p.idx0 ? __ldg(p.idx0 + gr) : gr;
+        if (p.add1) i1[h] = p.idx1 ? __ldg(p.idx1 + gr) : gr;
       }
     }
-    float acc[BN / 2];
+    const int g = li * nk;                                   // first chunk of this tile in the ring
+    int s = g % STAGES, ph = (g / STAGES) & 1;
+    float acc[2][BN / 2];
 #pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.f;
+    // Warp wq of the other warpgroup has waited for the last chunk of local tile li - 1.  Both hand-off barriers are per
+    // warp pair, one arrival per phase: a warp's own arrival completes the phase before the one it waits for next.
+    if (li > 0) tc::mbar_wait(&mma_turn[wq], (li - 1) & 1);
     int prev = -1;
     for (int kc = 0; kc < nk; ++kc) {
       tc::mbar_wait(&full[s], ph);
@@ -267,13 +280,16 @@ gemm_bf16x3_kernel(const Params p) {
       tc::wgmma_fence();
 #pragma unroll
       for (int j = 0; j < BK / 16; ++j) {
-        const uint32_t a_hi = sa + wg * 8 * SBO + j * 2 * LBO;
         const uint32_t b_hi = sa + 2 * F::A_PLANE + j * 2 * LBO;
-        const uint64_t dah = tc::smem_desc(a_hi, LBO, SBO), dal = tc::smem_desc(a_hi + F::A_PLANE, LBO, SBO);
         const uint64_t dbh = tc::smem_desc(b_hi, LBO, SBO), dbl = tc::smem_desc(b_hi + F::B_PLANE, LBO, SBO);
-        tc::Wgmma<BN>::template mma<0, 0>(acc, dal, dbh, 1);   // small terms first
-        tc::Wgmma<BN>::template mma<0, 0>(acc, dah, dbl, 1);
-        tc::Wgmma<BN>::template mma<0, 0>(acc, dah, dbh, 1);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint32_t a_hi = sa + h * 8 * SBO + j * 2 * LBO;
+          const uint64_t dah = tc::smem_desc(a_hi, LBO, SBO), dal = tc::smem_desc(a_hi + F::A_PLANE, LBO, SBO);
+          tc::Wgmma<BN>::template mma<0, 0>(acc[h], dal, dbh, 1);   // small terms first
+          tc::Wgmma<BN>::template mma<0, 0>(acc[h], dah, dbl, 1);
+          tc::Wgmma<BN>::template mma<0, 0>(acc[h], dah, dbh, 1);
+        }
       }
       tc::wgmma_commit();
       tc::wgmma_wait<1>();                                   // the MMAs of chunk kc - 1 are complete
@@ -284,47 +300,68 @@ gemm_bf16x3_kernel(const Params p) {
       prev = s;
       if (++s == STAGES) { s = 0; ph ^= 1; }
     }
+    if (tile + (int)gridDim.x < total) {                     // local tile li + 1 may start its mainloop
+      __syncwarp();
+      if (lane == 0) tc::mbar_arrive(&mma_turn[wq]);
+    }
     tc::wgmma_wait_all();
     __syncwarp();
     if (lane == 0 && prev >= 0) tc::mbar_arrive(&empty[prev]);
-    // ---- epilogue: stage the fragment (thread holds acc[4 j + 2 h + e] = row lane / 4 + 8 h, column 8 j + 2 (lane % 4)
-    //      + e of the warp's rows), then row by row: (acc + bias) + (addend0 + addend1) ----
-#pragma unroll
-    for (int j = 0; j < BN / 8; ++j)
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-        *reinterpret_cast<float2*>(stg + ((lane >> 2) + 8 * h) * F::PITCH + 8 * j + 2 * (lane & 3)) =
-            make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-    __syncwarp();
+    // ---- epilogue, one row half after the other: stage the fragment (thread holds acc[h][4 j + 2 e + t] = row
+    //      lane / 4 + 8 e, column 8 j + 2 (lane % 4) + t of the warp's rows), then row by row:
+    //      (acc + bias) + (addend0 + addend1) ----
     const int col = n0 + (lane % F::LPR) * 4;
     const float4 b = ld4s(p.bias ? p.bias + col : nullptr);
-    float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f), q4 = s4;
-    epilogue_rows<BN>(stg, p.C, p.ldc, p.add0, p.ld0, p.add1, p.ld1, i0, i1, m0 + wrow, M, col, lane, b, s4, q4);
-    if (do_stats) {
-      // lanes lane % LPR hold the same columns for different rows: fold them, fixed order
+    float4 s4[2], q4[2];
 #pragma unroll
-      for (int o = F::LPR; o < 32; o <<= 1) {
-        s4.x += __shfl_xor_sync(0xffffffffu, s4.x, o); s4.y += __shfl_xor_sync(0xffffffffu, s4.y, o);
-        s4.z += __shfl_xor_sync(0xffffffffu, s4.z, o); s4.w += __shfl_xor_sync(0xffffffffu, s4.w, o);
-        q4.x += __shfl_xor_sync(0xffffffffu, q4.x, o); q4.y += __shfl_xor_sync(0xffffffffu, q4.y, o);
-        q4.z += __shfl_xor_sync(0xffffffffu, q4.z, o); q4.w += __shfl_xor_sync(0xffffffffu, q4.w, o);
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          *reinterpret_cast<float2*>(stg + ((lane >> 2) + 8 * e) * F::PITCH + 8 * j + 2 * (lane & 3)) =
+              make_float2(acc[h][4 * j + 2 * e], acc[h][4 * j + 2 * e + 1]);
+      __syncwarp();
+      s4[h] = make_float4(0.f, 0.f, 0.f, 0.f); q4[h] = s4[h];
+      epilogue_rows<BN>(stg, p.C, p.ldc, p.add0, p.ld0, p.add1, p.ld1, i0[h], i1[h], m0 + h * 64 + wrow, M, col, lane,
+                        b, s4[h], q4[h]);
+      __syncwarp();                                          // staged rows read before they are overwritten
+    }
+    if (do_stats) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        // lanes lane % LPR hold the same columns for different rows: fold them, fixed order
+#pragma unroll
+        for (int o = F::LPR; o < 32; o <<= 1) {
+          s4[h].x += __shfl_xor_sync(0xffffffffu, s4[h].x, o); s4[h].y += __shfl_xor_sync(0xffffffffu, s4[h].y, o);
+          s4[h].z += __shfl_xor_sync(0xffffffffu, s4[h].z, o); s4[h].w += __shfl_xor_sync(0xffffffffu, s4[h].w, o);
+          q4[h].x += __shfl_xor_sync(0xffffffffu, q4[h].x, o); q4[h].y += __shfl_xor_sync(0xffffffffu, q4[h].y, o);
+          q4[h].z += __shfl_xor_sync(0xffffffffu, q4[h].z, o); q4[h].w += __shfl_xor_sync(0xffffffffu, q4[h].w, o);
+        }
       }
+      if (li > 0) tc::mbar_wait(&stat_bar[wq], (li - 1) & 1);   // the other warpgroup has added local tile li - 1
       if (lane < F::LPR) {
-        stat[col] += s4.x; stat[col + 1] += s4.y; stat[col + 2] += s4.z; stat[col + 3] += s4.w;
-        stat[N + col] += q4.x; stat[N + col + 1] += q4.y; stat[N + col + 2] += q4.z; stat[N + col + 3] += q4.w;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float* st = stat + (h * 4 + wq) * 2 * N;
+          st[col] += s4[h].x; st[col + 1] += s4[h].y; st[col + 2] += s4[h].z; st[col + 3] += s4[h].w;
+          st[N + col] += q4[h].x; st[N + col + 1] += q4[h].y; st[N + col + 2] += q4[h].z; st[N + col + 3] += q4[h].w;
+        }
+      }
+      if (tile + (int)gridDim.x < total) {                   // hand the rows to the warp that owns local tile li + 1
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&stat_bar[wq]);
       }
     }
-    __syncwarp();                                            // staged rows read before the next tile overwrites them
   }
   if (do_stats) {
-    // one partial row per CTA: the eight consumer warps' partials summed in a fixed order
+    // one partial row per CTA: the eight column partials summed in a fixed order
     asm volatile("bar.sync 1, %0;" ::"n"(MMA_WARPS * 32) : "memory");
-    const float* all = reinterpret_cast<const float*>(smem + F::STAT_OFF);
     float* out_row = p.stats + (int64_t)blockIdx.x * 2 * N;
     for (int i = tid; i < 2 * N; i += MMA_WARPS * 32) {
       float t = 0.f;
 #pragma unroll
-      for (int w = 0; w < MMA_WARPS; ++w) t += all[w * 2 * N + i];
+      for (int w = 0; w < STAT_ROWS; ++w) t += stat[w * 2 * N + i];
       out_row[i] = t;
     }
   }

@@ -96,6 +96,14 @@ __device__ __forceinline__ void bulk_prefetch_l2(const void* src_gmem, uint32_t 
 // generic-proxy smem writes -> visible to the async proxy (tensor core operand reads)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
+// ---- per-warpgroup register budget ------------------------------------------------------------
+// Executed by all warps of a warpgroup: lower / raise the registers per thread of that warpgroup to N (a multiple of 8
+// in 24 .. 256).  A producer warpgroup gives registers back so that the consumer warpgroups can take them.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---- wgmma (warpgroup MMA, accumulator in registers) ------------------------------------------
 // K-major / MN-major SWIZZLE_NONE shared-memory matrix descriptor (GMMA descriptor bit layout)
 __device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
