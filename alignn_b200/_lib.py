@@ -52,6 +52,8 @@ class EgcBwdArgs(C.Structure):
         ("gx_out", _fp), ("gy_out", _fp),
         ("GM", _fp), ("GP", _fp), ("GSh", _fp),
         ("partials", _fp), ("partials_src", _fp),
+        ("parent_in_ptr", _fp), ("parent_in_eid", _fp), ("parent_out_ptr", _fp), ("parent_out_eid", _fp),
+        ("parent_Nn", C.c_int64),
         ("stream", _fp),
     ]
 

@@ -465,6 +465,66 @@ __device__ __forceinline__ void norm_backward_row(const float (&r)[RowCfg<D>::VP
   }
 }
 
+// Node side of the destination-keyed backward for node v: node-norm backward, GP[v, 3d:4d] = dL/dx', GSh[v] = dL/dSh,
+// and {dL/dSh, dL/dS} of v parked in the warp's shared segment `wseg` [2][D] for its in-edge loop (each lane re-reads
+// only what it wrote).  Shared by egc_backward_dst_kernel and egc_backward_line_kernel so both produce the same bits.
+template <int D, int NORM>
+__device__ __forceinline__ void bwd_node_side(const alignn_b200_egc_bwd_args& a, int64_t v, const float* __restrict__ nvec,
+                                              float* __restrict__ acc, float* __restrict__ wseg, int lane) {
+  using C = RowCfg<D>;
+  constexpr int V = C::VPL;
+  float gsh[V], gs[V];
+  float xp[V], go[V], gxp[V], sv[V], hv[V];
+  ld_row<D, false>(xp, a.XP + v * D, lane);
+  ld_row<D, false>(go, a.gx_out + v * D, lane);
+  norm_backward_row<D, NORM>(xp, go, a.ln_eps, nvec, gxp, acc + 2 * D, acc + 3 * D, lane);
+  st_row<D, false>(a.GP + v * 4 * D + 3 * D, gxp, lane);
+  ld_row<D, false>(sv, a.S + v * D, lane);
+  ld_row<D, false>(hv, a.H + v * D, lane);
+#pragma unroll
+  for (int k = 0; k < V; ++k) {
+    const float inv = 1.f / (sv[k] + a.gate_eps);
+    gsh[k] = gxp[k] * inv;
+    gs[k] = -gxp[k] * hv[k] * inv;
+  }
+  smem_row_add<D>(acc + 4 * D, gxp, lane);
+  st_row<D, false>(a.GSh + v * D, gsh, lane);
+#pragma unroll
+  for (int c = 0; c < C::CH; ++c)
+#pragma unroll
+    for (int j = 0; j < C::W; ++j) {
+      wseg[c * 32 * C::W + lane * C::W + j] = gsh[c * C::W + j];
+      wseg[D + c * 32 * C::W + lane * C::W + j] = gs[c * C::W + j];
+    }
+  __syncwarp();
+}
+
+// One in-edge of the destination whose segment is parked in `wseg`: edge-norm backward (when the edge output is used)
+// plus the gate term, gm = dL/dm; accB += gm.  m / go: the edge's pre-activation and output-gradient rows, cv: Bh[src].
+template <int D, int NORM>
+__device__ __forceinline__ void bwd_edge_gm(const alignn_b200_egc_bwd_args& a, const float (&m)[RowCfg<D>::VPL],
+                                           const float (&go)[RowCfg<D>::VPL], const float (&cv)[RowCfg<D>::VPL],
+                                           const float* __restrict__ evec, float* __restrict__ acc,
+                                           const float* __restrict__ wseg, float (&gm)[RowCfg<D>::VPL],
+                                           float (&accB)[RowCfg<D>::VPL], int lane) {
+  constexpr int V = RowCfg<D>::VPL;
+  if (a.gy_out) {
+    norm_backward_row<D, NORM>(m, go, a.ln_eps, evec, gm, acc, acc + D, lane);
+  } else {
+#pragma unroll
+    for (int k = 0; k < V; ++k) gm[k] = 0.f;
+  }
+  float gsh[V], gs[V];
+  ld_srow<D>(gsh, wseg, lane);
+  ld_srow<D>(gs, wseg + D, lane);
+#pragma unroll
+  for (int k = 0; k < V; ++k) {
+    const float sg = sigmoidf_(m[k]);
+    gm[k] += (gsh[k] * cv[k] + gs[k]) * sg * (1.f - sg);
+    accB[k] += gm[k];
+  }
+}
+
 template <int D, int NORM>   // NORM: the norm mode of both bn_nodes and bn_edges (compile-time: unused vectors vanish)
 __global__ void __launch_bounds__(kThreads)
 egc_backward_dst_kernel(alignn_b200_egc_bwd_args a) {
@@ -493,34 +553,7 @@ egc_backward_dst_kernel(alignn_b200_egc_bwd_args a) {
 
   float* wseg = sseg + wib * 2 * D;
   for (int64_t v = warp0; v < a.Nn; v += nwarps) {
-    {  // node side
-      float gsh[V], gs[V];
-      float xp[V], go[V], gxp[V], sv[V], hv[V];
-      ld_row<D, false>(xp, a.XP + v * D, lane);
-      ld_row<D, false>(go, a.gx_out + v * D, lane);
-      norm_backward_row<D, NORM>(xp, go, a.ln_eps, nvec, gxp, acc + 2 * D, acc + 3 * D, lane);
-      st_row<D, false>(a.GP + v * 4 * D + 3 * D, gxp, lane);
-      ld_row<D, false>(sv, a.S + v * D, lane);
-      ld_row<D, false>(hv, a.H + v * D, lane);
-#pragma unroll
-      for (int k = 0; k < V; ++k) {
-        const float inv = 1.f / (sv[k] + a.gate_eps);
-        gsh[k] = gxp[k] * inv;
-        gs[k] = -gxp[k] * hv[k] * inv;
-      }
-      smem_row_add<D>(acc + 4 * D, gxp, lane);
-      st_row<D, false>(a.GSh + v * D, gsh, lane);
-      // parked in shared memory for the edge loop (each lane re-reads only what it wrote)
-      using C2 = RowCfg<D>;
-#pragma unroll
-      for (int c = 0; c < C2::CH; ++c)
-#pragma unroll
-        for (int j = 0; j < C2::W; ++j) {
-          wseg[c * 32 * C2::W + lane * C2::W + j] = gsh[c * C2::W + j];
-          wseg[D + c * 32 * C2::W + lane * C2::W + j] = gs[c * C2::W + j];
-        }
-      __syncwarp();
-    }
+    bwd_node_side<D, NORM>(a, v, nvec, acc, wseg, lane);
     float accB[V];
 #pragma unroll
     for (int k = 0; k < V; ++k) accB[k] = 0.f;
@@ -550,23 +583,7 @@ egc_backward_dst_kernel(alignn_b200_egc_bwd_args a) {
           ld_row<D, true>(mn, a.M + en * D, lane);
           if (a.gy_out) ld_row<D, true>(gon, a.gy_out + en * D, lane);
         }
-        if (a.gy_out) {
-          norm_backward_row<D, NORM>(m, go, a.ln_eps, evec, gm, acc, acc + D, lane);
-        } else {
-#pragma unroll
-          for (int k = 0; k < V; ++k) gm[k] = 0.f;
-        }
-        {
-          float gsh[V], gs[V];
-          ld_srow<D>(gsh, wseg, lane);
-          ld_srow<D>(gs, wseg + D, lane);
-#pragma unroll
-          for (int k = 0; k < V; ++k) {
-            const float sg = sigmoidf_(m[k]);
-            gm[k] += (gsh[k] * cv[k] + gs[k]) * sg * (1.f - sg);
-            accB[k] += gm[k];
-          }
-        }
+        bwd_edge_gm<D, NORM>(a, m, go, cv, evec, acc, wseg, gm, accB, lane);
         st_row<D, false>(a.GM + e * D, gm, lane);   // re-read by the src-keyed pass and the GEMMs
         if (more) {
 #pragma unroll
@@ -633,9 +650,9 @@ egc_backward_src_kernel(alignn_b200_egc_bwd_args a, float* __restrict__ partials
         ld_row<D, false>(gs0, a.GSh + t0 * D, lane);
         ld_row<D, false>(gs1, a.GSh + t1 * D, lane);
 #pragma unroll
-        for (int k = 0; k < V; ++k) { accA[k] += gm0[k]; accC[k] += gs0[k] * sigmoidf_(m0[k]); }
+        for (int k = 0; k < V; ++k) { accA[k] += gm0[k]; accC[k] = fmaf(gs0[k], sigmoidf_(m0[k]), accC[k]); }
 #pragma unroll
-        for (int k = 0; k < V; ++k) { accA[k] += gm1[k]; accC[k] += gs1[k] * sigmoidf_(m1[k]); }
+        for (int k = 0; k < V; ++k) { accA[k] += gm1[k]; accC[k] = fmaf(gs1[k], sigmoidf_(m1[k]), accC[k]); }
       }
       if (i < cnt) {
         const int64_t e = __shfl_sync(0xffffffffu, my_e, i);
@@ -647,7 +664,7 @@ egc_backward_src_kernel(alignn_b200_egc_bwd_args a, float* __restrict__ partials
 #pragma unroll
         for (int k = 0; k < V; ++k) {
           accA[k] += gm[k];
-          accC[k] += gsh[k] * sigmoidf_(m[k]);
+          accC[k] = fmaf(gsh[k], sigmoidf_(m[k]), accC[k]);
         }
       }
     }
@@ -661,6 +678,199 @@ egc_backward_src_kernel(alignn_b200_egc_bwd_args a, float* __restrict__ partials
     const int extra = blockIdx.x + gridDim.x;              // rows [gridDim.x, partial_rows_total) belong to no block
     if (extra < partial_rows_total)
       for (int i = threadIdx.x; i < 2 * D; i += blockDim.x) partials_src[(int64_t)extra * 2 * D + i] = 0.f;
+  }
+}
+
+// =============================================================================================
+// Backward on a line graph, both passes in one: one CTA per atom of the parent graph g.
+// L(g) has an edge (i -> j) for every pair of bonds with dst(i) == src(j) == a, i != j, emitted destination-major with
+// the sources of each j in the order of a's in-list.  So the L(g) edges at atom a are one complete bipartite block,
+// sources in(a) x destinations out(a) (less the self pair of a self-loop bond), and the CTA that owns a holds ALL the
+// in-edges of its destinations and ALL the out-edges of its sources: it produces GP[j, 2d:4d], GSh[j] and GM of the
+// block exactly as egc_backward_dst_kernel does, and GP[i, 0:2d] exactly as egc_backward_src_kernel does, without
+// reading GM / M back.
+//   Warps own destinations j, kLineWarps at a time, in out-list (= ascending id) order.  The sources i are processed in
+// rounds, all warps on the same source: the warp does the destination-side work of edge (i, j) and stages gm and
+// sigma(m) of that edge in shared memory; after one barrier the CTA adds the staged rows over the warps in ascending j
+// -- the same sequential order and the same fmaf as the source-keyed kernel -- onto the running sums GP[i, 0:2d].  When
+// out(a) takes more than one chunk of warps, the running sums go back to GP[i] between chunks (only this CTA owns them).
+// Edge ids: (in(a)[t], j) is L(g) edge in_ptr_lg[j] + t, minus one after the excluded self pair.
+// partials: [6][D] per CTA as the destination-keyed pass; partials_src: [2][D] per CTA as the source-keyed pass.
+// =============================================================================================
+// 12 warps, one CTA per SM (registers): a 12 x 12 block (k = 12 neighbours) is one chunk, so the running sums never go
+// back through GP and the atom's index chain and node side are paid once.  Measured faster than 6 warps x 2 CTAs and
+// 4 warps x 3 CTAs per SM on the headline L(g); an L2 prefetch of the warp's next edge rows did not help.
+constexpr int kLineWarps = 12;
+constexpr int kLineThreads = kLineWarps * 32;
+
+template <int D>
+constexpr size_t line_bwd_smem_floats() {
+  // sacc [W][6][D], nvec [12][D], wseg [W][2][D], stage [2][W][2][D], ssrc [2][D]
+  return (size_t)(kLineWarps * 6 + 12 + kLineWarps * 2 + 2 * kLineWarps * 2 + 2) * D;
+}
+
+template <int D, int NORM>
+__global__ void __launch_bounds__(kLineThreads, 1)
+egc_backward_line_kernel(alignn_b200_egc_bwd_args a, int partial_rows_total) {
+  using C = RowCfg<D>;
+  constexpr int V = C::VPL;
+  constexpr int W = kLineWarps;
+  extern __shared__ __align__(16) float dyn_smem[];
+  float* sacc = dyn_smem;                        // [W][6][D]: per-warp partial sums of the destination side
+  float* nvec = sacc + W * 6 * D;                // node norm vectors [6][D], then edge norm vectors [6][D]
+  float* evec = nvec + 6 * D;
+  float* sseg = nvec + 12 * D;                   // [W][2][D]: dL/dSh, dL/dS of the warp's destination
+  float* stage = sseg + W * 2 * D;               // [2][W][2][D]: gm, sigma(m) of the round's edge, double-buffered
+  float* ssrc = stage + 2 * W * 2 * D;           // [2][D]: this CTA's sums of GP[:, 0:2d]
+  __shared__ int sself[W];                       // per warp: round of the excluded self pair, or -1
+  {
+    const float* srcs[12] = {a.n_w, a.n_b, a.n_mean, a.n_rstd, a.n_c1, a.n_c2, a.e_w, a.e_b, a.e_mean, a.e_rstd, a.e_c1, a.e_c2};
+#pragma unroll
+    for (int q = 0; q < 12; ++q)
+      for (int i = threadIdx.x; i < D; i += blockDim.x) nvec[q * D + i] = srcs[q] ? srcs[q][i] : 0.f;
+  }
+  for (int i = threadIdx.x; i < W * 6 * D; i += blockDim.x) sacc[i] = 0.f;
+  for (int i = threadIdx.x; i < 2 * D; i += blockDim.x) ssrc[i] = 0.f;
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  float* acc = sacc + wib * 6 * D;
+  float* wseg = sseg + wib * 2 * D;
+  int round = 0;                                 // rounds run by this CTA so far: picks the stage buffer
+
+  for (int64_t at = blockIdx.x; at < a.parent_Nn; at += gridDim.x) {
+    const int ip0 = a.parent_in_ptr[at], kin = a.parent_in_ptr[at + 1] - ip0;
+    const int op0 = a.parent_out_ptr[at], kout = a.parent_out_ptr[at + 1] - op0;
+    if (kout == 0) {                             // sources without out-edges: GP[i, 0:2d] = 0
+      for (int t = 0; t < kin; ++t) {
+        const int64_t i = a.parent_in_eid[ip0 + t];
+        for (int q = threadIdx.x; q < 2 * D; q += blockDim.x) a.GP[i * 4 * D + q] = 0.f;
+      }
+      continue;
+    }
+    for (int c0 = 0; c0 < kout; c0 += W) {
+      const int nd = min(W, kout - c0);
+      const bool last_chunk = c0 + W >= kout;
+      const bool active = wib < nd;
+      __syncthreads();                           // the previous chunk's round sums have read wseg / sself
+      int64_t j = 0, ebase = 0;
+      int selfpos = -1;
+      if (active) {
+        j = a.parent_out_eid[op0 + c0 + wib];
+        ebase = a.in_ptr[j];
+        if (a.in_ptr[j + 1] - ebase != kin) {    // j is a self-loop bond: find it in a's in-list
+          for (int t0 = 0; t0 < kin; t0 += 32) {
+            const bool hit = t0 + lane < kin && a.parent_in_eid[ip0 + t0 + lane] == (int)j;
+            const unsigned bal = __ballot_sync(0xffffffffu, hit);
+            if (bal) { selfpos = t0 + __ffs(bal) - 1; break; }
+          }
+        }
+        if (lane == 0) sself[wib] = selfpos;
+        bwd_node_side<D, NORM>(a, j, nvec, acc, wseg, lane);
+      }
+      auto edge_of = [&](int t) { return ebase + t - ((selfpos >= 0 && t > selfpos) ? 1 : 0); };
+      // the first 32 sources, one per lane: every warp shuffles the round's source from its own copy (t < kin)
+      const int my_i = lane < kin ? a.parent_in_eid[ip0 + lane] : 0;
+      auto source = [&](int t) { return t < 32 ? __shfl_sync(0xffffffffu, my_i, t) : a.parent_in_eid[ip0 + t]; };
+      float accB[V], m[V], go[V], cv[V];
+#pragma unroll
+      for (int k = 0; k < V; ++k) accB[k] = 0.f;
+      // the warp's next edge: its M / gy_out rows and its source's Bh row are requested one round ahead
+      int tn = selfpos == 0 ? 1 : 0;
+      {
+        const int64_t in_ = kin > 0 ? source(min(tn, kin - 1)) : 0;
+        if (active && tn < kin) {
+          const int64_t e = edge_of(tn);
+          ld_row<D, true>(m, a.M + e * D, lane);
+          if (a.gy_out) ld_row<D, true>(go, a.gy_out + e * D, lane);
+          ld_row<D, false>(cv, a.P + in_ * 4 * D + D, lane);
+        }
+      }
+      // this thread's 4 channels of the round sums (2d / 4 <= kLineThreads: at most one float4 per thread)
+      const int q = threadIdx.x * 4;
+      static_assert(2 * D <= 4 * kLineThreads, "one float4 of GP[i, 0:2d] per thread");
+      for (int t = 0; t < kin; ++t, ++round) {
+        const int64_t i = source(t);
+        float* stg = stage + (round & 1) * W * 2 * D;
+        // running sum of GP[i, q:q+4] from the previous chunks (written by this thread), requested before the edge work
+        float4 r = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (c0 > 0 && q < 2 * D) r = *reinterpret_cast<const float4*>(a.GP + i * 4 * D + q);
+        const int tnext = (t + 1 == selfpos) ? t + 2 : t + 1;
+        const int64_t inext = source(min(tnext, kin - 1));
+        if (active && t != selfpos) {
+          const int64_t e = edge_of(t);
+          float gm[V], mn[V], gon[V], cvn[V];
+          if (tnext < kin) {
+            const int64_t en = edge_of(tnext);
+            ld_row<D, true>(mn, a.M + en * D, lane);
+            if (a.gy_out) ld_row<D, true>(gon, a.gy_out + en * D, lane);
+            ld_row<D, false>(cvn, a.P + inext * 4 * D + D, lane);
+          }
+          bwd_edge_gm<D, NORM>(a, m, go, cv, evec, acc, wseg, gm, accB, lane);
+          st_row<D, false>(a.GM + e * D, gm, lane);
+          float sg[V];
+#pragma unroll
+          for (int k = 0; k < V; ++k) sg[k] = sigmoidf_(m[k]);
+#pragma unroll
+          for (int c = 0; c < C::CH; ++c)
+#pragma unroll
+            for (int u = 0; u < C::W; ++u) {
+              stg[wib * 2 * D + c * 32 * C::W + lane * C::W + u] = gm[c * C::W + u];
+              stg[wib * 2 * D + D + c * 32 * C::W + lane * C::W + u] = sg[c * C::W + u];
+            }
+          if (tnext < kin) {
+#pragma unroll
+            for (int k = 0; k < V; ++k) { m[k] = mn[k]; go[k] = gon[k]; cv[k] = cvn[k]; }
+          }
+        }
+        __syncthreads();
+        // GP[i, 0:2d] += this round's edges, warps (= destinations) in ascending order
+        if (q < 2 * D) {
+          if (q < D) {                           // dL/d e_src = sum GM
+            for (int w = 0; w < nd; ++w) {
+              if (t == sself[w]) continue;
+              const float4 g = *reinterpret_cast<const float4*>(stg + w * 2 * D + q);
+              r.x += g.x; r.y += g.y; r.z += g.z; r.w += g.w;
+            }
+          } else {                               // dL/d Bh = sum GSh[j] * sigma(m)
+            for (int w = 0; w < nd; ++w) {
+              if (t == sself[w]) continue;
+              const float4 g = *reinterpret_cast<const float4*>(sseg + w * 2 * D + (q - D));
+              const float4 sg = *reinterpret_cast<const float4*>(stg + w * 2 * D + q);
+              r.x = fmaf(g.x, sg.x, r.x); r.y = fmaf(g.y, sg.y, r.y); r.z = fmaf(g.z, sg.z, r.z); r.w = fmaf(g.w, sg.w, r.w);
+            }
+          }
+          *reinterpret_cast<float4*>(a.GP + i * 4 * D + q) = r;
+          if (last_chunk) {
+            float4* s4 = reinterpret_cast<float4*>(ssrc + q);
+            float4 u = *s4;
+            u.x += r.x; u.y += r.y; u.z += r.z; u.w += r.w;
+            *s4 = u;
+          }
+        }
+      }
+      if (active) {
+        st_row<D, false>(a.GP + j * 4 * D + 2 * D, accB, lane);
+        smem_row_add<D>(acc + 5 * D, accB, lane);
+      }
+    }
+  }
+  __syncthreads();
+  if (a.partials) {                              // fixed-order sum over the CTA's warps -> one partial row
+    float* out_row = a.partials + (int64_t)blockIdx.x * 6 * D;
+    for (int i = threadIdx.x; i < 6 * D; i += blockDim.x) {
+      float t = 0.f;
+#pragma unroll
+      for (int w = 0; w < W; ++w) t += sacc[w * 6 * D + i];
+      out_row[i] = t;
+    }
+  }
+  if (a.partials_src)
+    for (int i = threadIdx.x; i < 2 * D; i += blockDim.x) a.partials_src[(int64_t)blockIdx.x * 2 * D + i] = ssrc[i];
+  // rows [gridDim.x, partial_rows_total) belong to no CTA
+  for (int64_t r = blockIdx.x + gridDim.x; r < partial_rows_total; r += gridDim.x) {
+    if (a.partials)
+      for (int i = threadIdx.x; i < 6 * D; i += blockDim.x) a.partials[r * 6 * D + i] = 0.f;
+    if (a.partials_src)
+      for (int i = threadIdx.x; i < 2 * D; i += blockDim.x) a.partials_src[r * 2 * D + i] = 0.f;
   }
 }
 
@@ -1148,6 +1358,35 @@ int alignn_b200_egc_backward(const alignn_b200_egc_bwd_args* a) {
   cudaStream_t st = (cudaStream_t)a->stream;
   const int grid = grid_for_rows(a->Nn);
   if (a->norm_nodes != a->norm_edges) return ALIGNN_ERR_BAD_ARG;   // both norms of a conv are of one kind (alignn.py:71-76)
+  const bool line = a->parent_in_ptr || a->parent_in_eid || a->parent_out_ptr || a->parent_out_eid || a->parent_Nn;
+  if (line) {
+    // one pass per atom of the parent graph (egc_backward_line_kernel); `grid` partial rows, as the two-pass path
+    if (!a->parent_in_ptr || !a->parent_out_ptr || a->parent_Nn <= 0 ||
+        (a->Nn > 0 && (!a->parent_in_eid || !a->parent_out_eid)) || (a->Ne > 0 && (!a->M || !a->GM)))
+      return ALIGNN_ERR_BAD_ARG;
+#define LAUNCH_BWD_LINE(NORM)                                                                                   \
+  DISPATCH_D(a->d, {                                                                                           \
+    const size_t smem_bytes = alignn::line_bwd_smem_floats<D>() * sizeof(float);                               \
+    static alignn::DeviceOnce configured; int cfg_dev;                                                         \
+    if (configured.needed(&cfg_dev)) {                                                                         \
+      cudaError_t e = cudaFuncSetAttribute(alignn::egc_backward_line_kernel<D, NORM>,                          \
+                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);      \
+      if (e != cudaSuccess) return alignn::record_cuda_error((int)e);                                          \
+      configured.done(cfg_dev);                                                                                \
+    }                                                                                                          \
+    const int64_t want = a->parent_Nn < grid ? a->parent_Nn : grid;                                            \
+    const int grid_line = alignn::one_wave_grid((const void*)alignn::egc_backward_line_kernel<D, NORM>,        \
+                                                alignn::kLineThreads, smem_bytes, (int)want);                  \
+    alignn::egc_backward_line_kernel<D, NORM><<<grid_line, alignn::kLineThreads, smem_bytes, st>>>(*a, grid);  \
+  })
+    switch (a->norm_nodes) {
+      case ALIGNN_NORM_LAYER: LAUNCH_BWD_LINE(ALIGNN_NORM_LAYER); break;
+      case ALIGNN_NORM_AFFINE: LAUNCH_BWD_LINE(ALIGNN_NORM_AFFINE); break;
+      default: LAUNCH_BWD_LINE(ALIGNN_NORM_STATS); break;
+    }
+#undef LAUNCH_BWD_LINE
+    return check_launch();
+  }
 #define LAUNCH_BWD_DST(NORM)                                                                                   \
   DISPATCH_D(a->d, {                                                                                           \
     const size_t smem_bytes = (size_t)(alignn::kWarpsPerBlock * 8 + 12) * D * sizeof(float);                   \

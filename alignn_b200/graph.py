@@ -32,18 +32,24 @@ def _np(a):
 
 
 class EdgeIndex:
-    """Sorted-CSR edge index of one graph (both orientations), int32 tensors."""
+    """Sorted-CSR edge index of one graph (both orientations), int32 tensors.
+
+    `parent`: set only by `Graph.line_graph()` on the L(g) it emits -- the parent g's (in_ptr, in_eid, out_ptr,
+    out_eid).  It asserts that this graph is exactly the builders' L(g) of that parent, so the edges at each atom of g
+    form one bipartite block (sources in(a), destinations out(a)); `ops.egc_backward` then runs the one-pass
+    line-graph backward.  None everywhere else (atom graphs, `batch`, `unbatch`, `as_graph`, `reverse`)."""
 
     __slots__ = ("src", "dst", "in_ptr", "in_eid", "out_ptr", "out_eid", "dst_sorted",
-                 "max_in_deg", "num_nodes")
+                 "max_in_deg", "num_nodes", "parent")
 
-    def __init__(self, src, dst, in_ptr, in_eid, out_ptr, out_eid, dst_sorted, max_in_deg, num_nodes):
+    def __init__(self, src, dst, in_ptr, in_eid, out_ptr, out_eid, dst_sorted, max_in_deg, num_nodes, parent=None):
         self.src, self.dst = src, dst
         self.in_ptr, self.in_eid = in_ptr, in_eid
         self.out_ptr, self.out_eid = out_ptr, out_eid
         self.dst_sorted = bool(dst_sorted)
         self.max_in_deg = int(max_in_deg)
         self.num_nodes = int(num_nodes)
+        self.parent = None if parent is None else tuple(parent)
 
     @staticmethod
     def build(src: np.ndarray, dst: np.ndarray, num_nodes: int) -> "EdgeIndex":
@@ -99,14 +105,17 @@ class EdgeIndex:
 
     def to(self, device, non_blocking=False) -> "EdgeIndex":
         moved = [getattr(self, f).to(device, non_blocking=non_blocking) for f in self._FIELDS]
-        return EdgeIndex(*moved, self.dst_sorted, self.max_in_deg, self.num_nodes)
+        parent = None if self.parent is None else [t.to(device, non_blocking=non_blocking) for t in self.parent]
+        return EdgeIndex(*moved, self.dst_sorted, self.max_in_deg, self.num_nodes, parent)
 
     def pin_memory(self) -> "EdgeIndex":
         moved = [getattr(self, f).pin_memory() for f in self._FIELDS]
-        return EdgeIndex(*moved, self.dst_sorted, self.max_in_deg, self.num_nodes)
+        parent = None if self.parent is None else [t.pin_memory() for t in self.parent]
+        return EdgeIndex(*moved, self.dst_sorted, self.max_in_deg, self.num_nodes, parent)
 
     def nbytes(self) -> int:
-        return sum(getattr(self, f).numel() * 4 for f in self._FIELDS)
+        n = sum(getattr(self, f).numel() * 4 for f in self._FIELDS)
+        return n + (0 if self.parent is None else sum(t.numel() * 4 for t in self.parent))
 
 
 class _EdgeBatch:
@@ -250,6 +259,7 @@ class Graph:
         _lib.check(lib.alignn_b200_line_graph_build_host(p(src), p(in_ptr), p(in_eid), E, p(bne), bne.shape[0], T,
                                                          p(li), p(lj), p(lbne)), "alignn_b200_line_graph_build_host")
         lg = Graph(li, lj, E, self._bne.clone(), lbne)
+        lg.index.parent = (ix.in_ptr, ix.in_eid, ix.out_ptr, ix.out_eid)
         if self.device.type != "cpu":
             lg = lg.to(self.device)
         if shared:
@@ -280,6 +290,7 @@ class Graph:
                        "alignn_b200_line_graph_fill")
         lbne = torch.tensor([b - a for a, b in zip(at[:-1], at[1:])], dtype=torch.int64)
         lg = Graph(lsrc, ldst, E, self._bne.clone(), lbne)
+        lg.index.parent = (ix.in_ptr, ix.in_eid, ix.out_ptr, ix.out_eid)
         if shared:
             lg.ndata.update(self.edata)
         return lg

@@ -222,9 +222,20 @@ def egc_backward(ix: EdgeIndex, P, M, XP, S, H, gx_out, gy_out, n, e, *, reduce:
         n_c1=g(n, "c1"), n_c2=g(n, "c2"), e_c1=g(e, "c1"), e_c2=g(e, "c2"),
         gx_out=ptr(gx_out), gy_out=ptr(gy_out), GM=ptr(GM), GP=ptr(GP), GSh=ptr(GSh),
         partials=ptr(part), partials_src=ptr(part_src), stream=stream_ptr())
-    # destination-keyed pass reads M, gy_out, node rows and writes GM, GP; source-keyed pass reads GM, M: SURVEY 8d
-    nb = 4 * d * (Ne * (2 + (gy_out is not None)) + 9 * Nn) + 12 * Ne + 4 * d * 2 * Ne
-    with _span("egc_backward(dst+src)", nb):
+    if ix.parent is not None:
+        # L(g) of a parent graph: one pass per parent atom (include/alignn_b200.h).  Compulsory bytes: M, gy_out read
+        # and GM written once; node rows XP, gx_out, S, H, Bh read and GP [4d], GSh written; parent CSR + L(g) in_ptr.
+        pin, peid, pout, poeid = ix.parent
+        require_cuda(pin, peid, pout, poeid)
+        a.parent_in_ptr, a.parent_in_eid, a.parent_out_ptr, a.parent_out_eid = ptr(pin), ptr(peid), ptr(pout), ptr(poeid)
+        a.parent_Nn = pin.numel() - 1
+        name = "egc_backward(line)"
+        nb = 4 * d * (Ne * (2 + (gy_out is not None)) + 10 * Nn) + 4 * (2 * pin.numel() + 2 * Nn + Nn + 1)
+    else:
+        # destination-keyed pass reads M, gy_out, node rows and writes GM, GP; source-keyed pass reads GM, M: SURVEY 8d
+        name = "egc_backward(dst+src)"
+        nb = 4 * d * (Ne * (2 + (gy_out is not None)) + 9 * Nn) + 12 * Ne + 4 * d * 2 * Ne
+    with _span(name, nb):
         _lib.check(lib.alignn_b200_egc_backward(C.byref(a)), "alignn_b200_egc_backward")
     extra = (GSh,) if keep_gsh else ()
     if not reduce:              # the caller sums the per-block partial rows itself (WgradQueue: one batched launch per backward)

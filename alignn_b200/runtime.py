@@ -137,6 +137,11 @@ class BucketedForward:
         # line graph never does (Graph.line_graph emits destination-sorted edges)
         if dst.index.dst_sorted and not src.index.dst_sorted:
             raise RuntimeError("BucketedForward: line graph of the batch is not destination-sorted")
+        # the line-graph descriptor (parent CSR of the padded batch) has the bucket's shapes too
+        if (dst.index.parent is None) != (src.index.parent is None):
+            raise RuntimeError("BucketedForward: line-graph descriptor present in only one of the batches")
+        for t, u in zip(dst.index.parent or (), src.index.parent or ()):
+            t.copy_(u, non_blocking=True)
         dst.index.max_in_deg = src.index.max_in_deg
         dst._seg.copy_(src._seg, non_blocking=True)
         dst._bnn, dst._bne = src._bnn, src._bne

@@ -164,6 +164,16 @@ typedef struct {
   float* partials;
   /* per-block partials of the source-keyed pass, [partial_rows, 2, d] = {sum dL/d e_src, sum dL/d Bh} */
   float* partials_src;
+  /* Line-graph descriptor, optional.  When this graph is L(g) of a parent graph g EXACTLY as the line-graph builders
+     emit it (alignn_b200_line_graph_build_host / alignn_b200_line_graph_fill, then the CSR build: node i of L(g) is
+     bond i of g; an edge (i -> j) for every pair with dst(i) == src(j), i != j; edges sorted by (j, position of i in
+     the in-list of g), so in_eid is the identity and may be NULL), the parent's CSR (in_ptr, in_eid, out_ptr, out_eid
+     of g, int32) and its node count may be given: one kernel then runs over the atoms of g and produces everything
+     in one pass over the edge rows, bit-identical GM, GP and GSh; the per-block partial rows are grouped differently
+     (same buffer shapes; rows no block owns are zeroed).  All NULL / 0: the destination- and source-keyed kernels. */
+  const int32_t* parent_in_ptr; const int32_t* parent_in_eid;
+  const int32_t* parent_out_ptr; const int32_t* parent_out_eid;
+  int64_t parent_Nn;
   alignn_stream_t stream;
 } alignn_b200_egc_bwd_args;
 
