@@ -7,3 +7,4 @@ library (include/alignn_b200.h).  See DESIGN.md.
 __version__ = "0.1.0"
 
 from .graph import Graph, batch, unbatch, reverse, graph, as_graph, bond_cosines  # noqa: F401
+from .ealignn_atomwise import eALIGNNAtomWise, eALIGNNAtomWiseConfig  # noqa: F401,E402

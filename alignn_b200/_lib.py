@@ -157,6 +157,12 @@ _SIGNATURES = {
     "alignn_b200_radius_graph_fill": (C.c_int, [_fp, _fp, C.c_int64, C.c_int64, C.c_double, C.c_double, _fp, _fp, _fp, _fp, _fp, _fp]),
     "alignn_b200_pair_force_scatter": (C.c_int, [_fp, _fp, _fp, _fp, _fp, C.c_int64, C.c_int, _fp, _fp]),
     "alignn_b200_virial_stress": (C.c_int, [_fp, _fp, _fp, _fp, _fp, C.c_int64, C.c_float, _fp, _fp]),
+    "alignn_b200_bond_cutoff_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "alignn_b200_bond_cutoff_offsets": (C.c_int, [_fp, _fp, _fp, _fp, C.c_int64, C.c_float, _fp, _fp, _fp, C.c_size_t, _fp]),
+    "alignn_b200_bond_cutoff_fill": (C.c_int, [_fp, _fp, _fp, _fp, _fp, _fp, C.c_int64, C.c_int64, _fp, _fp, _fp, _fp, _fp,
+                                               _fp]),
+    "alignn_b200_remove_net_torque_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "alignn_b200_remove_net_torque": (C.c_int, [_fp, _fp, _fp, C.c_int64, C.c_int64, C.c_int, _fp, _fp, C.c_size_t, _fp]),
     "alignn_b200_debug_egc_flags": (None, [C.c_int]),
     "alignn_b200_segment_mean": (C.c_int, [_fp, _fp, C.c_int64, C.c_int, _fp, _fp]),
     "alignn_b200_segment_mean_backward": (C.c_int, [_fp, _fp, C.c_int64, C.c_int, _fp, _fp]),

@@ -131,6 +131,7 @@ class ALIGNNAtomWise(nn.Module):
     (alignn_b200_egc_backward_vjp); the embedding MLPs, pooling and force / virial reductions are torch operators there.
     Stress: the batched virial of :610-638 (`batch_stress=True`, the default) from the same pair forces.
     Cutoff envelope on the bond lengths (`use_cutoff_function`, both `multiply_cutoff` settings, :434-451).
+    `forward((g, lat))` builds L(g) inside forward (:379-386; on the device for a CUDA graph).
     Not built (SURVEY.md section 8f): `batch_stress=False` (:573-590), include_pos_deriv.
     """
 
@@ -183,10 +184,17 @@ class ALIGNNAtomWise(nn.Module):
     def _forward(self, g, second: bool):
         c = self.config
         if len(self.alignn_layers) > 0:
-            if len(g) != 3:
-                raise NotImplementedError("pass (g, lg, lat); building L(g) inside forward is not part of the built path")
-            g, lg, lat = g
-            lg = as_graph(lg)
+            if len(g) == 3:
+                g, lg, lat = g
+                lg = as_graph(lg)
+            else:
+                # (g, lat): L(g) built here (:379-386), on the device for a CUDA graph; its cosines come from r below
+                if not c.lg_on_fly:
+                    raise ValueError("ALIGNNAtomWise((g, lat)) builds L(g) inside forward and needs lg_on_fly=True for "
+                                     "its bond angles; pass (g, lg, lat) otherwise")
+                g, lat = g
+                g = as_graph(g)
+                lg = g.line_graph(shared=True)
         else:
             g, lat = g[0], g[-1]
             lg = None

@@ -22,7 +22,7 @@ from typing import Optional, Sequence
 import numpy as np
 import torch
 
-__all__ = ["Graph", "EdgeIndex", "batch", "unbatch", "reverse", "graph", "as_graph", "bond_cosines"]
+__all__ = ["Graph", "EdgeIndex", "batch", "unbatch", "reverse", "graph", "as_graph", "bond_cosines", "lightweight_graph"]
 
 
 def _np(a):
@@ -388,6 +388,30 @@ def as_graph(g) -> Graph:
     out.ndata.update(dict(g.ndata))
     out.edata.update(dict(g.edata))
     return out
+
+
+def lightweight_graph(g: Graph, cart: torch.Tensor, inner_cutoff: float):
+    """The bonds of a CUDA graph `g` no longer than `inner_cutoff`, as eALIGNN builds them inside forward
+    (`lightweight_line_graph` with `compute_pair_vector_and_distance`, alignn/models/utils.py:47-55, 129-222):
+    r = (cart[dst] + edata["images"]) - cart[src] in fp32, bonds with |r| > inner_cutoff dropped, order kept.
+    Returns (filtered Graph, r' [E',3]).  The filtered graph shares `ndata`, holds `edata` filtered to the kept bonds plus
+    `edge_ids` (crystal-local ids when the batch has several crystals, global ids otherwise, as the reference numbers
+    them) and the kept bonds per crystal in batch_num_edges.  Its index is built on the device, so its
+    `line_graph()` also runs there and carries the parent descriptor."""
+    from . import ops
+    if g.device.type != "cuda":
+        raise RuntimeError("lightweight_graph needs a CUDA graph (the filter is a device kernel)")
+    eoff = g.edge_graph_offsets64()
+    src, dst, r, _, eids, kept = ops.bond_cutoff_filter(cart, g.index, g.edata["images"], eoff, inner_cutoff)
+    glob = eids
+    if g.batch_size > 1:                                    # crystal-local ids -> positions in g
+        gid = torch.repeat_interleave(torch.arange(g.batch_size, device=g.device), kept.to(g.device), output_size=eids.numel())
+        glob = eids + eoff[gid]
+    out = Graph(src, dst, g.num_nodes(), g.batch_num_nodes(), kept)
+    out.ndata.update(g.ndata)
+    out.edata = {k: v[glob] for k, v in g.edata.items()}
+    out.edata["edge_ids"] = eids
+    return out, r
 
 
 def bond_cosines(r: torch.Tensor, lg: Graph) -> torch.Tensor:

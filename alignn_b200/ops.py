@@ -333,6 +333,55 @@ def virial_stress(r: torch.Tensor, pair_forces: torch.Tensor, edge_offsets64: to
     return out
 
 
+@_on_tensor_device
+def bond_cutoff_filter(cart: torch.Tensor, ix: EdgeIndex, images: torch.Tensor, edge_offsets64: torch.Tensor,
+                       cutoff: float):
+    """Bonds of `ix` no longer than `cutoff`, with r = (cart[dst] + images) - cart[src] recomputed in fp32
+    (`lightweight_line_graph` + `compute_pair_vector_and_distance`, alignn/models/utils.py:47-55, 129-222).
+    Returns (src', dst', r', images', edge_ids, kept bonds per crystal as a host int64 tensor); one read-back of the
+    B+1 kept-bond boundaries sizes the outputs."""
+    lib = _lib.load()
+    cart, images = cart.contiguous(), images.contiguous().to(torch.float32)
+    require_cuda(cart, images, ix.src, ix.dst)
+    E, dev, B = ix.src.numel(), cart.device, edge_offsets64.numel() - 1
+    r = torch.empty(E, 3, device=dev, dtype=torch.float32)
+    off = torch.empty(E + 1, device=dev, dtype=torch.int32)
+    nb = int(lib.alignn_b200_bond_cutoff_workspace_bytes(E))
+    if nb == 0:
+        raise ValueError("graph too large for int32 edge index")
+    ws = torch.empty(nb, device=dev, dtype=torch.uint8)
+    st = stream_ptr()
+    _lib.check(lib.alignn_b200_bond_cutoff_offsets(ptr(cart), ptr(ix.src), ptr(ix.dst), ptr(images), E, float(cutoff), ptr(r),
+                                                   ptr(off), ptr(ws), nb, st), "alignn_b200_bond_cutoff_offsets")
+    at = off[edge_offsets64].cpu()                            # kept bonds before each crystal's first bond; last = E'
+    Ek = int(at[-1])
+    i32 = lambda: torch.empty(Ek, device=dev, dtype=torch.int32)  # noqa: E731
+    src, dst = i32(), i32()
+    r_k, img_k = (torch.empty(Ek, 3, device=dev, dtype=torch.float32) for _ in range(2))
+    eids = torch.empty(Ek, device=dev, dtype=torch.int64)
+    _lib.check(lib.alignn_b200_bond_cutoff_fill(ptr(ix.src), ptr(ix.dst), ptr(r), ptr(images), ptr(off), edge_offsets64.data_ptr(),
+                                                B, E, ptr(src), ptr(dst), ptr(r_k), ptr(img_k), eids.data_ptr(), st),
+               "alignn_b200_bond_cutoff_fill")
+    return src, dst, r_k, img_k, eids, (at[1:] - at[:-1]).long()
+
+
+@_on_tensor_device
+def remove_net_torque(pos: torch.Tensor, forces: torch.Tensor, node_offsets64: torch.Tensor) -> torch.Tensor:
+    """Forces with the batch's net torque removed (`remove_net_torque`, alignn/models/utils.py:295-398; batch-wide
+    centre and torque, one 3x3 solve per crystal in double, pseudo-inverse for an exactly singular system).  A batch of
+    exactly 3 atoms crosses along dim 0, as torch.cross without `dim` does there."""
+    lib = _lib.load()
+    pos, forces = pos.contiguous(), forces.contiguous()
+    require_cuda(pos, forces)
+    N, B = forces.shape[0], node_offsets64.numel() - 1
+    out = torch.empty(N, 3, device=forces.device, dtype=torch.float32)
+    nb = int(lib.alignn_b200_remove_net_torque_workspace_bytes(B))
+    ws = torch.empty(nb, device=forces.device, dtype=torch.uint8)
+    _lib.check(lib.alignn_b200_remove_net_torque(ptr(pos), ptr(forces), node_offsets64.data_ptr(), B, N, int(N == 3), ptr(out),
+                                                 ptr(ws), nb, stream_ptr()), "alignn_b200_remove_net_torque")
+    return out
+
+
 class _SegmentMean(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, gptr):

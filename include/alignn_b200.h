@@ -466,6 +466,43 @@ int alignn_b200_virial_stress(const float* r, const float* pair_forces, const in
                               const int64_t* node_offsets, const float* V, int64_t batch_size, float multiplier,
                               float* stress, alignn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * eALIGNN force-field steps (csrc/ff_device.cu).  Device pointers, caller-owned buffers, enqueue-only on `stream`.
+ * ---------------------------------------------------------------------------------------- */
+/* Bond cutoff filter = `lightweight_line_graph(g, "bondlength", gt inner_cutoff)` with the bond vectors of
+ * `compute_pair_vector_and_distance` (alignn/models/utils.py:47-55, 129-222; called at ealignn_atomwise.py:309-318).
+ * offsets: r[e] = (cart_coords[dst[e]] + images[e]) - cart_coords[src[e]] in fp32, one component at a time in that order
+ *   (bit-identical to torch), r [E,3]; bond e is dropped iff |r[e]| > cutoff (a NaN length is kept, as torch.gt is false
+ *   for NaN); offsets[E+1] = exclusive scan of the keep flags, offsets[E] = kept bonds.  |r| is computed in fp32 and may
+ *   round differently from torch.norm: a bond within an ulp of the cutoff may be classified differently.
+ * fill: the kept bonds in their original order -> src_out / dst_out / r_out [E',3] / images_out [E',3], and edge_ids
+ *   [E'] int64 numbered as the reference does (utils.py:159-179, 206): the bond's index inside its crystal when
+ *   batch_size > 1, its global index otherwise.  edge_offsets [batch_size+1] int64 = prefix of batch_num_edges.  Read
+ *   offsets back at edge_offsets to get E' and the kept bonds per crystal. */
+size_t alignn_b200_bond_cutoff_workspace_bytes(int64_t num_edges);
+int alignn_b200_bond_cutoff_offsets(const float* cart_coords, const int32_t* src, const int32_t* dst, const float* images,
+                                    int64_t num_edges, float cutoff, float* r, int32_t* offsets, void* workspace,
+                                    size_t workspace_bytes, alignn_stream_t stream);
+int alignn_b200_bond_cutoff_fill(const int32_t* src, const int32_t* dst, const float* r, const float* images,
+                                 const int32_t* offsets, const int64_t* edge_offsets, int64_t batch_size, int64_t num_edges,
+                                 int32_t* src_out, int32_t* dst_out, float* r_out, float* images_out, int64_t* edge_ids,
+                                 alignn_stream_t stream);
+
+/* Net-torque removal = `remove_net_torque` (alignn/models/utils.py:295-398, ealignn_atomwise.py:409-412), quirks kept:
+ * com = mean of ALL positions of the batch, r_i = pos_i - com, tau = sum over the WHOLE batch of r_i x F_i; per crystal
+ * b: M_b = sum r_i r_i^T - (sum |r_i|^2) I, mu_b = M_b^{-1} (-tau) (the same tau for every crystal);
+ * out_i = F_i + r_i x mu_b.  pos / forces / out [N,3] fp32, node_offsets [B+1] int64.  Sums in double with fixed-order
+ * block partials; each 3x3 system is solved in double by LU with partial pivoting, and by the pseudo-inverse
+ * (symmetric eigendecomposition, eigenvalues below 3 eps max|lambda| dropped) when a pivot is exactly zero.  The
+ * reference switches the WHOLE batch to the pseudo-inverse when any crystal is singular; choosing per crystal differs
+ * from that by rounding only.  (That branch of the reference raises an IndexError on its 1-D right-hand side; this call
+ * computes what it means.)  cross_dim0 = 1 (only valid with N == 3): torch.cross without `dim` crosses along dim 0
+ * of the [3,3] tensors, i.e. the columns, and so does this call. */
+size_t alignn_b200_remove_net_torque_workspace_bytes(int64_t batch_size);
+int alignn_b200_remove_net_torque(const float* pos, const float* forces, const int64_t* node_offsets, int64_t batch_size,
+                                  int64_t num_nodes, int cross_dim0, float* out, void* workspace, size_t workspace_bytes,
+                                  alignn_stream_t stream);
+
 /* Per-graph mean over node rows (dgl.nn.AvgPooling, alignn.py:325) and its backward. */
 int alignn_b200_segment_mean(const float* x, const int32_t* graph_ptr /*[B+1]*/, int64_t B, int d, float* out,
                              alignn_stream_t stream);
