@@ -106,6 +106,13 @@ class BiasEntry(C.Structure):
     _fields_ = [("a", _fp), ("b", _fp), ("dst", _fp), ("n", C.c_int32)]
 
 
+class CrystalBatch(C.Structure):
+    _fields_ = [("cart_coords", _fp), ("shifts", _fp), ("cells", _fp), ("lattices", _fp), ("atom_offsets", _fp),
+                ("shift_offsets", _fp), ("crystal_of_atom", _fp), ("cutoffs", _fp),
+                ("num_crystals", C.c_int64), ("num_atoms", C.c_int64), ("num_images", C.c_int64), ("max_images", C.c_int64),
+                ("atol", C.c_double)]
+
+
 # name -> (restype, argtypes); mirrors include/alignn_b200.h one to one
 _SIGNATURES = {
     "alignn_b200_version": (C.c_int, []),
@@ -155,6 +162,15 @@ _SIGNATURES = {
     "alignn_b200_radius_graph_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "alignn_b200_radius_graph_offsets": (C.c_int, [_fp, _fp, C.c_int64, C.c_int64, C.c_double, C.c_double, _fp, _fp, C.c_size_t, _fp]),
     "alignn_b200_radius_graph_fill": (C.c_int, [_fp, _fp, C.c_int64, C.c_int64, C.c_double, C.c_double, _fp, _fp, _fp, _fp, _fp, _fp]),
+    "alignn_b200_crystal_scan_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "alignn_b200_crystal_scan_count": (C.c_int, [C.POINTER(CrystalBatch), C.c_int, _fp, _fp, _fp, C.c_size_t, _fp]),
+    "alignn_b200_crystal_radius_fill": (C.c_int, [C.POINTER(CrystalBatch), _fp, _fp, _fp, _fp, _fp, _fp]),
+    "alignn_b200_knn_graph_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int64]),
+    "alignn_b200_knn_graph_select": (C.c_int, [C.POINTER(CrystalBatch), _fp, C.c_int64, C.c_int, _fp, _fp, C.c_size_t, _fp]),
+    "alignn_b200_knn_graph_order": (C.c_int, [C.POINTER(CrystalBatch), _fp, _fp, C.c_int64, C.c_int64, _fp, _fp, C.c_size_t,
+                                              _fp]),
+    "alignn_b200_knn_graph_emit": (C.c_int, [C.POINTER(CrystalBatch), _fp, C.c_int64, C.c_int64, _fp, _fp, _fp, _fp, _fp,
+                                             C.c_size_t, _fp]),
     "alignn_b200_pair_force_scatter": (C.c_int, [_fp, _fp, _fp, _fp, _fp, C.c_int64, C.c_int, _fp, _fp]),
     "alignn_b200_virial_stress": (C.c_int, [_fp, _fp, _fp, _fp, _fp, C.c_int64, C.c_float, _fp, _fp]),
     "alignn_b200_bond_cutoff_workspace_bytes": (C.c_size_t, [C.c_int64]),

@@ -1,5 +1,6 @@
 // Device-side structure builders and the force / stress reductions of SURVEY.md section 8f -- the GPU twins of
-// csrc/graph_host.cu (sorted-CSR index, line graph, periodic radius scan; bit-identical outputs) and
+// csrc/graph_host.cu (sorted-CSR index, line graph; bit-identical outputs; the periodic scans are in
+// csrc/crystal_graph_device.cu) and
 // the d=3 reductions of ALIGNN-FF (alignn/models/alignn_atomwise.py:547-563, 610-635).  Pure integer work except the two d=3 reductions; everything deterministic
 // (stable radix sort, fixed-order sums, integer atomics only for counting).  CUB (ships with the CUDA toolkit) does
 // the scans and the stable key-value sort; it is plumbing here, like cudart.
@@ -108,45 +109,6 @@ __global__ void lg_fill_kernel(const int32_t* __restrict__ src, const int32_t* _
     lsrc[o + k] = i;
     ldst[o + k] = (int32_t)j;
   }
-}
-
-// ---- periodic radius graph (alignn/graphs.py:267-364) -----------------------------------------------
-// One warp per home-cell atom u walks (image c, atom v) in the host builder's order; 32 candidates per step, a ballot
-// gives each hit its ordered slot.  Double precision with explicit round-to-nearest operations (no FMA contraction),
-// the same operation order as csrc/graph_host.cu: d = (shift + x_v) - x_u ; dist = sqrt((dx*dx + dy*dy) + dz*dz).
-template <bool kFill>
-__global__ void radius_scan_kernel(const double* __restrict__ X, const double* __restrict__ shifts, int64_t n, int64_t n_images,
-                                   double cutoff, double atol, const int32_t* __restrict__ off, int32_t* __restrict__ cnt,
-                                   int32_t* __restrict__ u_out, int32_t* __restrict__ v_out, int32_t* __restrict__ c_out,
-                                   float* __restrict__ r_out) {
-  const int lane = threadIdx.x & 31;
-  const int64_t u = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  if (u >= n) return;
-  const double xu = X[3 * u], yu = X[3 * u + 1], zu = X[3 * u + 2];
-  int32_t t = kFill ? off[u] : 0;
-  for (int64_t c = 0; c < n_images; ++c) {
-    const double sx = shifts[3 * c], sy = shifts[3 * c + 1], sz = shifts[3 * c + 2];
-    for (int64_t v0 = 0; v0 < n; v0 += 32) {
-      const int64_t v = v0 + lane;
-      bool hit = false;
-      double dx = 0.0, dy = 0.0, dz = 0.0;
-      if (v < n) {
-        dx = __dsub_rn(__dadd_rn(sx, X[3 * v]), xu);
-        dy = __dsub_rn(__dadd_rn(sy, X[3 * v + 1]), yu);
-        dz = __dsub_rn(__dadd_rn(sz, X[3 * v + 2]), zu);
-        const double dist = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)));
-        hit = dist <= cutoff && !(fabs(dist) <= atol);
-      }
-      const unsigned m = __ballot_sync(0xffffffffu, hit);
-      if (kFill && hit) {
-        const int32_t k = t + __popc(m & ((1u << lane) - 1u));
-        u_out[k] = (int32_t)u; v_out[k] = (int32_t)v; c_out[k] = (int32_t)c;
-        r_out[3 * k] = (float)dx; r_out[3 * k + 1] = (float)dy; r_out[3 * k + 2] = (float)dz;
-      }
-      t += __popc(m);
-    }
-  }
-  if (!kFill && lane == 0) cnt[u] = t;
 }
 
 // ---- forces and stress (alignn_atomwise.py:547-563, 610-635) -----------------------------------------
@@ -258,44 +220,6 @@ int alignn_b200_line_graph_fill(const int32_t* src, const int32_t* dst, const in
   if (!src || !dst || !in_ptr || !in_eid || !offsets || !lsrc || !ldst) return ALIGNN_ERR_BAD_ARG;
   lg_fill_kernel<<<blocks_for(num_edges * 32), kBlock, 0, (cudaStream_t)stream>>>(src, dst, in_ptr, in_eid, num_edges, offsets,
                                                                                 lsrc, ldst);
-  return alignn::check_launch();
-}
-
-size_t alignn_b200_radius_graph_workspace_bytes(int64_t num_atoms) {
-  if (num_atoms < 0 || num_atoms >= ((int64_t)1 << 31) - 1) return 0;
-  size_t scan_b = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, scan_b, (const int32_t*)nullptr, (int32_t*)nullptr, (int)(num_atoms + 1));
-  return alignn::device::align256((size_t)(num_atoms + 1) * 4) + alignn::device::align256(scan_b);
-}
-
-int alignn_b200_radius_graph_offsets(const double* cart_coords, const double* shifts, int64_t num_atoms, int64_t num_images,
-                                     double cutoff, double atol, int32_t* offsets, void* workspace, size_t workspace_bytes,
-                                     alignn_stream_t stream) {
-  using namespace alignn::device;
-  if (num_atoms < 0 || num_images < 0 || !offsets || !workspace || (num_atoms > 0 && !cart_coords) || (num_images > 0 && !shifts))
-    return ALIGNN_ERR_BAD_ARG;
-  if (workspace_bytes < alignn_b200_radius_graph_workspace_bytes(num_atoms)) return ALIGNN_ERR_WORKSPACE;
-  cudaStream_t st = (cudaStream_t)stream;
-  int32_t* cnt = reinterpret_cast<int32_t*>(workspace);
-  void* cubws = reinterpret_cast<uint8_t*>(workspace) + align256((size_t)(num_atoms + 1) * 4);
-  size_t b = workspace_bytes - align256((size_t)(num_atoms + 1) * 4);
-  cudaMemsetAsync(cnt, 0, (size_t)(num_atoms + 1) * 4, st);
-  if (num_atoms > 0)
-    radius_scan_kernel<false><<<blocks_for(num_atoms * 32), kBlock, 0, st>>>(cart_coords, shifts, num_atoms, num_images, cutoff,
-                                                                          atol, nullptr, cnt, nullptr, nullptr, nullptr, nullptr);
-  cub::DeviceScan::ExclusiveSum(cubws, b, cnt, offsets, (int)(num_atoms + 1), st);     // offsets[N] = number of bonds
-  return alignn::check_launch();
-}
-
-int alignn_b200_radius_graph_fill(const double* cart_coords, const double* shifts, int64_t num_atoms, int64_t num_images,
-                                  double cutoff, double atol, const int32_t* offsets, int32_t* u, int32_t* v,
-                                  int32_t* image_index, float* r, alignn_stream_t stream) {
-  using namespace alignn::device;
-  if (num_atoms < 0 || num_images < 0) return ALIGNN_ERR_BAD_ARG;
-  if (num_atoms == 0) return ALIGNN_OK;
-  if (!cart_coords || (num_images > 0 && !shifts) || !offsets || !u || !v || !image_index || !r) return ALIGNN_ERR_BAD_ARG;
-  radius_scan_kernel<true><<<blocks_for(num_atoms * 32), kBlock, 0, (cudaStream_t)stream>>>(
-      cart_coords, shifts, num_atoms, num_images, cutoff, atol, offsets, nullptr, u, v, image_index, r);
   return alignn::check_launch();
 }
 

@@ -416,7 +416,8 @@ int alignn_b200_radius_graph_build_host(const double* cart_coords, const double*
                                         int64_t* v, int64_t* image_index, float* r);
 
 /* ------------------------------------------------------------------------------------------
- * Device-side structure builders and ALIGNN-FF reductions (csrc/graph_device.cu).  All pointers are DEVICE pointers;
+ * Device-side structure builders and ALIGNN-FF reductions (csrc/graph_device.cu; the radius scan is in
+ * csrc/crystal_graph_device.cu).  All pointers are DEVICE pointers;
  * the caller owns every buffer including the workspace; calls only enqueue on `stream`.  Integer results are
  * bit-identical to the host builders above; the two d=3 sums are deterministic (fixed order, no float atomics).
  * Replace, on the GPU: `dgl.graph((u, v))` + CSR/CSC views (alignn/graphs.py:544), `g.line_graph(shared=True)`
@@ -453,6 +454,65 @@ int alignn_b200_radius_graph_offsets(const double* cart_coords, const double* sh
 int alignn_b200_radius_graph_fill(const double* cart_coords, const double* shifts, int64_t num_atoms, int64_t num_images,
                                   double cutoff, double atol, const int32_t* offsets, int32_t* u, int32_t* v,
                                   int32_t* image_index, float* r, alignn_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Crystal graphs for a batch of B structures on the device (csrc/crystal_graph_device.cu): the neighbour lists of
+ * `Graph.atom_dgl_multigraph` (alignn/graphs.py:472-589) for both of its strategies.  Device pointers except
+ * `lattices`, caller-owned buffers, enqueue-only on `stream`.  The caller builds, per crystal b, the image table
+ * `cells` (integer cell offsets as doubles, meshgrid "ij" order) and `shifts = cells @ lattice_b`, concatenated over
+ * the batch with shift_offsets[B+1]; atoms are concatenated with atom_offsets[B+1] and crystal_of_atom[N].
+ * Rejected (ALIGNN_ERR_BAD_ARG, nothing enqueued): B < 1, N < 1, a NULL input, a lattice with zero or non-finite
+ * determinant, max_neighbors < 1.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct {
+  const double* cart_coords;      /* [N,3] Cartesian coordinates                                             */
+  const double* shifts;           /* [I,3] per-crystal image shifts, concatenated                            */
+  const double* cells;            /* [I,3] the matching cell offsets                                         */
+  const double* lattices;         /* [B,3,3] lattice row vectors, HOST memory (checked, copied by the emit)  */
+  const int64_t* atom_offsets;    /* [B+1]                                                                   */
+  const int64_t* shift_offsets;   /* [B+1]                                                                   */
+  const int32_t* crystal_of_atom; /* [N]                                                                     */
+  const double* cutoffs;          /* [B] per-crystal cutoff                                                  */
+  int64_t num_crystals;           /* B */
+  int64_t num_atoms;              /* N */
+  int64_t num_images;             /* I = shift_offsets[B] */
+  int64_t max_images;             /* largest per-crystal image count */
+  double atol;                    /* pairs with |d| <= atol are the atom itself */
+} alignn_b200_crystal_batch;
+
+/* Candidate scan (the radius scan above, batched): for every atom u of crystal b, every (image c, atom v of b) with
+ * atol < |(shifts[c] + x_v) - x_u| <= cutoffs[b] in double precision.  offsets[N+1] = exclusive scan of the per-atom
+ * counts (offsets[N] = total).  status[b] = the crystal's smallest per-atom count (strategy 1, k-NN: the crystal needs
+ * a grown cutoff if it is below k, graphs.py:166-186) or 1 if the crystal's last atom has a bond (strategy 0, radius:
+ * graphs.py:347-350).  Read status and offsets[N] back to decide the next round. */
+size_t alignn_b200_crystal_scan_workspace_bytes(int64_t num_atoms);
+int alignn_b200_crystal_scan_count(const alignn_b200_crystal_batch* batch, int strategy, int32_t* offsets, int32_t* status,
+                                   void* workspace, size_t workspace_bytes, alignn_stream_t stream);
+/* Radius strategy: the bonds in (u, c, v) order per atom, exactly `radius_graph` of each crystal concatenated with
+ * atom ids offset: u, v [E] global ids, r [E,3] = fp32 displacement, images [E,3] = fp32 cell offsets. */
+int alignn_b200_crystal_radius_fill(const alignn_b200_crystal_batch* batch, const int32_t* offsets, int32_t* u, int32_t* v,
+                                    float* r, float* images, alignn_stream_t stream);
+
+/* k-nearest strategy (`nearest_neighbor_edges` + `build_undirected_edgedata`, graphs.py:155-264, use_canonize=True),
+ * three calls on one workspace sized for the candidate count C = offsets[N] of the final scan round.  The image tables
+ * must be symmetric (cells[I-1-c] == -cells[c]).
+ * select: per atom, candidates ordered by (dist, v, image); everything with dist <= the k-th distance is kept (exact
+ *   double compare, graphs.py:202-214).  kept_offsets[N+1] = exclusive scan of the kept counts; read kept_offsets[N].
+ * order:  each kept (u, v, c) -> (u, v, c) if v >= u else (v, u, -c); pairs in order of first encounter (atoms
+ *   ascending, then (dist, v, image)), images ascending inside a pair, duplicates dropped (graphs.py:127-152,
+ *   218-223, 240-244).  bond_offsets[B+1] int64 = first bond of each crystal; read it back to size the outputs.
+ * emit:   every (a, b, image) -> rows (a, b, d) and (b, a, -d), d = fp32(((frac_b + image) - frac_a) @ lattice)
+ *   in double (graphs.py:245-257); images [E,3] fp32 on both rows.  frac_coords [N,3] device. */
+size_t alignn_b200_knn_graph_workspace_bytes(int64_t num_atoms, int64_t num_crystals, int64_t num_candidates);
+int alignn_b200_knn_graph_select(const alignn_b200_crystal_batch* batch, const int32_t* offsets, int64_t num_candidates,
+                                 int max_neighbors, int32_t* kept_offsets, void* workspace, size_t workspace_bytes,
+                                 alignn_stream_t stream);
+int alignn_b200_knn_graph_order(const alignn_b200_crystal_batch* batch, const int32_t* offsets, const int32_t* kept_offsets,
+                                int64_t num_candidates, int64_t num_kept, int64_t* bond_offsets, void* workspace,
+                                size_t workspace_bytes, alignn_stream_t stream);
+int alignn_b200_knn_graph_emit(const alignn_b200_crystal_batch* batch, const double* frac_coords, int64_t num_candidates,
+                               int64_t num_kept, int32_t* u, int32_t* v, float* r, float* images, void* workspace,
+                               size_t workspace_bytes, alignn_stream_t stream);
 
 /* forces[v] = sum over in-edges of pair_forces - (add_reverse ? sum over out-edges : 0)   (alignn_atomwise.py:547-563:
  * update_all(copy_e, sum) on g and on dgl.reverse(g)); pair_forces [E,3], forces [Nn,3].  in_eid NULL = identity. */
