@@ -113,6 +113,12 @@ class CrystalBatch(C.Structure):
                 ("atol", C.c_double)]
 
 
+class FireParams(C.Structure):
+    _fields_ = [("maxstep", C.c_double), ("dtmax", C.c_double), ("finc", C.c_double), ("fdec", C.c_double),
+                ("astart", C.c_double), ("fa", C.c_double), ("fmax", C.c_double), ("n_min", C.c_int32),
+                ("max_steps", C.c_int32), ("force_multiplier", C.c_float)]
+
+
 # name -> (restype, argtypes); mirrors include/alignn_b200.h one to one
 _SIGNATURES = {
     "alignn_b200_version": (C.c_int, []),
@@ -179,6 +185,8 @@ _SIGNATURES = {
                                                _fp]),
     "alignn_b200_remove_net_torque_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "alignn_b200_remove_net_torque": (C.c_int, [_fp, _fp, _fp, C.c_int64, C.c_int64, C.c_int, _fp, _fp, C.c_size_t, _fp]),
+    "alignn_b200_fire_step": (C.c_int, [C.POINTER(FireParams), _fp, C.c_int64, _fp, _fp, C.c_int64, _fp, C.c_int64, _fp, _fp,
+                                        _fp, _fp, _fp, _fp]),
     "alignn_b200_debug_egc_flags": (None, [C.c_int]),
     "alignn_b200_segment_mean": (C.c_int, [_fp, _fp, C.c_int64, C.c_int, _fp, _fp]),
     "alignn_b200_segment_mean_backward": (C.c_int, [_fp, _fp, C.c_int64, C.c_int, _fp, _fp]),

@@ -102,6 +102,14 @@ def cutoff_function_based_edges(r: torch.Tensor, inner_cutoff: float = 4, expone
     return torch.where(r <= inner_cutoff, env, torch.zeros_like(r))
 
 
+def bond_penalty(bondlength: torch.Tensor, config) -> torch.Tensor:
+    """Per-bond penalty penalty_factor * (penalty_threshold - bondlength) for bonds shorter than penalty_threshold, zero
+    otherwise (alignn_atomwise.py:498-510; the model adds its sum to every crystal's energy)."""
+    c = config
+    return torch.where(bondlength < c.penalty_threshold, c.penalty_factor * (c.penalty_threshold - bondlength),
+                       torch.zeros_like(bondlength))
+
+
 EV_PER_A3_IN_GPA = 160.21766208          # 1 eV/A^3 in GPa (alignn_atomwise.py:569)
 
 
@@ -237,8 +245,7 @@ class ALIGNNAtomWise(nn.Module):
         natoms = g.batch_num_nodes_on_device().to(out.dtype)
         en_out = out * natoms if c.energy_mult_natoms else out          # (:495-497)
         if c.use_penalty:                                               # (:498-510) zero for bonds >= threshold
-            pen = torch.where(bondlength < c.penalty_threshold, c.penalty_factor * (c.penalty_threshold - bondlength),
-                              torch.zeros_like(bondlength))
+            pen = bond_penalty(bondlength, c)
             en_out = en_out + pen.sum()
             if not c.energy_mult_natoms:
                 # the reference does `en_out = out; en_out += total_penalty` in place, so the (whole-batch) penalty also

@@ -382,6 +382,52 @@ def remove_net_torque(pos: torch.Tensor, forces: torch.Tensor, node_offsets64: t
     return out
 
 
+FIRE_DEFAULTS = dict(maxstep=0.2, dtmax=1.0, n_min=5, finc=1.1, fdec=0.5, astart=0.1, fa=0.99)   # ase FIRE defaults
+FIRE_DT0, FIRE_A0 = 0.1, 0.1                                                                    # its initial dt and a
+FIRE_BAD_INPUT = 3            # istate status of a crystal whose batch slice does not match its atom count
+FIRE_MAX_STEPS = 2 ** 31 - 1  # steps travels as an int32
+
+
+@_on_tensor_device
+def fire_step(grad: torch.Tensor, active: torch.Tensor, batch_offsets: torch.Tensor, atom_offsets: torch.Tensor,
+              positions: torch.Tensor, velocities: torch.Tensor, forces: torch.Tensor, fstate: torch.Tensor,
+              istate: torch.Tensor, *, fmax: float, steps: int, force_multiplier: float = 1.0, **fire) -> None:
+    """One FIRE step (ASE 3.22.1 `FIRE.step` with `Optimizer.converged` and the step limit of `Dynamics.irun`) for the
+    running crystals listed in `active`, in place, one launch (csrc/fire_device.cu, alignn_b200_fire_step).
+
+    grad [M,3] fp32: the model's forces for the crystals of `active` in that order (batch_offsets [A+1] int32; slice j
+    must hold exactly the atoms of crystal active[j]); atom_offsets [B+1] int64 with atom_offsets[B] == N; positions /
+    velocities [N,3] float64; forces [N,3] fp32 (written: the scaled forces of this evaluation); fstate [B,2] float64 =
+    {dt, a}; istate [B,4] int32 = {Nsteps, first step pending, steps taken, status (0 running, 1 converged, 2 step limit,
+    FIRE_BAD_INPUT: slice j is not crystal active[j]'s atoms or lies outside grad -- nothing else is read or written for
+    that crystal)}.  Enqueue only: the statuses are the caller's to read back.  `fire` overrides FIRE_DEFAULTS."""
+    lib = _lib.load()
+    par = dict(FIRE_DEFAULTS, **fire)
+    want = ((grad, torch.float32), (active, torch.int32), (batch_offsets, torch.int32), (atom_offsets, torch.int64),
+            (positions, torch.float64), (velocities, torch.float64), (forces, torch.float32), (fstate, torch.float64),
+            (istate, torch.int32))
+    for t, dt in want:
+        if not t.is_cuda or t.device != grad.device:
+            raise RuntimeError(f"fire_step needs all operands on one CUDA device; got {t.device} and {grad.device}")
+        if t.dtype != dt or not t.is_contiguous():
+            raise RuntimeError(f"fire_step: expected a contiguous {dt} tensor, got {t.dtype}")
+    B, A = atom_offsets.numel() - 1, active.numel()
+    N = positions.numel() // 3
+    if (velocities.numel() != 3 * N or forces.numel() != 3 * N or fstate.numel() != 2 * B or istate.numel() != 4 * B
+            or batch_offsets.numel() != A + 1 or grad.dim() != 2 or grad.shape[1] != 3):
+        raise ValueError("fire_step: inconsistent operand shapes")
+    if isinstance(steps, bool) or int(steps) != steps or not 1 <= int(steps) <= FIRE_MAX_STEPS:
+        raise ValueError(f"fire_step: steps must be an integer in [1, {FIRE_MAX_STEPS}], got {steps!r}")
+    if not 0 <= int(par["n_min"]) <= FIRE_MAX_STEPS:
+        raise ValueError(f"fire_step: n_min must be in [0, {FIRE_MAX_STEPS}], got {par['n_min']!r}")
+    p = _lib.FireParams(float(par["maxstep"]), float(par["dtmax"]), float(par["finc"]), float(par["fdec"]),
+                        float(par["astart"]), float(par["fa"]), float(fmax), int(par["n_min"]), int(steps),
+                        float(force_multiplier))
+    _lib.check(lib.alignn_b200_fire_step(C.byref(p), active.data_ptr(), A, atom_offsets.data_ptr(), batch_offsets.data_ptr(),
+                                         B, grad.data_ptr(), grad.shape[0], positions.data_ptr(), velocities.data_ptr(), forces.data_ptr(),
+                                         fstate.data_ptr(), istate.data_ptr(), stream_ptr()), "alignn_b200_fire_step")
+
+
 class _SegmentMean(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, gptr):

@@ -563,6 +563,45 @@ int alignn_b200_remove_net_torque(const float* pos, const float* forces, const i
                                   int64_t num_nodes, int cross_dim0, float* out, void* workspace, size_t workspace_bytes,
                                   alignn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Structure relaxation (csrc/fire_device.cu): one step of ASE 3.22.1's FIRE (`FIRE.step`, ase/optimize/fire.py) with
+ * the convergence test and step limit of `Optimizer.converged` / `Dynamics.irun` (ase/optimize/optimize.py), for a
+ * batch of crystals relaxed together -- what `ForceField.optimize_atoms(optimizer="FIRE", optimize_lattice=False)`
+ * (alignn/ff/ff.py:373-417) runs one crystal at a time on the forces of `AlignnAtomwiseCalculator.calculate`
+ * (alignn/ff/calculators.py:280-372).  Device pointers, caller-owned buffers, enqueue-only on `stream`.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct {
+  double maxstep;           /* cap on |dr| over the whole crystal (0.2)                    */
+  double dtmax;             /* 1.0 */
+  double finc, fdec;        /* 1.1, 0.5 */
+  double astart, fa;        /* 0.1, 0.99 */
+  double fmax;              /* converged when max_i |F_i|^2 < fmax^2 (strict)              */
+  int32_t n_min;            /* Nmin = 5: dt grows only once Nsteps > n_min                 */
+  int32_t max_steps;        /* steps >= 1: a crystal takes at most this many FIRE steps    */
+  float force_multiplier;   /* F = fp32(grad * force_multiplier), the calculator's scaling */
+} alignn_b200_fire_params;
+
+/* One launch per relaxation step: one CTA per entry of active[num_active] (crystal ids, each listed once), for a model
+ * batch holding those crystals' atoms in that order.  Per crystal c with status 0 (running):
+ *   F = fp32(grad[batch_offsets[j] + i] * force_multiplier) for its atoms i, written to forces[atom_offsets[c] + i]
+ *   (so forces hold the last evaluation); if max_i |F_i|^2 < fmax^2 the status becomes 1 (converged), else if c has
+ *   taken max_steps steps it becomes 2 (step limit), else one FIRE step updates velocities, positions and the state.
+ *   The j-th batch slice must be crystal c's atoms: batch_offsets[j+1] - batch_offsets[j] == atom_offsets[c+1] -
+ *   atom_offsets[c], inside [0, grad_rows).  Otherwise nothing is read or written for c except its status, which
+ *   becomes 3 (inconsistent input); read the status back to detect it.
+ *   Sums are in double with a fixed-order block reduction; the per-element updates follow numpy's order exactly.
+ * Crystals with a nonzero status, and ids outside [0, num_crystals), are not touched.
+ *   grad [grad_rows, 3] fp32 (the model batch, atoms compacted); batch_offsets [num_active+1] int32;
+ *   atom_offsets [num_crystals+1] int64; positions / velocities [N,3] double; forces [N,3] fp32;
+ *   fstate [num_crystals,2] double = {dt, a}; istate [num_crystals,4] int32 = {Nsteps, first step pending (v is None),
+ *   steps taken, status}.  Initial state: velocities 0, {dt, a} = {0.1, 0.1}, istate {0, 1, 0, 0}.
+ * Rejected (ALIGNN_ERR_BAD_ARG, nothing enqueued): NULL params or a NULL array, num_active outside [0, num_crystals],
+ * grad_rows < 0, maxstep or dtmax not > 0, fmax negative or not finite, a non-finite factor, n_min < 0, max_steps < 1. */
+int alignn_b200_fire_step(const alignn_b200_fire_params* params, const int32_t* active, int64_t num_active,
+                          const int64_t* atom_offsets, const int32_t* batch_offsets, int64_t num_crystals,
+                          const float* grad, int64_t grad_rows, double* positions, double* velocities, float* forces,
+                          double* fstate, int32_t* istate, alignn_stream_t stream);
+
 /* Per-graph mean over node rows (dgl.nn.AvgPooling, alignn.py:325) and its backward. */
 int alignn_b200_segment_mean(const float* x, const int32_t* graph_ptr /*[B+1]*/, int64_t B, int d, float* out,
                              alignn_stream_t stream);
