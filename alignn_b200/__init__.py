@@ -8,4 +8,4 @@ __version__ = "0.1.0"
 
 from .graph import Graph, batch, unbatch, reverse, graph, as_graph, bond_cosines  # noqa: F401
 from .ealignn_atomwise import eALIGNNAtomWise, eALIGNNAtomWiseConfig  # noqa: F401,E402
-from .relax import relax_structures, RelaxResult  # noqa: F401,E402
+from .relax import relax_structures, RelaxResult, CellRelaxResult  # noqa: F401,E402

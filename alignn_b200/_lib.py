@@ -119,6 +119,10 @@ class FireParams(C.Structure):
                 ("max_steps", C.c_int32), ("force_multiplier", C.c_float)]
 
 
+class FireCellParams(C.Structure):
+    _fields_ = [("fire", FireParams), ("stress_wt", C.c_float)]
+
+
 # name -> (restype, argtypes); mirrors include/alignn_b200.h one to one
 _SIGNATURES = {
     "alignn_b200_version": (C.c_int, []),
@@ -187,6 +191,8 @@ _SIGNATURES = {
     "alignn_b200_remove_net_torque": (C.c_int, [_fp, _fp, _fp, C.c_int64, C.c_int64, C.c_int, _fp, _fp, C.c_size_t, _fp]),
     "alignn_b200_fire_step": (C.c_int, [C.POINTER(FireParams), _fp, C.c_int64, _fp, _fp, C.c_int64, _fp, C.c_int64, _fp, _fp,
                                         _fp, _fp, _fp, _fp]),
+    "alignn_b200_fire_cell_step": (C.c_int, [C.POINTER(FireCellParams), _fp, C.c_int64, _fp, _fp, C.c_int64, _fp, C.c_int64,
+                                             _fp, C.c_int64, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
     "alignn_b200_debug_egc_flags": (None, [C.c_int]),
     "alignn_b200_segment_mean": (C.c_int, [_fp, _fp, C.c_int64, C.c_int, _fp, _fp]),
     "alignn_b200_segment_mean_backward": (C.c_int, [_fp, _fp, C.c_int64, C.c_int, _fp, _fp]),

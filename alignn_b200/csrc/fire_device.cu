@@ -17,6 +17,7 @@
 
 #include "api_common.h"
 #include "alignn_b200.h"
+#include "fire_common.cuh"
 
 namespace alignn {
 namespace fire {
@@ -25,18 +26,6 @@ constexpr int kBlock = 256;
 enum { kRunning = 0, kConverged = 1, kExhausted = 2, kBadInput = 3 };   // istate[c][3]
 enum { kNsteps = 0, kFirst = 1, kTaken = 2, kStatus = 3 };      // istate columns
 enum { kFrozen = 0, kFirstStep = 1, kMix = 2, kReset = 3 };     // what the velocity pass does
-
-// NaN-propagating max (numpy's max): once a NaN is seen it stays
-__device__ __forceinline__ double nan_max(double m, double x) { return (x > m || x != x) ? x : m; }
-
-// x / y rounded to nearest without the division's out-of-line slow path (which needs a stack frame): Markstein's
-// correction of x * RN(1/y) with one fma is the correctly rounded quotient whenever no step overflows or underflows --
-// forces, velocities and displacements are far inside that range.
-__device__ __forceinline__ double div_rn(double x, double y) {
-  const double r = __drcp_rn(y);
-  const double q = __dmul_rn(x, r);
-  return __fma_rn(__fma_rn(-y, q, x), r, q);
-}
 
 __global__ void __launch_bounds__(kBlock)
 fire_step_kernel(const alignn_b200_fire_params p, const int32_t* __restrict__ active, const int64_t* __restrict__ atom_off,

@@ -89,6 +89,25 @@ def _checked_structures(structures, neighbor_strategy: str, max_neighbors: int):
     return lats, Xs
 
 
+def knn_cut_is_tied(lattice_mat, cart_coords, max_neighbors: int = 12, rtol: float = 1e-6, reach: int = 3) -> bool:
+    """True when some atom's max_neighbors-th and next nearest neighbour distances (over the periodic images within
+    `reach` cells) are equal to `rtol` relative.  The images x + R and x - R of an atom are always equally far, so such
+    ties are common.  The k-nearest graph keeps every candidate at the k-th distance, compared exactly, so at a tie
+    rounding-level changes of the cell or positions decide which images the graph keeps."""
+    lat = np.asarray(lattice_mat, dtype=np.float64)
+    X = np.asarray(cart_coords, dtype=np.float64)
+    k = int(max_neighbors)
+    r = np.arange(-reach, reach + 1)
+    shifts = np.stack(np.meshgrid(r, r, r, indexing="ij"), -1).reshape(-1, 3).astype(np.float64) @ lat
+    cand = (X[None, :, :] + shifts[:, None, :]).reshape(-1, 3)
+    for x in X:
+        d = np.linalg.norm(cand - x, axis=1)
+        d = np.sort(d[d > 1e-8])
+        if d.size > k and d[k] - d[k - 1] <= rtol * d[k - 1]:
+            return True
+    return False
+
+
 def _neighbors_device(structures, neighbor_strategy: str, cutoff: float, max_neighbors: int, cutoff_extra: float,
                       device):
     """The batched device builder behind `knn_graph_device` and `crystal_graphs_device` (csrc/crystal_graph_device.cu).

@@ -428,6 +428,58 @@ def fire_step(grad: torch.Tensor, active: torch.Tensor, batch_offsets: torch.Ten
                                          fstate.data_ptr(), istate.data_ptr(), stream_ptr()), "alignn_b200_fire_step")
 
 
+FIRE_CELL_DEGENERATE = 4      # istate status of a crystal whose cell lost its volume or whose expm(L) is not finite
+
+
+@_on_tensor_device
+def fire_cell_step(grad: torch.Tensor, stress: torch.Tensor, active: torch.Tensor, batch_offsets: torch.Tensor,
+                   atom_offsets: torch.Tensor, positions: torch.Tensor, velocities: torch.Tensor, forces: torch.Tensor,
+                   cells0: torch.Tensor, logdef: torch.Tensor, defgrad: torch.Tensor, cells: torch.Tensor,
+                   cell_velocities: torch.Tensor, cell_forces: torch.Tensor, stress_out: torch.Tensor, fstate: torch.Tensor,
+                   istate: torch.Tensor, *, fmax: float, steps: int, force_multiplier: float = 1.0, stress_wt: float = 1.0,
+                   **fire) -> None:
+    """One FIRE step on ASE 3.22.1's `ExpCellFilter` (atoms and cell together) for the running crystals listed in
+    `active`, in place, one launch (csrc/fire_cell_device.cu, alignn_b200_fire_cell_step).
+
+    As `fire_step`, plus: stress [A,3,3] fp32, the model's stress of crystal active[j] in row j; stress_out [B,6] fp32
+    (written: the calculator's Voigt stress, eV/A^3); cell_forces [B,3,3] float64 (written: the filter's cell rows);
+    the filter state, [B,3,3] float64 each: cells0 (the starting cells), logdef (L, initially 0), defgrad (F = expm(L),
+    initially I), cells (C = C0 F^T, initially cells0), cell_velocities (initially 0).  Status FIRE_CELL_DEGENERATE:
+    the cell's volume is not finite and > 0, or expm(L) is not finite; the crystal is frozen."""
+    lib = _lib.load()
+    par = dict(FIRE_DEFAULTS, **fire)
+    want = ((grad, torch.float32), (stress, torch.float32), (active, torch.int32), (batch_offsets, torch.int32),
+            (atom_offsets, torch.int64), (positions, torch.float64), (velocities, torch.float64), (forces, torch.float32),
+            (cells0, torch.float64), (logdef, torch.float64), (defgrad, torch.float64), (cells, torch.float64),
+            (cell_velocities, torch.float64), (cell_forces, torch.float64), (stress_out, torch.float32),
+            (fstate, torch.float64), (istate, torch.int32))
+    for t, dt in want:
+        if not t.is_cuda or t.device != grad.device:
+            raise RuntimeError(f"fire_cell_step needs all operands on one CUDA device; got {t.device} and {grad.device}")
+        if t.dtype != dt or not t.is_contiguous():
+            raise RuntimeError(f"fire_cell_step: expected a contiguous {dt} tensor, got {t.dtype}")
+    B, A = atom_offsets.numel() - 1, active.numel()
+    N = positions.numel() // 3
+    if (velocities.numel() != 3 * N or forces.numel() != 3 * N or fstate.numel() != 2 * B or istate.numel() != 4 * B
+            or batch_offsets.numel() != A + 1 or grad.dim() != 2 or grad.shape[1] != 3
+            or stress.numel() != 9 * A or stress_out.numel() != 6 * B
+            or any(t.numel() != 9 * B for t in (cells0, logdef, defgrad, cells, cell_velocities, cell_forces))):
+        raise ValueError("fire_cell_step: inconsistent operand shapes")
+    if isinstance(steps, bool) or int(steps) != steps or not 1 <= int(steps) <= FIRE_MAX_STEPS:
+        raise ValueError(f"fire_cell_step: steps must be an integer in [1, {FIRE_MAX_STEPS}], got {steps!r}")
+    if not 0 <= int(par["n_min"]) <= FIRE_MAX_STEPS:
+        raise ValueError(f"fire_cell_step: n_min must be in [0, {FIRE_MAX_STEPS}], got {par['n_min']!r}")
+    p = _lib.FireCellParams(_lib.FireParams(float(par["maxstep"]), float(par["dtmax"]), float(par["finc"]),
+                                            float(par["fdec"]), float(par["astart"]), float(par["fa"]), float(fmax),
+                                            int(par["n_min"]), int(steps), float(force_multiplier)), float(stress_wt))
+    _lib.check(lib.alignn_b200_fire_cell_step(C.byref(p), active.data_ptr(), A, atom_offsets.data_ptr(), batch_offsets.data_ptr(),
+                                              B, grad.data_ptr(), grad.shape[0], stress.data_ptr(), A, positions.data_ptr(),
+                                              velocities.data_ptr(), forces.data_ptr(), cells0.data_ptr(), logdef.data_ptr(),
+                                              defgrad.data_ptr(), cells.data_ptr(), cell_velocities.data_ptr(),
+                                              cell_forces.data_ptr(), stress_out.data_ptr(), fstate.data_ptr(),
+                                              istate.data_ptr(), stream_ptr()), "alignn_b200_fire_cell_step")
+
+
 class _SegmentMean(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, gptr):

@@ -602,6 +602,37 @@ int alignn_b200_fire_step(const alignn_b200_fire_params* params, const int32_t* 
                           const float* grad, int64_t grad_rows, double* positions, double* velocities, float* forces,
                           double* fstate, int32_t* istate, alignn_stream_t stream);
 
+/* Structure relaxation with the cell (csrc/fire_cell_device.cu): one FIRE step on ASE 3.22.1's `ExpCellFilter`
+ * (ase/constraints.py; no mask, no hydrostatic strain, no constant volume, scalar_pressure 0, cell_factor 1) -- what
+ * `ForceField.optimize_atoms(optimizer="FIRE", optimize_lattice=True)`, the reference's default, runs one crystal at a
+ * time with the forces and Voigt stress of `AlignnAtomwiseCalculator.calculate`. */
+typedef struct {
+  alignn_b200_fire_params fire;
+  float stress_wt;          /* the calculator's stress scaling: s = fp32(voigt(stress) * stress_wt / 160.21766208) */
+} alignn_b200_fire_cell_params;
+
+/* As alignn_b200_fire_step, on the filter's n + 3 rows: the atom rows f_i F and the cell rows (the symmetrised
+ * -expm(Y)[0:3,3:6], Y = [[L, -W expm(-L)], [0, L]], W = -V full(s) F^-T, or W itself when the two are neither
+ * np.isclose nor aligned with a cosine above 0.8).  Per running crystal c (j its index in active):
+ *   stress [stress_rows = num_active, 3, 3] fp32: the model's stress of crystal active[j] in row j;
+ *   stress_out [num_crystals, 6] fp32: the calculator's Voigt stress (xx yy zz yz xz xy, eV/A^3) of this evaluation;
+ *   cell_forces [num_crystals, 3, 3] double: the filter's cell rows of this evaluation;
+ *   filter state, [num_crystals, 3, 3] double each: cells0 (C0, the cell the relaxation started from), logdef (L),
+ *   defgrad (F = expm(L)), cells (C = C0 F^T; rows are lattice vectors), cell_velocities (the cell rows' FIRE
+ *   velocities).  Initial state: L = 0, F = I, C = C0, cell velocities 0.
+ *   A step moves L += dr_cell, F = expm(L), C = C0 F^T and x_i = F_new (F^-1 x_i + dr_i); |dr| and the maxstep cap
+ *   run over all n + 3 rows, and convergence is max over the n + 3 rows of |row|^2 < fmax^2.
+ *   Status 4 (cell degenerate): |det C| is not finite and > 0 (nothing else is written), or expm(L) of the step is not
+ *   finite (velocities and FIRE state are written, positions and the cell state are not); the crystal is frozen.
+ * Rejected (ALIGNN_ERR_BAD_ARG, nothing enqueued): as alignn_b200_fire_step, and stress_rows != num_active or a
+ * non-finite stress_wt. */
+int alignn_b200_fire_cell_step(const alignn_b200_fire_cell_params* params, const int32_t* active, int64_t num_active,
+                               const int64_t* atom_offsets, const int32_t* batch_offsets, int64_t num_crystals,
+                               const float* grad, int64_t grad_rows, const float* stress, int64_t stress_rows,
+                               double* positions, double* velocities, float* forces, double* cells0, double* logdef,
+                               double* defgrad, double* cells, double* cell_velocities, double* cell_forces,
+                               float* stress_out, double* fstate, int32_t* istate, alignn_stream_t stream);
+
 /* Per-graph mean over node rows (dgl.nn.AvgPooling, alignn.py:325) and its backward. */
 int alignn_b200_segment_mean(const float* x, const int32_t* graph_ptr /*[B+1]*/, int64_t B, int d, float* out,
                              alignn_stream_t stream);

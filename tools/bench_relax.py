@@ -14,7 +14,15 @@ run with CUDA events around its phases gives the per-step split (build, model, F
 from its first enqueue to its last, host work inside it included).  The two arms must end at the same positions.  The
 device name, power limit and SM clock limit are read in the same run.
 
-    python tools/bench_relax.py [--structures 64] [--steps 10] [--seed 0]
+--optimize-lattice relaxes the cells too (relax_structures(optimize_lattice=True), ASE's ExpCellFilter): every cell
+starts strained and sheared (atoms moved with it), the model computes stress (stresswise_weight=1), and the per-crystal
+arm runs the oracle's filtered FIRE (oracle/cell_filter_oracle.py) on the host graph of the current cell.  The largest
+difference between the two arms' final positions and cells is reported, with the number of crystals on which they agree
+to 1e-5 A and, for every crystal on which they part, whether its 12th-neighbour cut lies inside a distance tie
+(`neighbors.knn_cut_is_tied`, at any structure the host arm evaluated), where rounding picks the images the graph
+keeps.
+
+    python tools/bench_relax.py [--structures 64] [--steps 10] [--seed 0] [--optimize-lattice]
 """
 import argparse
 import json
@@ -46,6 +54,7 @@ def main():
     ap.add_argument("--structures", type=int, default=64)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--optimize-lattice", action="store_true", help="relax the cells too (ExpCellFilter)")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_relax.py needs a CUDA device")
@@ -53,6 +62,7 @@ def main():
     __graft_entry__.build()
     from alignn_b200 import neighbors, ops, relax_structures
     from alignn_b200.alignn_atomwise import ALIGNNAtomWise, ALIGNNAtomWiseConfig
+    from oracle import cell_filter_oracle as CF
     from oracle import fire_oracle as FO
 
     dev = torch.device("cuda:0")
@@ -64,18 +74,26 @@ def main():
                for i in pick]
     sizes = [x.shape[0] for _, x in structs]
     feats = torch.from_numpy(rng.normal(size=(sum(sizes), 92)).astype(np.float32)).to(dev)
+    cell = a.optimize_lattice
+    if cell:                                                   # strained, sheared cells, the atoms moved with them
+        srng = np.random.default_rng(a.seed + 1)
+        Ds = [np.eye(3) + np.diag(srng.uniform(-0.04, 0.04, 3)) + srng.uniform(-0.03, 0.03, (3, 3)) for _ in structs]
+        structs = [(lat @ D.T, X @ D.T) for (lat, X), D in zip(structs, Ds)]
     torch.manual_seed(1)
     cfg = ALIGNNAtomWiseConfig(name="alignn_atomwise", alignn_layers=4, gcn_layers=4, hidden_features=256,
-                               atom_input_features=92, gradwise_weight=1.0)
+                               atom_input_features=92, gradwise_weight=1.0, stresswise_weight=1.0 if cell else 0.0)
     model = ALIGNNAtomWise(cfg).to(dev).eval()
 
     def batched():
-        r = relax_structures(model, structs, feats, fmax=0.0, steps=a.steps)
+        r = relax_structures(model, structs, feats, fmax=0.0, steps=a.steps, optimize_lattice=cell)
         torch.cuda.synchronize()
         return r
 
+    visited = []                                               # per crystal: every (cell, x) the host arm evaluated
+
     def per_crystal():
         out, o = [], 0
+        visited.clear()
         for lat, X in structs:
             n = X.shape[0]
             f_b = feats[o:o + n].cpu()
@@ -85,7 +103,21 @@ def main():
                 g, lg = neighbors.crystal_graph(lat, x, f_b, cutoff=8.0, neighbor_strategy="k-nearest", max_neighbors=12)
                 res = model((g.to(dev), lg.to(dev), lat_t))
                 return float(res["out"].detach() * n), res["grad"].detach().reshape(-1, 3).cpu().numpy()
-            out.append(FO.relax(evaluate, X, fmax=0.0, steps=a.steps))
+
+            seen = []
+            visited.append(seen)
+
+            def evaluate_cell(c, x, f_b=f_b, n=n, seen=seen):
+                seen.append((c, x))
+                g, lg = neighbors.crystal_graph(c, x, f_b, cutoff=8.0, neighbor_strategy="k-nearest", max_neighbors=12)
+                g.ndata["V"] = torch.full((n,), abs(float(np.dot(np.cross(c[0], c[1]), c[2]))), dtype=torch.float32)
+                res = model((g.to(dev), lg.to(dev), torch.tensor(c, dtype=torch.float32).view(1, 3, 3).to(dev)))
+                return (float(res["out"].detach() * n), res["grad"].detach().reshape(-1, 3).cpu().numpy(),
+                        res["stresses"].detach().reshape(3, 3).cpu().numpy())
+            if cell:
+                out.append(CF.relax(evaluate_cell, lat, X, fmax=0.0, steps=a.steps))
+            else:
+                out.append(FO.relax(evaluate, X, fmax=0.0, steps=a.steps))
             o += n
         torch.cuda.synchronize()
         return out
@@ -104,7 +136,29 @@ def main():
     aoff = got.atom_offsets.cpu().tolist()
     dmax = max(float(np.abs(P[aoff[b]:aoff[b + 1]] - r["positions"]).max()) for b, r in enumerate(ref))
     assert got.nsteps.tolist() == [a.steps] * len(structs) and all(r["nsteps"] == a.steps for r in ref)
-    assert dmax <= 1e-5, f"the arms end {dmax} A apart"
+    extra = {}
+    if not cell:
+        assert dmax <= 1e-5, f"the arms end {dmax} A apart"
+    else:
+        # reported, not asserted: the arms' matrix functions (the kernel's Pade, scipy's expm / logm) differ by
+        # rounding, and where an atom's 12th and 13th neighbours are equally far (the images x + R and x - R) that
+        # rounding picks the image the k-nearest graph keeps, after which the two trajectories part
+        Cg = got.cells.cpu().numpy()
+        dcell = [float(np.abs(Cg[b] - r["cell"]).max()) for b, r in enumerate(ref)]
+        dpos = [float(np.abs(P[aoff[b]:aoff[b + 1]] - r["positions"]).max()) for b, r in enumerate(ref)]
+        moved = max(float(np.abs(r["cell"] - lat).max()) for r, (lat, _) in zip(ref, structs))
+        agree = sum(p <= 1e-5 and c <= 1e-5 for p, c in zip(dpos, dcell))
+        # per crystal: does its 12th-neighbour cut fall inside a distance tie at any structure the host arm evaluated?
+        tied = [any(neighbors.knn_cut_is_tied(c, x) for c, x in seen) for seen in visited]
+        parted = [b for b in range(len(structs)) if dpos[b] > 1e-5 or dcell[b] > 1e-5]
+        extra = {"max_cell_difference_A": max(dcell), "crystals_within_1e-5_A": f"{agree}/{len(structs)}",
+                 "crystals_with_a_knn_tie": sum(tied),
+                 "parted_crystals": [dict(id=b, positions_A=round(dpos[b], 4), cell_A=round(dcell[b], 4), knn_tie=tied[b])
+                                     for b in parted],
+                 "every_parted_crystal_has_a_knn_tie": all(tied[b] for b in parted),
+                 "max_difference_on_crystals_without_a_tie_A": max([max(dpos[b], dcell[b]) for b in range(len(structs))
+                                                                    if not tied[b]], default=0.0),
+                 "max_cell_change_A": round(moved, 4)}
     ops.TIMER = ops.KernelTimer()
     try:
         batched()
@@ -114,12 +168,13 @@ def main():
     evals = a.steps + 1
     split = {k[len("relax_"):]: round(summ[k]["total_ms"] / evals, 3) for k in summ if k.startswith("relax_")}
     med_b, med_p = statistics.median(ms["batched"]), statistics.median(ms["per_crystal"])
+    what = "ExpCellFilter FIRE on atoms and strained, sheared cells" if cell else "FIRE"
     out = dict(workload=f"{len(structs)} jittered sample structures ({sum(sizes)} atoms), ALIGNNAtomWise 4+4 d=256, "
-                        f"k-nearest 8 A / 12, fmax=0, {a.steps} FIRE steps ({evals} evaluations per crystal)",
+                        f"k-nearest 8 A / 12, fmax=0, {a.steps} {what} steps ({evals} evaluations per crystal)",
                batched_ms=[round(v, 1) for v in ms["batched"]], batched_ms_median=round(med_b, 1),
                per_crystal_ms=[round(v, 1) for v in ms["per_crystal"]], per_crystal_ms_median=round(med_p, 1),
                speedup_median=round(med_p / med_b, 2), batched_ms_per_evaluation_split=split,
-               max_position_difference_A=dmax, device=device_info())
+               max_position_difference_A=dmax, **extra, device=device_info())
     print(json.dumps(out))
 
 
