@@ -200,6 +200,10 @@ _SIGNATURES = {
                                              _fp, C.c_int64, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
     "alignn_b200_md_step": (C.c_int, [C.POINTER(MdParams), _fp, C.c_int64, _fp, C.c_int64, _fp, _fp, _fp, _fp, _fp, _fp, _fp,
                                       _fp, _fp]),
+    "alignn_b200_phonon_force_constants": (C.c_int, [_fp, C.c_double, C.c_float, _fp, C.c_int64, _fp, _fp, C.c_int64, _fp,
+                                                     _fp, C.c_int64, _fp, _fp, _fp, _fp]),
+    "alignn_b200_phonon_dynamical_matrix": (C.c_int, [_fp, C.c_int64, _fp, _fp, C.c_int64, C.c_int64, _fp, _fp, C.c_int64,
+                                                      _fp, _fp, _fp]),
     "alignn_b200_debug_egc_flags": (None, [C.c_int]),
     "alignn_b200_segment_mean": (C.c_int, [_fp, _fp, C.c_int64, C.c_int, _fp, _fp]),
     "alignn_b200_segment_mean_backward": (C.c_int, [_fp, _fp, C.c_int64, C.c_int, _fp, _fp]),

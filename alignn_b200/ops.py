@@ -533,6 +533,84 @@ def md_step(grad: torch.Tensor, atom_offsets: torch.Tensor, masses: torch.Tensor
                                        stream_ptr()), "alignn_b200_md_step")
 
 
+PHONON_BAD_INPUT = 3              # status of a crystal whose slices do not lie inside the buffers
+PHONON_NON_FINITE = 5             # status of a crystal with a non-finite force product
+PHONON_MAX_CELLS = 3072           # ALIGNN_B200_PHONON_MAX_CELLS: cells of one supercell
+
+
+def _supercell_arg(supercell):
+    if supercell is None:
+        return None
+    s = tuple(int(v) for v in supercell)
+    if len(s) != 3:
+        raise ValueError(f"supercell must have 3 entries, got {supercell!r}")
+    return C.cast((C.c_int32 * 3)(*s), C.c_void_p)
+
+
+def _phonon_operands(what, want, device):
+    for t, dt_ in want:
+        if not t.is_cuda or t.device != device:
+            raise RuntimeError(f"{what} needs all operands on one CUDA device; got {t.device} and {device}")
+        if t.dtype != dt_ or not t.is_contiguous():
+            raise RuntimeError(f"{what}: expected a contiguous {dt_} tensor, got {t.dtype}")
+
+
+@_on_tensor_device
+def phonon_force_constants(grad: torch.Tensor, atom_offsets: torch.Tensor, row_offsets: torch.Tensor,
+                           fc_offsets: torch.Tensor, masses: torch.Tensor, force_constants: torch.Tensor,
+                           dynamical_matrix: torch.Tensor, status: torch.Tensor, *, supercell, delta: float,
+                           force_multiplier: float = 1.0) -> None:
+    """ASE 3.22.1's `Phonons.read(acoustic=True)` for every crystal of a batch, one launch (csrc/phonon_device.cu,
+    alignn_b200_phonon_force_constants): Frederiksen-corrected central differences, three rounds of symmetrize and
+    acoustic, mass weighting.
+
+    grad [rows,3] fp32: the model's forces of every displaced supercell (crystal c's 6n supercells of Nc n rows from
+    row_offsets[c], displacement order atom, direction, sign -1 then +1); atom_offsets / row_offsets / fc_offsets [B+1]
+    int64; masses [sum n] float64 (amu); force_constants / dynamical_matrix [fc_offsets[B]] float64 (written: crystal
+    c's [Nc, 3n, 3n] C_N and D_N at fc_offsets[c]); status [B] int32 (0 ok, PHONON_BAD_INPUT: a slice is not inside its
+    buffer, PHONON_NON_FINITE: a force product is not finite -- nothing else is read or written for it).  supercell is
+    (N0, N1, N2); delta in A.  Enqueue only: the statuses are the caller's to read back."""
+    lib = _lib.load()
+    _phonon_operands("phonon_force_constants", [(grad, torch.float32), (atom_offsets, torch.int64),
+                                                (row_offsets, torch.int64), (fc_offsets, torch.int64),
+                                                (masses, torch.float64), (force_constants, torch.float64),
+                                                (dynamical_matrix, torch.float64), (status, torch.int32)], grad.device)
+    B = atom_offsets.numel() - 1
+    if (B < 1 or row_offsets.numel() != B + 1 or fc_offsets.numel() != B + 1 or status.numel() != B
+            or grad.dim() != 2 or grad.shape[1] != 3 or dynamical_matrix.numel() != force_constants.numel()):
+        raise ValueError("phonon_force_constants: inconsistent operand shapes")
+    _lib.check(lib.alignn_b200_phonon_force_constants(
+        _supercell_arg(supercell), float(delta), float(force_multiplier), atom_offsets.data_ptr(), B,
+        row_offsets.data_ptr(), grad.data_ptr(), grad.shape[0], masses.data_ptr(), fc_offsets.data_ptr(),
+        force_constants.numel(), force_constants.data_ptr(), dynamical_matrix.data_ptr(), status.data_ptr(),
+        stream_ptr()), "alignn_b200_phonon_force_constants")
+
+
+@_on_tensor_device
+def phonon_dynamical_matrix(dynamical_matrix: torch.Tensor, fc_offsets: torch.Tensor, crystals: torch.Tensor,
+                            qpoints: torch.Tensor, out: torch.Tensor, status: torch.Tensor, *, supercell,
+                            modes: int) -> None:
+    """D(q) = sum_R exp(-2 pi i q.R) D_N[R] (ASE 3.22.1 `Phonons.band_structure`'s Fourier sum) for a block of
+    (crystal, q) pairs whose crystals all have `modes` modes, one launch (alignn_b200_phonon_dynamical_matrix).
+
+    dynamical_matrix [fc_offsets[B]] float64 (the D_N of `phonon_force_constants`); fc_offsets [B+1] int64; crystals
+    [Q] int32; qpoints [Q,3] float64 (fractional); out [Q, modes, modes] complex128 (written: Hermitian, both
+    triangles); status [B] int32 (PHONON_BAD_INPUT: crystal c's D_N slice is not [Nc, modes, modes] inside the buffer;
+    its pairs are not written).  Enqueue only."""
+    lib = _lib.load()
+    _phonon_operands("phonon_dynamical_matrix", [(dynamical_matrix, torch.float64), (fc_offsets, torch.int64),
+                                                 (crystals, torch.int32), (qpoints, torch.float64),
+                                                 (out, torch.complex128), (status, torch.int32)],
+                     dynamical_matrix.device)
+    B, Q = fc_offsets.numel() - 1, crystals.numel()
+    if B < 1 or status.numel() != B or qpoints.numel() != 3 * Q or out.numel() != Q * int(modes) * int(modes):
+        raise ValueError("phonon_dynamical_matrix: inconsistent operand shapes")
+    _lib.check(lib.alignn_b200_phonon_dynamical_matrix(
+        _supercell_arg(supercell), int(modes), dynamical_matrix.data_ptr(), fc_offsets.data_ptr(), B,
+        dynamical_matrix.numel(), crystals.data_ptr(), qpoints.data_ptr(), Q, out.data_ptr(), status.data_ptr(),
+        stream_ptr()), "alignn_b200_phonon_dynamical_matrix")
+
+
 class _SegmentMean(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, gptr):

@@ -672,6 +672,50 @@ int alignn_b200_md_step(const alignn_b200_md_params* params, const int64_t* atom
                         double* positions, double* momenta, float* forces, double* kinetic_energy, double* temperature,
                         int32_t* status, alignn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Phonons (csrc/phonon_device.cu): ASE 3.22.1's finite-displacement `Phonons` (ase/phonons.py) with
+ * `read(acoustic=True)` and its defaults (method='frederiksen', symmetrize=3, offset 0) and the Fourier sum of
+ * `band_structure` -- what `ase_phonon` (alignn/ff/ff.py:1337-1430) runs one crystal at a time -- for a batch of
+ * crystals sharing one supercell (N0, N1, N2) of Nc = N0 N1 N2 cells.  Cell c = (m0, m1, m2) in C order.  Device
+ * pointers except `supercell` (host, int32 [3]), caller-owned buffers, enqueue-only on `stream`.
+ * ---------------------------------------------------------------------------------------- */
+#define ALIGNN_B200_PHONON_MAX_CELLS 3072   /* Nc limit: the dynamical-matrix kernel keeps one phase per cell in 48 KB */
+
+/* One launch for the batch, one CTA per crystal.  Crystal c has n = atom_offsets[c+1] - atom_offsets[c] atoms and
+ * M = 3n modes; its forces are the 6n displaced supercells of Nc n rows each, rows row_offsets[c] + k Nc n + cell n + a'
+ * for displacement k = 6a + 2i + (sign > 0) (atom a of cell 0, direction i, sign -1 then +1).  Per crystal with status 0:
+ *   F = fp32(grad * force_multiplier), widened to double; f[a] -= f.sum(0) on each displaced set (a fixed-order double
+ *   reduction); C_N[cell, 3a+i, 3a'+j] = (F_minus - F_plus) / (2 delta) of row cell n + a', component j; three rounds of
+ *   symmetrize (C[R] = 0.5 C[R] + 0.5 C[-R]^T, the cells at N/2 along an even axis left out) and acoustic (each
+ *   diagonal block of cell 0 minus the sum over cells and a' of its block row); D_N = C_N * (m_a^-1/2 m_a'^-1/2).
+ *   force_constants and dynamical_matrix get [Nc, M, M] double at fc_offsets[c].
+ *   Status 3 (inconsistent input): row_offsets[c+1] - row_offsets[c] != 6 n Nc n, the rows not inside [0, grad_rows),
+ *   fc_offsets[c+1] - fc_offsets[c] != Nc M M or not inside [0, fc_elems), or n < 1.  Status 5: a force product is not
+ *   finite.  Either way nothing else is read or written for c.  Crystals with a nonzero status are not touched.
+ *   atom_offsets / row_offsets / fc_offsets [num_crystals+1] int64; grad [grad_rows, 3] fp32; masses [sum n] double
+ *   (amu, > 0); status [num_crystals] int32.
+ * Rejected (ALIGNN_ERR_BAD_ARG, nothing enqueued): a NULL pointer, a supercell entry < 1 or Nc above
+ * ALIGNN_B200_PHONON_MAX_CELLS, delta not finite and > 0, a non-finite force_multiplier, num_crystals < 1,
+ * grad_rows or fc_elems < 0. */
+int alignn_b200_phonon_force_constants(const int32_t* supercell, double delta, float force_multiplier,
+                                       const int64_t* atom_offsets, int64_t num_crystals, const int64_t* row_offsets,
+                                       const float* grad, int64_t grad_rows, const double* masses,
+                                       const int64_t* fc_offsets, int64_t fc_elems, double* force_constants,
+                                       double* dynamical_matrix, int32_t* status, alignn_stream_t stream);
+
+/* D(q) = sum_R exp(-2 pi i q.R) D_N[R] for num_q (crystal, q) pairs whose crystals all have `modes` = M modes, one CTA
+ * per pair: crystals [num_q] int32, qpoints [num_q, 3] double (fractional, reciprocal basis of the unit cell).  R is
+ * Phonons.lattice_vectors: per axis (m + N/2) % N - N/2.  The sum runs in cell order.  out [num_q, M, M] complex128
+ * (interleaved double pairs): the upper triangle r <= s as summed, the lower its conjugate, the diagonal's imaginary
+ * part 0.  Status 3 for crystal c when fc_offsets[c+1] - fc_offsets[c] != Nc M M or the slice is not inside
+ * [0, fc_elems); the pairs of a crystal with a nonzero status, or an id outside [0, num_crystals), are not written.
+ * Rejected (ALIGNN_ERR_BAD_ARG, nothing enqueued): a NULL pointer, a bad supercell (as above), modes not a positive
+ * multiple of 3, num_crystals < 1, fc_elems < 0, num_q outside [0, INT32_MAX]. */
+int alignn_b200_phonon_dynamical_matrix(const int32_t* supercell, int64_t modes, const double* dynamical_matrix,
+                                        const int64_t* fc_offsets, int64_t num_crystals, int64_t fc_elems,
+                                        const int32_t* crystals, const double* qpoints, int64_t num_q, double* out,
+                                        int32_t* status, alignn_stream_t stream);
+
 /* Per-graph mean over node rows (dgl.nn.AvgPooling, alignn.py:325) and its backward. */
 int alignn_b200_segment_mean(const float* x, const int32_t* graph_ptr /*[B+1]*/, int64_t B, int d, float* out,
                              alignn_stream_t stream);
