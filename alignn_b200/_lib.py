@@ -86,6 +86,8 @@ class GemmGatherArgs(C.Structure):
         ("C", _fp), ("ldc", C.c_int64),
         ("stats", _fp),
         ("stream", _fp),
+        ("bn_R", _fp), ("ld_bn_R", C.c_int64),
+        ("bn_scale", _fp), ("bn_shift", _fp), ("bn_mean", _fp), ("bn_rstd", _fp),
     ]
 
 

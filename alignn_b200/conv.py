@@ -92,6 +92,12 @@ class _EdgeGatedConvFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, cfg: _Cfg, x, y, W_sg, b_sg, W_dg, b_dg, W_eg, b_eg, W_su, b_su, W_du, b_du, nw, nb, ew, eb):
         ix = cfg.index
+        d = x.shape[1]
+        # inputs that are train-mode BatchNorm outputs: their gradients (gx, gy below) also leave those BatchNorms'
+        # backward statistics (ops.bn_fold_take)
+        ctx.fold_in = (None, None)
+        if cfg.norm_nodes != NORM_LAYER:
+            ctx.fold_in = (ops.bn_fold_take(x, d), ops.bn_fold_take(y, d))
         x = x.contiguous()
         y = y.contiguous()
         ops.require_cuda(x, y)
@@ -143,6 +149,8 @@ class _EdgeGatedConvFn(torch.autograd.Function):
             n_aux = ops.bn_finalize(out["partials"], 1, Nn, nw, nb, bnn.eps, _momentum(bnn),
                                     bnn.running_mean if track_n else None, bnn.running_var if track_n else None)
             x_out = ops.affine_silu_residual(out["XP"], x if cfg.residual else None, n_aux[0], n_aux[1])
+            ctx.fold_out = (ops.bn_fold_offer(x_out, out["XP"], *n_aux),
+                            ops.bn_fold_offer(y_out, out["M"], *e_aux) if y_out is not None else None)
             for bn in (bnn, bne):
                 if bn.track_running_stats and bn.num_batches_tracked is not None:
                     bn.num_batches_tracked.add_(1)
@@ -193,9 +201,13 @@ def _first_backward(ctx, gx_out, gy_out, saved=None, create_graph=False):
             sc, sh, mu, rs = cfg.e_aux
             e = dict(w=sc, b=sh, mean=mu, rstd=rs)
         if cfg.norm_nodes == NORM_STATS:
-            n["c1"], n["c2"] = ops.bn_backward_reduce(XP, gx_out, n["w"], n["b"], n["mean"], n["rstd"])
+            # from the partials the consumer's data-gradient GEMM attached to gx_out / gy_out, else a reduction pass
+            fn, fe = ctx.fold_out
+            n["c1"], n["c2"] = ops.bn_backward_stats(fn, gx_out, XP, n["w"], n["b"], n["mean"], n["rstd"])
             if gy_out is not None:
-                e["c1"], e["c2"] = ops.bn_backward_reduce(M, gy_out, e["w"], e["b"], e["mean"], e["rstd"])
+                e["c1"], e["c2"] = ops.bn_backward_stats(fe, gy_out, M, e["w"], e["b"], e["mean"], e["rstd"])
+            elif fe is not None:
+                fe.release()
     # Parameter gradients are off the critical path of backward.  With a queue installed (FlatGradAllReducer.deferring())
     # the five weight-gradient GEMMs and the nine bias / norm-parameter reductions of this conv are only registered
     # here and computed by two batched launches at the end of backward, straight into the flat gradient buffer.
@@ -214,8 +226,11 @@ def _first_backward(ctx, gx_out, gy_out, saved=None, create_graph=False):
     # residual added in the epilogue) and weight gradients (wgrad_tc.cu, split-K over rows)
     need = ctx.needs_input_grad
     gx = gy = None
+    fold_x, fold_y = (None, None) if create_graph else ctx.fold_in
+    ctx.fold_in = (None, None)          # used once: a retained graph's next backward falls back (ops.BNFold)
     if need[1]:
-        gx = ops.gemm_gather(GP, img_catT, None, add0=gx_out if cfg.residual else None)
+        gx, part = ops.dgrad_gemm(fold_x, GP, img_catT, add0=gx_out if cfg.residual else None)
+        ops.bn_fold_attach(gx, fold_x, part)
     if deferred:
         for j, W in enumerate((W_sg, W_du, W_dg, W_su)):           # column blocks of GP: e_src | Bh | e_dst | src_update
             queue.add(GP[:, j * d:(j + 1) * d], x, W)
@@ -236,7 +251,8 @@ def _first_backward(ctx, gx_out, gy_out, saved=None, create_graph=False):
         gW_eg = ops.wgrad(GM, y, groups=1)
     if need[2]:
         res_y = gy_out if (gy_out is not None and cfg.residual) else None
-        gy = ops.gemm_gather(GM, img_egT, None, add0=res_y)
+        gy, part = ops.dgrad_gemm(fold_y, GM, img_egT, add0=res_y)
+        ops.bn_fold_attach(gy, fold_y, part)
     if not params or deferred:
         grads = (None, gx, gy) + (None,) * 14
         return (grads, GP, GM, res[4]) if create_graph else grads

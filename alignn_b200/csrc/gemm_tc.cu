@@ -3,12 +3,17 @@
 //
 //   C[r, :] = A[r, :] * W^T (+ bias) (+ add0[i0(r), :]) (+ add1[i1(r), :])                                  r < M
 //   stats[cta][0/1][c] = partial sums over the CTA's tiles of C[r, c] and C[r, c]^2                         (optional)
+//   or, BatchNorm-backward statistics (gemm_bf16x3_bn_bwd_kernel), with gu = C[r, c] silu'(R[r, c] scale[c] + shift[c]):
+//   stats[cta][0/1][c] = partial sums over the CTA's tiles of gu and gu (R[r, c] - mean[c]) rstd[c]
 //
 // gemm_nt is the plain form (add0 = the residual, no index).  gemm_gather is the edge-gate kernel of the conv path: with
 // A = edge features y, add0 = P[src, 0:d] (e_src), add1 = P[dst, 2d:3d] (e_dst + both biases) it is the pre-activation
 // gate  m = e_src[src] + e_dst[dst] + edge_gate(y)  of alignn/models/alignn.py:98-101 in ONE pass over y, plus the
 // per-channel batch statistics BatchNorm1d(m) needs (alignn.py:123).  With add0 = the incoming gradient it is the
-// data-gradient GEMM of the backward (residual in the epilogue).
+// data-gradient GEMM of the backward (residual in the epilogue).  When the data gradient C is the incoming gradient of a
+// train-mode BatchNorm1d + SiLU (the output of the previous layer), the BatchNorm-backward form of the kernel also reads
+// that BatchNorm's input R row by row and leaves the sums bn_backward_reduce would take over C and R: the reduction pass
+// over the gradient and its launches go away.
 //
 // A is the fp32 activation matrix, read once per column tile: the producer warps copy its K-chunks global -> shared with
 // cp.async into a ring of fp32 stages (the bytes in flight are set by shared memory, not by registers) and split them
@@ -73,12 +78,20 @@ struct Cfg {
   static constexpr int BAR_OFF = STAT_OFF + STAT_BYTES;
   static constexpr int SMEM = BAR_OFF + 128;
   static_assert(SMEM <= 232448, "shared memory budget of one sm_90 CTA");
+  // BatchNorm-backward form: scale, shift, mean, rstd [4][kMaxStatN] after the barriers, read per row by the epilogue
+  // (sixteen registers per lane fewer than holding this lane's columns of them)
+  static constexpr int BNV_OFF = SMEM;
+  static constexpr int SMEM_BNB = BNV_OFF + 4 * kMaxStatN * 4;
+  static_assert(SMEM_BNB <= 232448, "shared memory budget of one sm_90 CTA");
   // row-oriented epilogue: LPR lanes per row (one float4 each), RPI rows per warp instruction, ITERS instructions
   // for the warp's rows, G rows whose addends are in flight before the first store
   static constexpr int LPR = BN / 4;
   static constexpr int RPI = 32 / LPR;
   static constexpr int ITERS = WARP_ROWS / RPI;
   static constexpr int G = ITERS < 8 ? ITERS : 8;
+  // the BatchNorm-backward epilogue computes more per row: at BN = 128 (the other row half's 64 accumulators still
+  // live) eight rows in flight spill, four do not
+  static constexpr int G_BNB = BN == 128 ? 4 : G;
 };
 
 struct Params {
@@ -90,6 +103,9 @@ struct Params {
   const float* add1; int64_t ld1; const int32_t* idx1;
   float* C; int64_t ldc;
   float* stats;                                          // [gridDim.x][2][N] or NULL (requires N <= kMaxStatN)
+  // BatchNorm-backward statistics (gemm_bf16x3_bn_bwd_kernel only): R [M, N] row stride ldr, per-channel vectors [N]
+  const float* bnR; int64_t ldr;
+  const float *bn_scale, *bn_shift, *bn_mean, *bn_rstd;
 };
 
 // byte offset of element (r, k) inside one chunk plane (rows x BK, core-matrix order)
@@ -103,46 +119,74 @@ __device__ __forceinline__ float4 ld4s(const float* p) {          // 4 scalars: 
 // One consumer warp's WARP_ROWS rows of the tile, from its staged accumulator rows `stg` (row pitch Cfg::PITCH):
 //   C[r, col .. col + 3] = (acc + bias) + (add0[i0(r)] + add1[i1(r)]),   r = row0 + rw
 // i0 / i1 of row rw sit in lane rw (-1: no addend); col = n0 + 4 (lane % LPR).  s / q collect this lane's column
-// sums of C and C^2 over its valid rows in row order.
-template <int BN>
+// sums of C and C^2 over its valid rows in row order -- or, with BNB, of gu = C silu'(R sc + sh) and gu (R - mu) rs,
+// the arithmetic of bn_backward_reduce_kernel (egc_kernels.cu), R's rows loaded together with the add0 rows (add1 is
+// NULL then).
+__device__ __forceinline__ void bn_bwd_acc(float o, float v, float sc, float sh, float mu, float rs, float& s, float& q) {
+  const float gu = o * dsilu_(v * sc + sh);
+  s += gu;
+  q += gu * (v - mu) * rs;
+}
+
+template <int BN, bool BNB>
 __device__ __forceinline__ void epilogue_rows(const float* stg, float* __restrict__ C, int64_t ldc,
                                               const float* __restrict__ add0, int64_t ld0,
                                               const float* __restrict__ add1, int64_t ld1, int i0, int i1, int row0,
-                                              int M, int col, int lane, float4 b, float4& s, float4& q) {
+                                              int M, int col, int lane, float4 b, float4& s, float4& q,
+                                              const float* __restrict__ R, int64_t ldr, const float* bnv) {
   using F = Cfg<BN>;
   const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
   const int lr = lane / F::LPR, c = (lane % F::LPR) * 4;
+  constexpr int G = BNB ? F::G_BNB : F::G;
 #pragma unroll 1   // unrolled, the row groups of BN = 128 spill at the 128-register cap
-  for (int g0 = 0; g0 < F::ITERS; g0 += F::G) {
-    float4 va[F::G], vb[F::G];
+  for (int g0 = 0; g0 < F::ITERS; g0 += G) {
+    // with BNB, R's rows take the registers of the second addend (add1 is NULL there)
+    float4 va[G], vb[G];
 #pragma unroll
-    for (int g = 0; g < F::G; ++g) {                         // every addend row of the group is requested first
+    for (int g = 0; g < G; ++g) {                            // every addend row of the group is requested first
       const int rw = (g0 + g) * F::RPI + lr;
-      const int ia = __shfl_sync(0xffffffffu, i0, rw), ib = __shfl_sync(0xffffffffu, i1, rw);
+      const int ia = __shfl_sync(0xffffffffu, i0, rw);
       va[g] = ia >= 0 ? ld4(add0 + (int64_t)ia * ld0 + col) : z4;
-      vb[g] = ib >= 0 ? ld4(add1 + (int64_t)ib * ld1 + col) : z4;
+      if constexpr (BNB) {
+        vb[g] = row0 + rw < M ? ld4(R + (int64_t)(row0 + rw) * ldr + col) : z4;
+      } else {
+        const int ib = __shfl_sync(0xffffffffu, i1, rw);
+        vb[g] = ib >= 0 ? ld4(add1 + (int64_t)ib * ld1 + col) : z4;
+      }
     }
 #pragma unroll
-    for (int g = 0; g < F::G; ++g) {
+    for (int g = 0; g < G; ++g) {
       const int rw = (g0 + g) * F::RPI + lr;
       if (row0 + rw >= M) continue;
       const float4 a = *reinterpret_cast<const float4*>(stg + rw * F::PITCH + c);
-      const float4 a0 = va[g], a1 = vb[g];
+      const float4 a0 = va[g], a1 = BNB ? z4 : vb[g];
       float4 o;
       o.x = (a.x + b.x) + (a0.x + a1.x);
       o.y = (a.y + b.y) + (a0.y + a1.y);
       o.z = (a.z + b.z) + (a0.z + a1.z);
       o.w = (a.w + b.w) + (a0.w + a1.w);
       *reinterpret_cast<float4*>(C + (int64_t)(row0 + rw) * ldc + col) = o;
-      s.x += o.x; s.y += o.y; s.z += o.z; s.w += o.w;
-      q.x = fmaf(o.x, o.x, q.x); q.y = fmaf(o.y, o.y, q.y); q.z = fmaf(o.z, o.z, q.z); q.w = fmaf(o.w, o.w, q.w);
+      if constexpr (BNB) {
+        const float4 v = vb[g];
+        const float4 sc = *reinterpret_cast<const float4*>(bnv + col);
+        const float4 sh = *reinterpret_cast<const float4*>(bnv + kMaxStatN + col);
+        const float4 mu = *reinterpret_cast<const float4*>(bnv + 2 * kMaxStatN + col);
+        const float4 rs = *reinterpret_cast<const float4*>(bnv + 3 * kMaxStatN + col);
+        bn_bwd_acc(o.x, v.x, sc.x, sh.x, mu.x, rs.x, s.x, q.x);
+        bn_bwd_acc(o.y, v.y, sc.y, sh.y, mu.y, rs.y, s.y, q.y);
+        bn_bwd_acc(o.z, v.z, sc.z, sh.z, mu.z, rs.z, s.z, q.z);
+        bn_bwd_acc(o.w, v.w, sc.w, sh.w, mu.w, rs.w, s.w, q.w);
+      } else {
+        s.x += o.x; s.y += o.y; s.z += o.z; s.w += o.w;
+        q.x = fmaf(o.x, o.x, q.x); q.y = fmaf(o.y, o.y, q.y); q.z = fmaf(o.z, o.z, q.z); q.w = fmaf(o.w, o.w, q.w);
+      }
     }
   }
 }
 
-template <int BN>
-__global__ void __launch_bounds__(THREADS, 1)
-gemm_bf16x3_kernel(const Params p) {
+// The whole kernel; BNB selects the BatchNorm-backward statistics (stats != NULL and the bn fields of Params set).
+template <int BN, bool BNB>
+__device__ __forceinline__ void gemm_bf16x3_body(const Params& p) {
   using F = Cfg<BN>;
   extern __shared__ __align__(128) uint8_t smem[];
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + F::BAR_OFF);
@@ -155,7 +199,7 @@ gemm_bf16x3_kernel(const Params p) {
   const int n_tiles = N / BN;
   const int m_tiles = (M + BM - 1) / BM;
   const int total = m_tiles * n_tiles;
-  const bool do_stats = p.stats != nullptr;
+  const bool do_stats = BNB || p.stats != nullptr;
 
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full[s], LOAD_WARPS + 1); tc::mbar_init(&empty[s], MMA_WARPS / 2); }
@@ -165,6 +209,13 @@ gemm_bf16x3_kernel(const Params p) {
   if (do_stats) {
     float* stat = reinterpret_cast<float*>(smem + F::STAT_OFF);
     for (int i = tid; i < STAT_ROWS * 2 * N; i += THREADS) stat[i] = 0.f;
+  }
+  float* bnv = reinterpret_cast<float*>(smem + F::BNV_OFF);
+  if constexpr (BNB) {
+    for (int i = tid; i < N; i += THREADS) {
+      bnv[i] = __ldg(p.bn_scale + i); bnv[kMaxStatN + i] = __ldg(p.bn_shift + i);
+      bnv[2 * kMaxStatN + i] = __ldg(p.bn_mean + i); bnv[3 * kMaxStatN + i] = __ldg(p.bn_rstd + i);
+    }
   }
   __syncthreads();
 
@@ -323,8 +374,8 @@ gemm_bf16x3_kernel(const Params p) {
               make_float2(acc[h][4 * j + 2 * e], acc[h][4 * j + 2 * e + 1]);
       __syncwarp();
       s4[h] = make_float4(0.f, 0.f, 0.f, 0.f); q4[h] = s4[h];
-      epilogue_rows<BN>(stg, p.C, p.ldc, p.add0, p.ld0, p.add1, p.ld1, i0[h], i1[h], m0 + h * 64 + wrow, M, col, lane,
-                        b, s4[h], q4[h]);
+      epilogue_rows<BN, BNB>(stg, p.C, p.ldc, p.add0, p.ld0, p.add1, p.ld1, i0[h], i1[h], m0 + h * 64 + wrow, M, col,
+                             lane, b, s4[h], q4[h], p.bnR, p.ldr, bnv);
       __syncwarp();                                          // staged rows read before they are overwritten
     }
     if (do_stats) {
@@ -366,6 +417,14 @@ gemm_bf16x3_kernel(const Params p) {
     }
   }
 }
+
+template <int BN>
+__global__ void __launch_bounds__(THREADS, 1)
+gemm_bf16x3_kernel(const Params p) { gemm_bf16x3_body<BN, false>(p); }
+
+template <int BN>
+__global__ void __launch_bounds__(THREADS, 1)
+gemm_bf16x3_bn_bwd_kernel(const Params p) { gemm_bf16x3_body<BN, true>(p); }
 
 // Weight images: W[N,K] fp32 (or W^T of a [K,N] array) -> [N/BN tiles][K/32 chunks][hi, lo][BN x 32 bf16 in
 // core-matrix order].  Every table entry converts one source block into its place inside a (possibly larger) image, so
@@ -420,24 +479,27 @@ inline int num_sms() {
   return sms;
 }
 
-template <int BN>
+template <int BN, bool BNB>
 int launch_bn(const Params& p, int grid, cudaStream_t st) {
   using F = Cfg<BN>;
+  auto kernel = BNB ? gemm_bf16x3_bn_bwd_kernel<BN> : gemm_bf16x3_kernel<BN>;
+  const int smem = BNB ? F::SMEM_BNB : F::SMEM;
   static alignn::DeviceOnce configured; int cfg_dev;   // idempotent attribute; a benign race sets it twice
   if (configured.needed(&cfg_dev)) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16x3_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, F::SMEM);
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return record_cuda_error((int)e);
     configured.done(cfg_dev);
   }
-  gemm_bf16x3_kernel<BN><<<grid, THREADS, F::SMEM, st>>>(p);
+  kernel<<<grid, THREADS, smem, st>>>(p);
   return check_launch();
 }
 
-inline int launch(const Params& p, int grid, cudaStream_t st) {
+template <bool BNB>
+int launch(const Params& p, int grid, cudaStream_t st) {
   switch (pick_bn(p.N)) {
-    case 128: return launch_bn<128>(p, grid, st);
-    case 64: return launch_bn<64>(p, grid, st);
-    case 32: return launch_bn<32>(p, grid, st);
+    case 128: return launch_bn<128, BNB>(p, grid, st);
+    case 64: return launch_bn<64, BNB>(p, grid, st);
+    case 32: return launch_bn<32, BNB>(p, grid, st);
     default: return ALIGNN_ERR_UNSUPPORTED_D;
   }
 }
@@ -488,7 +550,7 @@ int alignn_b200_gemm_nt(const float* A, int64_t lda, const void* w_image, int64_
   p.C = C; p.ldc = ldc;
   const int total = ((p.M + BM - 1) / BM) * (N / bn);
   const int grid = total < num_sms() ? total : num_sms();   // persistent: one CTA per SM
-  return launch(p, grid, (cudaStream_t)stream);
+  return launch<false>(p, grid, (cudaStream_t)stream);
 }
 
 int alignn_b200_gemm_gather_stat_rows(int64_t M, int N) {
@@ -514,6 +576,18 @@ int alignn_b200_gemm_gather(const alignn_b200_gemm_gather_args* a) {
   const int bn = pick_bn(a->N);
   if (bn == 0) return ALIGNN_ERR_UNSUPPORTED_D;
   if (a->stats && a->N > kMaxStatN) return ALIGNN_ERR_BAD_ARG;   // column partials of every warp live in shared memory
+  const bool bnb = a->bn_R != nullptr;
+  if (bnb) {
+    // the sums go to `stats` in place of the forward statistics; R is read through the non-coherent path while C is
+    // being written, so the two must not overlap
+    if (!a->stats || a->add1 || !a->bn_scale || !a->bn_shift || !a->bn_mean || !a->bn_rstd) return ALIGNN_ERR_BAD_ARG;
+    if ((a->ld_bn_R % 4) || a->ld_bn_R < a->N || ((uintptr_t)a->bn_R & 15)) return ALIGNN_ERR_BAD_ARG;
+    const uintptr_t r0 = (uintptr_t)a->bn_R, r1 = r0 + ((a->M - 1) * a->ld_bn_R + a->N) * sizeof(float);
+    const uintptr_t c0 = (uintptr_t)a->C, c1 = c0 + ((a->M - 1) * a->ldc + a->N) * sizeof(float);
+    if (r0 < c1 && c0 < r1) return ALIGNN_ERR_BAD_ARG;
+  } else if (a->bn_scale || a->bn_shift || a->bn_mean || a->bn_rstd) {
+    return ALIGNN_ERR_BAD_ARG;
+  }
   Params p;
   p.A = a->A; p.lda = a->lda;
   p.M = (int)a->M; p.N = a->N; p.K = a->K;
@@ -522,10 +596,12 @@ int alignn_b200_gemm_gather(const alignn_b200_gemm_gather_args* a) {
   p.add0 = a->add0; p.ld0 = a->ld0; p.idx0 = a->idx0;
   p.add1 = a->add1; p.ld1 = a->ld1; p.idx1 = a->idx1;
   p.C = a->C; p.ldc = a->ldc; p.stats = a->stats;
+  p.bnR = a->bn_R; p.ldr = a->ld_bn_R;
+  p.bn_scale = a->bn_scale; p.bn_shift = a->bn_shift; p.bn_mean = a->bn_mean; p.bn_rstd = a->bn_rstd;
   const int total = ((p.M + BM - 1) / BM) * (p.N / bn);
   int grid = total < num_sms() ? total : num_sms();
   if (p.stats) grid = alignn_b200_gemm_gather_stat_rows(p.M, p.N);   // the caller sized `stats` for this many CTAs
-  return launch(p, grid, (cudaStream_t)a->stream);
+  return bnb ? launch<true>(p, grid, (cudaStream_t)a->stream) : launch<false>(p, grid, (cudaStream_t)a->stream);
 }
 
 }  // extern "C"

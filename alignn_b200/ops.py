@@ -825,12 +825,17 @@ def gemm_nt(A: torch.Tensor, w: WeightImage, bias: Optional[torch.Tensor] = None
 def gemm_gather(A: torch.Tensor, w: WeightImage, bias: Optional[torch.Tensor] = None, *,
                 add0: Optional[torch.Tensor] = None, idx0: Optional[torch.Tensor] = None,
                 add1: Optional[torch.Tensor] = None, idx1: Optional[torch.Tensor] = None,
-                stats: bool = False, out: Optional[torch.Tensor] = None):
+                stats: bool = False, out: Optional[torch.Tensor] = None, bn_bwd=None):
     """out[r] = A[r] @ W^T (+ bias) (+ add0[idx0[r]]) (+ add1[idx1[r]]) on wgmma.
 
     add0 / add1 are 2-D fp32 views with unit column stride and w.N columns (column slices of a wider matrix are fine);
     idx None = identity (a residual).  stats=True also returns the per-CTA partial column sums [rows, 2, N] of out and
-    out^2 (alignn.py:123 batch statistics; feed `bn_finalize(partials, 0, M, ...)`)."""
+    out^2 (alignn.py:123 batch statistics; feed `bn_finalize(partials, 0, M, ...)`).
+
+    bn_bwd=(R, scale, shift, mean, rstd): out is the incoming gradient of a train-mode BatchNorm1d + SiLU with input
+    R [M, N]; also returns partials [rows, 2, N] of sum gu and sum gu * xhat, gu = out * silu'(R * scale + shift),
+    xhat = (R - mean) * rstd, i.e. what bn_backward_reduce reduces (c1, c2 = colsum(partials.view(rows, 2 * N), 1 / M)).
+    out itself is bitwise what the call without bn_bwd writes.  Needs add1 = None and no stats request."""
     lib = _lib.load()
     if A.dim() != 2 or A.stride(1) != 1 or A.shape[1] != w.K:
         raise RuntimeError(f"gemm_gather: A must be [M,{w.K}] with unit column stride, got {tuple(A.shape)}/{A.stride()}")
@@ -849,10 +854,20 @@ def gemm_gather(A: torch.Tensor, w: WeightImage, bias: Optional[torch.Tensor] = 
             raise RuntimeError("gemm_gather: identity-indexed addend must have M rows")
         if ix is not None and (ix.dtype != torch.int32 or not ix.is_cuda or not ix.is_contiguous() or ix.numel() != M):
             raise RuntimeError("gemm_gather: index must be a contiguous int32 CUDA tensor with M entries")
+    bn = (None,) * 5
+    if bn_bwd is not None:
+        if stats or add1 is not None:
+            raise RuntimeError("gemm_gather: bn_bwd excludes stats and add1")
+        bn = tuple(bn_bwd)
+        R = bn[0]
+        require_cuda(*bn[1:])
+        if R.dim() != 2 or R.shape != (M, w.N) or R.stride(1) != 1 or not R.is_cuda or R.dtype != torch.float32 \
+                or any(v.numel() != w.N for v in bn[1:]):
+            raise RuntimeError("gemm_gather: bn_bwd needs R [M, N] with unit column stride and [N] vectors")
     if out is None:
         out = torch.empty(M, w.N, device=A.device, dtype=torch.float32)
     part = None
-    if stats:
+    if stats or bn_bwd is not None:
         rows = int(lib.alignn_b200_gemm_gather_stat_rows(M, w.N))
         part = torch.empty(max(rows, 1), 2, w.N, device=A.device, dtype=torch.float32)
     a = _lib.GemmGatherArgs(
@@ -860,12 +875,16 @@ def gemm_gather(A: torch.Tensor, w: WeightImage, bias: Optional[torch.Tensor] = 
         w_image=ptr_any(w.buf), bias=ptr_any(bias),
         add0=ptr_any(add0), ld0=add0.stride(0) if add0 is not None else 0, idx0=ptr_any(idx0),
         add1=ptr_any(add1), ld1=add1.stride(0) if add1 is not None else 0, idx1=ptr_any(idx1),
-        C=ptr_any(out), ldc=out.stride(0), stats=ptr_any(part), stream=stream_ptr())
+        C=ptr_any(out), ldc=out.stride(0), stats=ptr_any(part), stream=stream_ptr(),
+        bn_R=ptr_any(bn[0]), ld_bn_R=bn[0].stride(0) if bn[0] is not None else 0,
+        bn_scale=ptr_any(bn[1]), bn_shift=ptr_any(bn[2]), bn_mean=ptr_any(bn[3]), bn_rstd=ptr_any(bn[4]))
     nb = 4 * M * (w.K + w.N) + (8 * M if idx0 is not None else 0) + (4 * M * w.N if (add0 is not None and idx0 is None) else 0)
+    nb += 4 * M * w.N if bn_bwd is not None else 0
     kind = "+gather" if idx0 is not None else ("+residual" if add0 is not None else "")
-    with _span(f"gemm_gather<{min(w.N, 256)}>" + kind + ("+stats" if stats else ""), nb):
+    kind += "+stats" if stats else ("+bn_bwd" if bn_bwd is not None else "")
+    with _span(f"gemm_gather<{min(w.N, 256)}>" + kind, nb):
         _lib.check(lib.alignn_b200_gemm_gather(C.byref(a)), "alignn_b200_gemm_gather")
-    return (out, part) if stats else out
+    return (out, part) if (stats or bn_bwd is not None) else out
 
 
 def wgrad_supported(DA: int, DB: int) -> bool:
@@ -1073,6 +1092,82 @@ def tc_linear(x: torch.Tensor, lin) -> torch.Tensor:
     return _TCLinearFn.apply(x, lin.weight, lin.bias, tbl)
 
 
+# ---- train-mode BatchNorm backward statistics taken by the consumer's data-gradient GEMM ----------------------------
+# The first pass of a train-mode BatchNorm1d + SiLU backward reduces its input R and the incoming gradient g_out to
+# c1 = mean(gu), c2 = mean(gu * xhat).  When g_out is the data gradient of the next layer's Linear, that GEMM's epilogue
+# already holds g_out and can take the two sums on the way out (gemm_gather(..., bn_bwd=...)), saving the reduction pass.
+# The hand-off between the two autograd Functions:
+#   forward   the producer marks its output with a BNFold (R and the four vectors); a consumer that finds the mark on
+#             its input keeps the BNFold on its ctx
+#   backward  the consumer computes that input's gradient with the fold and attaches (fold, partials, _version) to the
+#             tensor it returns; the producer uses the partials only if it receives that tensor at that version for its
+#             own BNFold, and otherwise runs bn_backward_reduce -- autograd summed several contributions, a hook replaced
+#             or changed the gradient, or no consumer GEMM produced it (the pool, user code).
+# R must not outlive the backward that needs it (the producer's saved tensors are freed there, and a graph kept alive
+# by the caller's `loss` would otherwise pin every R of the step): the consumer drops its reference after its data-
+# gradient GEMM, and the producer's backward releases the fold's tensors.  A second backward through a retained graph
+# therefore runs bn_backward_reduce.
+_FOLD_ATTR, _PART_ATTR = "_alignn_b200_bn_fold", "_alignn_b200_bn_part"
+
+
+class bn_fold:
+    """Process-wide switch: with `bn_fold.enabled = False` consumers take no fold and every train-mode BatchNorm
+    backward runs bn_backward_reduce."""
+    enabled = True
+
+
+class BNFold:
+    __slots__ = ("vecs",)
+
+    def __init__(self, R, scale, shift, mean, rstd):
+        self.vecs = (R, scale, shift, mean, rstd)        # None once the producer's backward has run
+
+    def release(self) -> None:
+        self.vecs = None
+
+
+def bn_fold_offer(out: torch.Tensor, R, scale, shift, mean, rstd) -> BNFold:
+    """Producer forward: mark the BatchNorm + SiLU output `out` of input R."""
+    fold = BNFold(R, scale, shift, mean, rstd)
+    setattr(out, _FOLD_ATTR, fold)
+    return fold
+
+
+def bn_fold_take(x: torch.Tensor, n_cols: int) -> Optional[BNFold]:
+    """Consumer forward: the mark of x's producer, if x's gradient will be a GEMM output of n_cols columns."""
+    fold = getattr(x, _FOLD_ATTR, None)
+    if fold is None or fold.vecs is None or not bn_fold.enabled or tuple(fold.vecs[0].shape) != (x.shape[0], n_cols):
+        return None
+    return fold
+
+
+def dgrad_gemm(fold: Optional[BNFold], A: torch.Tensor, w: "WeightImage", **kw):
+    """Consumer backward: gemm_gather(A, w, **kw) -> (C, partials of the fold or None)."""
+    if fold is None or fold.vecs is None:
+        return gemm_gather(A, w, **kw), None
+    return gemm_gather(A, w, bn_bwd=fold.vecs, **kw)
+
+
+def bn_fold_attach(g: torch.Tensor, fold: Optional[BNFold], part: Optional[torch.Tensor]) -> None:
+    """Consumer backward: attach the partials to the gradient tensor g that is returned to autograd."""
+    if fold is not None and part is not None:
+        setattr(g, _PART_ATTR, (fold, part, g._version))
+
+
+def bn_backward_stats(fold: Optional[BNFold], g_out: torch.Tensor, R, scale, shift, mean, rstd):
+    """Producer backward: (c1, c2) from the consumer's partials if g_out is the tensor they were taken over, unchanged,
+    for this producer's fold; bn_backward_reduce otherwise.  Releases the fold's tensors either way."""
+    got = getattr(g_out, _PART_ATTR, None)
+    if fold is not None:
+        fold.release()
+    if fold is not None and got is not None and got[0] is fold and got[2] == g_out._version:
+        n, d = R.shape
+        part = got[1]
+        c = colsum(part.view(part.shape[0], 2 * d), 1.0 / n)
+        return c[:d], c[d:]
+    return bn_backward_reduce(R, g_out, scale, shift, mean, rstd)
+
+
 # ---- Linear -> BatchNorm1d(train) -> SiLU (embedding MLP layers) ------------------------------------
 class _MLPBNTrainFn(torch.autograd.Function):
     """One embedding layer in train mode, entirely on library kernels: tensor-core Linear, two-stage batch
@@ -1080,6 +1175,7 @@ class _MLPBNTrainFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, weight, bias, gamma, beta, bn, tbl):
+        ctx.fold_in = bn_fold_take(x, tbl.images["wT"].N)        # x is itself a train-mode BatchNorm output
         x = _pad_cols(x, tbl.images["w"].K)
         # Linear + per-channel batch statistics in one pass (column sums leave through the GEMM epilogue)
         R, part = gemm_gather(x, tbl.images["w"], bias.contiguous(), stats=True)
@@ -1090,6 +1186,7 @@ class _MLPBNTrainFn(torch.autograd.Function):
         if track and bn.num_batches_tracked is not None:
             bn.num_batches_tracked.add_(1)
         out = affine_silu_residual(R, None, scale, shift)
+        ctx.fold_out = bn_fold_offer(out, R, scale, shift, mean, rstd)
         ctx.save_for_backward(x, R, scale, shift, mean, rstd)
         ctx.tbl = tbl
         ctx.k_in = weight.shape[1]
@@ -1100,17 +1197,20 @@ class _MLPBNTrainFn(torch.autograd.Function):
     def backward(ctx, go):
         lib = _lib.load()
         x, R, scale, shift, mean, rstd = ctx.saved_tensors
+        c1, c2 = bn_backward_stats(ctx.fold_out, go, R, scale, shift, mean, rstd)
         go = go.contiguous()
         n, d = R.shape
-        c1, c2 = bn_backward_reduce(R, go, scale, shift, mean, rstd)
         gR = torch.empty_like(R)
         with _span("bn_backward_apply", 12 * n * d):
             _lib.check(lib.alignn_b200_bn_backward_apply(ptr(R), ptr(go), ptr(scale), ptr(shift), ptr(mean), ptr(rstd),
                                                          ptr(c1.contiguous()), ptr(c2.contiguous()), n, d, ptr(gR), stream_ptr()),
                        "alignn_b200_bn_backward_apply")
         gx = None
+        fold_in, ctx.fold_in = ctx.fold_in, None         # used once: a retained graph's next backward falls back
         if ctx.needs_input_grad[0]:
-            gx = gemm_gather(gR, ctx.tbl.images["wT"])[:, :ctx.k_in]
+            gx, part = dgrad_gemm(fold_in, gR, ctx.tbl.images["wT"])
+            gx = gx[:, :ctx.k_in]
+            bn_fold_attach(gx, fold_in, part)            # on the view autograd receives
         if input_grads_only.active:
             return gx, None, None, None, None, None, None
         gw = wgrad(gR, x, 1)[:, :ctx.k_in]

@@ -353,6 +353,16 @@ typedef struct {
   float* C; int64_t ldc;
   float* stats;                                             /* [stat_rows][2][N] or NULL */
   alignn_stream_t stream;
+  /* BatchNorm-backward statistics (all NULL: off).  When C is the incoming gradient g_out of a train-mode
+   * BatchNorm1d + SiLU whose input is R [M, N] (row stride ld_bn_R) and vectors scale, shift, mean, rstd [N], `stats`
+   * (required) receives per-CTA partial sums of gu and gu * (R - mean) * rstd, gu = C * silu'(R * scale + shift), in
+   * place of the sums of C and C^2: what alignn_b200_bn_backward_reduce writes, in the layout above.  C is written
+   * exactly as without the request.  R must not overlap C. */
+  const float* bn_R; int64_t ld_bn_R;
+  const float* bn_scale; const float* bn_shift; const float* bn_mean; const float* bn_rstd;
+  /* Appended fields leave ALIGNN_B200_VERSION as it is: every existing field keeps its offset, and a caller built
+   * against the shorter struct passes the old struct_size, which the call rejects with ALIGNN_ERR_STRUCT_SIZE before
+   * it reads a field.  The version changes when an existing field moves or an entry point goes away. */
 } alignn_b200_gemm_gather_args;
 
 int alignn_b200_gemm_gather(const alignn_b200_gemm_gather_args* args);

@@ -62,7 +62,7 @@ def record_calls(args):
                 kind = ("+gather" if kw.get("idx0") is not None else ("+residual" if kw.get("add0") is not None else ""))
                 if kw.get("add1") is not None:
                     kind += "+add1" + ("[idx]" if kw.get("idx1") is not None else "")
-                kind += "+stats" if kw.get("stats") else ""
+                kind += "+stats" if kw.get("stats") else ("+bn_bwd" if kw.get("bn_bwd") is not None else "")
             key = (f"{name}<{min(w.N, 256)}>{kind}", A.shape[0], w.N, w.K)
             if key in calls:
                 calls[key][4] += 1
@@ -95,6 +95,8 @@ def compulsory_bytes(fn_name, call_args, kw, M, N, K):
         if t is None:
             continue
         b += 4 * M * N if ix is None else 4 * t.shape[0] * N + 4 * M   # a gathered table is read once, plus its index
+    if kw.get("bn_bwd") is not None:
+        b += 4 * M * N + 4 * 4 * N                          # the BatchNorm input R and its four per-channel vectors
     return b
 
 
