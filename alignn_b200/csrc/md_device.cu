@@ -14,18 +14,24 @@
 // every division is IEEE's correctly rounded one, so T0 / T at rest is +inf as in numpy; the sums differ from numpy's
 // only in their order.  No floating-point atomics: every result depends on the crystal's own atoms and the fixed block
 // size only, so it is bitwise repeatable and independent of the batch around it.
+//
+// md_thermostat_kernel does the same for ASE 3.22.1's stochastic thermostats `Langevin` and `Andersen` (fixcm=True;
+// ase/md/langevin.py, ase/md/andersen.py), which `ForceField.run_nvt_langevin` / `run_nvt_andersen`
+// (alignn/ff/ff.py:444-508) run; oracle/md_thermostat_oracle.py is its specification.  Their noise is the
+// counter-based stream of md_noise.cuh, keyed by each crystal's own seed.
 #include <math.h>
 #include <stdint.h>
 
 #include "api_common.h"
 #include "alignn_b200.h"
+#include "md_noise.cuh"
 
 namespace alignn {
 namespace md {
 
 constexpr int kBlock = 256;
-enum { kOk = 0, kBadInput = 3 };
-enum { kNVE = 0, kBerendsen = 1 };
+enum { kOk = 0, kBadInput = 3, kOneAtom = 6 };
+enum { kNVE = 0, kBerendsen = 1, kLangevin = 2, kAndersen = 3 };
 
 // sum over the block of three per-thread partials, in a fixed order; every thread returns the totals
 __device__ __forceinline__ void block_sum3(double (*red)[3], double a, double b, double c, double out[3]) {
@@ -143,6 +149,243 @@ md_step_kernel(const alignn_b200_md_params p, const int64_t* __restrict__ atom_o
   }
 }
 
+// ASE 3.22.1's `Langevin` and `Andersen` (fixcm=True), one launch per evaluation e, one CTA per crystal; the noise of
+// the step that follows evaluation e is md_noise.cuh's stream at step index e.  Per crystal:
+//   1. forces F = fp32(grad * force_multiplier), written out;
+//   2. e >= 1: the second half of the previous step on the velocities v and (Langevin) rnd_vel the first half left in
+//      the workspaces: Langevin v += c1 F/m - c2 v + rnd_vel; Andersen v += 0.5 F/m dt, v -= (m.v)/M; then p = v m;
+//   3. ekin and T of evaluation e from p, as md_step_kernel;
+//   4. e < steps: the first half of step e + 1 (see the header), ending with x = x_new and the workspaces holding the
+//      velocities recomputed from the positions (and rnd_vel).
+// Divisions by 2 and 8 are multiplications by 0.5 and 0.125, the same correctly rounded result.  Each division by n or
+// M and every sum is as in md_step_kernel: IEEE, fixed order, no atomics.
+__global__ void __launch_bounds__(kBlock)
+md_thermostat_kernel(const alignn_b200_md_thermostat_params p, const int64_t* __restrict__ atom_off,
+                     const float* __restrict__ grad, int64_t grad_rows, const double* __restrict__ masses,
+                     const double* __restrict__ target_T, const uint64_t* __restrict__ seeds, double* __restrict__ x,
+                     double* __restrict__ mom, double* __restrict__ vel, double* __restrict__ rvel,
+                     float* __restrict__ forces, double* __restrict__ ekin_out, double* __restrict__ temp_out,
+                     int32_t* __restrict__ status) {
+  __shared__ double red[kBlock][3];
+  const int64_t c = blockIdx.x;
+  if (status[c] != kOk) return;
+  const int64_t g0 = atom_off[c], n = atom_off[c + 1] - g0;
+  if (g0 < 0 || n < 1 || atom_off[c + 1] > grad_rows) {
+    if (threadIdx.x == 0) status[c] = kBadInput;
+    return;
+  }
+  const bool langevin = p.ensemble == kLangevin;
+  if (langevin && n == 1) {                                     // ASE divides by n - 1.0 = 0
+    if (threadIdx.x == 0) status[c] = kOneAtom;
+    return;
+  }
+  const float* gr = grad + 3 * g0;
+  const double* mc = masses + g0;
+  double* xc = x + 3 * g0;
+  double* pc = mom + 3 * g0;
+  double* vc = vel + 3 * g0;
+  double* rc = rvel + 3 * g0;
+  float* fc = forces + 3 * g0;
+  const int t = threadIdx.x;
+  const double dt = p.dt, fr = p.friction;
+  const double kT = __dmul_rn(p.kB, target_T[c]);              // units.kB * temperature_K
+  const uint64_t seed = seeds[c];
+  const uint32_t step = (uint32_t)p.evaluation;
+  // Langevin.updatevars' scalars: c1 = dt/2. - dt*dt*fr/8., c2 = dt*fr/2 - dt*dt*fr*fr/8.
+  const double c1 = __dsub_rn(__dmul_rn(dt, 0.5), __dmul_rn(__dmul_rn(__dmul_rn(dt, dt), fr), 0.125));
+  const double c2 = __dsub_rn(__dmul_rn(__dmul_rn(dt, fr), 0.5),
+                              __dmul_rn(__dmul_rn(__dmul_rn(__dmul_rn(dt, dt), fr), fr), 0.125));
+  double tot[3];
+  double M = 0.0;                                               // Andersen: masses.sum()
+  if (!langevin) {
+    double s = 0.0;
+    for (int64_t i = t; i < n; i += kBlock) s = __dadd_rn(s, mc[i]);
+    block_sum3(red, s, 0.0, 0.0, tot);
+    M = tot[0];
+  }
+
+  // ---- 1-3. forces, the second half of the previous step, p . (p / m)
+  double kin = 0.0;
+  if (p.evaluation == 0) {
+    for (int64_t i = t; i < n; i += kBlock) {
+      const double m = mc[i];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        fc[3 * i + k] = __fmul_rn(gr[3 * i + k], p.force_multiplier);
+        const double pd = pc[3 * i + k];
+        kin = __dadd_rn(kin, __dmul_rn(pd, __ddiv_rn(pd, m)));
+      }
+    }
+  } else if (langevin) {
+    for (int64_t i = t; i < n; i += kBlock) {
+      const double m = mc[i];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const float f = __fmul_rn(gr[3 * i + k], p.force_multiplier);
+        fc[3 * i + k] = f;
+        double v = vc[3 * i + k];
+        v = __dadd_rn(v, __dadd_rn(__dsub_rn(__ddiv_rn(__dmul_rn(c1, (double)f), m), __dmul_rn(c2, v)), rc[3 * i + k]));
+        const double pd = __dmul_rn(v, m);                      // set_momenta(v * masses)
+        pc[3 * i + k] = pd;
+        kin = __dadd_rn(kin, __dmul_rn(pd, __ddiv_rn(pd, m)));
+      }
+    }
+  } else {
+    double s[3] = {0.0, 0.0, 0.0};
+    for (int64_t i = t; i < n; i += kBlock) {
+      const double m = mc[i];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const float f = __fmul_rn(gr[3 * i + k], p.force_multiplier);
+        fc[3 * i + k] = f;
+        const double v = __dadd_rn(vc[3 * i + k], __dmul_rn(__ddiv_rn(__dmul_rn(0.5, (double)f), m), dt));
+        vc[3 * i + k] = v;
+        s[k] = __dadd_rn(s[k], __dmul_rn(m, v));
+      }
+    }
+    block_sum3(red, s[0], s[1], s[2], tot);
+    const double vcm[3] = {__ddiv_rn(tot[0], M), __ddiv_rn(tot[1], M), __ddiv_rn(tot[2], M)};
+    for (int64_t i = t; i < n; i += kBlock) {
+      const double m = mc[i];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const double pd = __dmul_rn(__dsub_rn(vc[3 * i + k], vcm[k]), m);
+        pc[3 * i + k] = pd;
+        kin = __dadd_rn(kin, __dmul_rn(pd, __ddiv_rn(pd, m)));
+      }
+    }
+  }
+  block_sum3(red, kin, 0.0, 0.0, tot);
+  const double ekin = __dmul_rn(0.5, tot[0]);
+  const double T = __ddiv_rn(__dmul_rn(2.0, ekin), __dmul_rn((double)(3 * n), p.kB));
+  if (t == 0) {
+    ekin_out[c] = ekin;
+    temp_out[c] = T;
+  }
+  if (p.evaluation == p.steps) return;
+
+  // ---- 4. the first half of the next step
+  const double nd = (double)n;
+  if (langevin) {
+    // draws, rnd_pos = c5 eta and rnd_vel = c3 xi - c4 eta; rnd_pos waits in the velocity workspace for the sums
+    double sp[3] = {0.0, 0.0, 0.0}, sv[3] = {0.0, 0.0, 0.0};
+    for (int64_t i = t; i < n; i += kBlock) {
+      const double m = mc[i];
+      const double sigma = __dsqrt_rn(__ddiv_rn(__dmul_rn(__dmul_rn(2.0, kT), fr), m));
+      const double c3 = __dsub_rn(__dmul_rn(__dmul_rn(p.sqrt_dt, sigma), 0.5),
+                                  __dmul_rn(__dmul_rn(__dmul_rn(p.dt_1_5, fr), sigma), 0.125));
+      const double c5 = __ddiv_rn(__dmul_rn(p.dt_1_5, sigma), p.two_sqrt3);
+      const double c4 = __dmul_rn(__dmul_rn(fr, 0.5), c5);
+      double z[6], u0, u1;
+#pragma unroll
+      for (int j = 0; j < 3; ++j) {
+        block_uniforms(seed, (uint32_t)i, step, (uint32_t)j, kTagLangevin, u0, u1);
+        box_muller(u0, u1, z[2 * j], z[2 * j + 1]);
+      }
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const double rp = __dmul_rn(c5, z[3 + k]);
+        const double rv = __dsub_rn(__dmul_rn(c3, z[k]), __dmul_rn(c4, z[3 + k]));
+        vc[3 * i + k] = rp;
+        rc[3 * i + k] = rv;
+        sp[k] = __dadd_rn(sp[k], rp);
+        sv[k] = __dadd_rn(sv[k], __dmul_rn(rv, m));
+      }
+    }
+    double spt[3];
+    block_sum3(red, sp[0], sp[1], sp[2], spt);
+    block_sum3(red, sv[0], sv[1], sv[2], tot);
+    const double factor = __dsqrt_rn(__ddiv_rn(nd, __dsub_rn(nd, 1.0)));
+    const double mp[3] = {__ddiv_rn(spt[0], nd), __ddiv_rn(spt[1], nd), __ddiv_rn(spt[2], nd)};
+    for (int64_t i = t; i < n; i += kBlock) {
+      const double m = mc[i];
+      const double mn = __dmul_rn(m, nd);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const double rp = __dmul_rn(__dsub_rn(vc[3 * i + k], mp[k]), factor);
+        const double rv = __dmul_rn(__dsub_rn(rc[3 * i + k], __ddiv_rn(tot[k], mn)), factor);
+        const double f = fc[3 * i + k];
+        double v = __ddiv_rn(pc[3 * i + k], m);                 // get_velocities()
+        v = __dadd_rn(v, __dadd_rn(__dsub_rn(__ddiv_rn(__dmul_rn(c1, f), m), __dmul_rn(c2, v)), rv));
+        const double x0 = xc[3 * i + k];
+        const double xn = __dadd_rn(__dadd_rn(x0, __dmul_rn(dt, v)), rp);
+        xc[3 * i + k] = xn;
+        vc[3 * i + k] = __ddiv_rn(__dsub_rn(__dsub_rn(xn, x0), rp), dt);
+        rc[3 * i + k] = rv;
+      }
+    }
+  } else {
+    // the centre-of-mass kick: every thread draws the crystal's three components itself
+    const double wcom = __dsqrt_rn(__ddiv_rn(kT, M));
+    double u[6];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) block_uniforms(seed, kComAtom, step, (uint32_t)j, kTagAndersen, u[2 * j], u[2 * j + 1]);
+    const double kick[3] = {boltzmann_random(wcom, u[0], u[3]), boltzmann_random(wcom, u[1], u[4]),
+                            boltzmann_random(wcom, u[2], u[5])};
+    double sx[3] = {0.0, 0.0, 0.0}, sv[3] = {0.0, 0.0, 0.0};
+    for (int64_t i = t; i < n; i += kBlock) {
+      const double m = mc[i];
+      const double w = __dsqrt_rn(__ddiv_rn(kT, m));
+      double a[10];
+#pragma unroll
+      for (int j = 0; j < 5; ++j) block_uniforms(seed, (uint32_t)i, step, (uint32_t)j, kTagAndersen, a[2 * j], a[2 * j + 1]);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        double v = __dadd_rn(__ddiv_rn(pc[3 * i + k], m), kick[k]);
+        v = __dadd_rn(v, __dmul_rn(__ddiv_rn(__dmul_rn(0.5, (double)fc[3 * i + k]), m), dt));
+        if (a[6 + k] <= p.andersen_prob) v = boltzmann_random(w, a[k], a[3 + k]);
+        vc[3 * i + k] = v;
+        sx[k] = __dadd_rn(sx[k], __dmul_rn(m, xc[3 * i + k]));
+        sv[k] = __dadd_rn(sv[k], __dmul_rn(m, v));
+      }
+    }
+    double sxt[3];
+    block_sum3(red, sx[0], sx[1], sx[2], sxt);
+    block_sum3(red, sv[0], sv[1], sv[2], tot);
+    const double old_com[3] = {__ddiv_rn(sxt[0], M), __ddiv_rn(sxt[1], M), __ddiv_rn(sxt[2], M)};
+    const double vcm[3] = {__ddiv_rn(tot[0], M), __ddiv_rn(tot[1], M), __ddiv_rn(tot[2], M)};
+    // x_new = x + v dt waits in the velocity workspace for the sum of m x_new
+    double sn[3] = {0.0, 0.0, 0.0};
+    for (int64_t i = t; i < n; i += kBlock) {
+      const double m = mc[i];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const double xn = __dadd_rn(xc[3 * i + k], __dmul_rn(__dsub_rn(vc[3 * i + k], vcm[k]), dt));
+        vc[3 * i + k] = xn;
+        sn[k] = __dadd_rn(sn[k], __dmul_rn(m, xn));
+      }
+    }
+    block_sum3(red, sn[0], sn[1], sn[2], tot);
+    const double shift[3] = {__dsub_rn(__ddiv_rn(tot[0], M), old_com[0]), __dsub_rn(__ddiv_rn(tot[1], M), old_com[1]),
+                             __dsub_rn(__ddiv_rn(tot[2], M), old_com[2])};
+    for (int64_t i = t; i < n; i += kBlock) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const double x0 = xc[3 * i + k];
+        const double xn = __dsub_rn(vc[3 * i + k], shift[k]);  // set_center_of_mass(old_com)
+        xc[3 * i + k] = xn;
+        vc[3 * i + k] = __ddiv_rn(__dsub_rn(xn, x0), dt);
+      }
+    }
+  }
+}
+
+// the stream itself, for tests: item (a, j), a in [0, atoms), is block j of atom index atom0 + a (mod 2^32)
+__global__ void __launch_bounds__(kBlock)
+md_noise_kernel(uint64_t seed, uint32_t step, uint32_t tag, uint32_t atom0, int64_t items, int32_t blocks,
+                uint32_t* __restrict__ words, double* __restrict__ uniforms, double* __restrict__ normals) {
+  const int64_t q = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  if (q >= items) return;
+  const uint32_t atom = atom0 + (uint32_t)(q / blocks), block = (uint32_t)(q % blocks);
+  const Words4 w = noise_block(seed, atom, step, block, tag);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) words[4 * q + k] = w.w[k];
+  const double u0 = unit_uniform(w.w[0], w.w[1]), u1 = unit_uniform(w.w[2], w.w[3]);
+  uniforms[2 * q] = u0;
+  uniforms[2 * q + 1] = u1;
+  box_muller(u0, u1, normals[2 * q], normals[2 * q + 1]);
+}
+
 }  // namespace md
 }  // namespace alignn
 
@@ -165,6 +408,41 @@ int alignn_b200_md_step(const alignn_b200_md_params* params, const int64_t* atom
   md_step_kernel<<<(unsigned)num_crystals, kBlock, 0, (cudaStream_t)stream>>>(
       p, atom_offsets, grad, grad_rows, masses, target_temperature, positions, momenta, forces, kinetic_energy,
       temperature, status);
+  return alignn::check_launch();
+}
+
+int alignn_b200_md_thermostat_step(const alignn_b200_md_thermostat_params* params, const int64_t* atom_offsets,
+                                   int64_t num_crystals, const float* grad, int64_t grad_rows, const double* masses,
+                                   const double* target_temperature, const uint64_t* seeds, double* positions,
+                                   double* momenta, double* velocities, double* rnd_vel, float* forces,
+                                   double* kinetic_energy, double* temperature, int32_t* status, alignn_stream_t stream) {
+  using namespace alignn::md;
+  if (!params || num_crystals < 1 || num_crystals > INT32_MAX || grad_rows < 0) return ALIGNN_ERR_BAD_ARG;
+  const alignn_b200_md_thermostat_params p = *params;
+  const auto positive = [](double v) { return isfinite(v) && v > 0.0; };
+  if (p.steps < 1 || p.evaluation < 0 || p.evaluation > p.steps || !positive(p.dt) || !positive(p.kB) ||
+      !isfinite(p.force_multiplier) || !isfinite(p.friction) || !(p.friction >= 0.0) ||
+      !(p.andersen_prob >= 0.0 && p.andersen_prob <= 1.0) || !positive(p.sqrt_dt) || !positive(p.dt_1_5) ||
+      !positive(p.two_sqrt3) || (p.ensemble != kLangevin && p.ensemble != kAndersen))
+    return ALIGNN_ERR_BAD_ARG;
+  if (!atom_offsets || !grad || !masses || !target_temperature || !seeds || !positions || !momenta || !velocities ||
+      !rnd_vel || !forces || !kinetic_energy || !temperature || !status)
+    return ALIGNN_ERR_BAD_ARG;
+  md_thermostat_kernel<<<(unsigned)num_crystals, kBlock, 0, (cudaStream_t)stream>>>(
+      p, atom_offsets, grad, grad_rows, masses, target_temperature, seeds, positions, momenta, velocities, rnd_vel,
+      forces, kinetic_energy, temperature, status);
+  return alignn::check_launch();
+}
+
+int alignn_b200_md_noise(uint64_t seed, int32_t step, int32_t tag, uint32_t atom0, int64_t atoms, int32_t blocks,
+                         uint32_t* words, double* uniforms, double* normals, alignn_stream_t stream) {
+  using namespace alignn::md;
+  if (step < 0 || atoms < 0 || atoms > INT32_MAX || blocks < 1 || blocks > 64 || !words || !uniforms || !normals)
+    return ALIGNN_ERR_BAD_ARG;
+  const int64_t items = atoms * blocks;
+  if (items == 0) return ALIGNN_OK;
+  md_noise_kernel<<<(unsigned)((items + kBlock - 1) / kBlock), kBlock, 0, (cudaStream_t)stream>>>(
+      seed, (uint32_t)step, (uint32_t)tag, atom0, items, blocks, words, uniforms, normals);
   return alignn::check_launch();
 }
 

@@ -1,4 +1,5 @@
-"""Molecular dynamics for a batch of crystals with ALIGNN-FF on the GPU: NVE velocity Verlet and NVT Berendsen.
+"""Molecular dynamics for a batch of crystals with ALIGNN-FF on the GPU: NVE velocity Verlet, NVT Berendsen, NVT Langevin
+and NVT Andersen.
 
 The reference runs MD one structure at a time: `ForceField.run_nve_velocity_verlet` and `run_nvt_berendsen`
 (alignn/ff/ff.py:419-443, 510-543) drive ASE's integrators, and every step its calculator (alignn/ff/calculators.py:
@@ -6,7 +7,10 @@ The reference runs MD one structure at a time: `ForceField.run_nve_velocity_verl
 integrate.  Here all crystals advance in lockstep: per evaluation one device graph build
 (`neighbors.crystal_graphs_device`), one model call and one integrator launch (`ops.md_step`, csrc/md_device.cu) that
 also writes each crystal's kinetic energy and temperature.  Each crystal follows the trajectory it would follow run
-alone; `oracle/md_oracle.py` is the specification (ASE 3.22.1 semantics, float64 state).
+alone; `oracle/md_oracle.py` is the specification (ASE 3.22.1 semantics, float64 state).  The stochastic thermostats
+(`ForceField.run_nvt_langevin` / `run_nvt_andersen`, alignn/ff/ff.py:444-508) launch `ops.md_thermostat_step` instead
+and draw their noise from a counter-based stream keyed by each crystal's seed (csrc/md_noise.cuh) rather than numpy's
+global RNG; `oracle/md_thermostat_oracle.py` is their specification.
 """
 from __future__ import annotations
 
@@ -25,7 +29,10 @@ _e, _amu, _k = 1.6021766208e-19, 1.660539040e-27, 1.38064852e-23
 FS = 1e-15 * (1e10 * math.sqrt(_e / _amu))     # 0.09822694788464063
 KB = _k / _e                                   # 8.617330337217213e-05
 
-ENSEMBLES = {"nve_velocity_verlet": ops.MD_NVE, "nvt_berendsen": ops.MD_NVT_BERENDSEN}
+ENSEMBLES = {"nve_velocity_verlet": ops.MD_NVE, "nvt_berendsen": ops.MD_NVT_BERENDSEN,
+             "nvt_langevin": ops.MD_NVT_LANGEVIN, "nvt_andersen": ops.MD_NVT_ANDERSEN}
+STOCHASTIC = (ops.MD_NVT_LANGEVIN, ops.MD_NVT_ANDERSEN)
+LANGEVIN_FRICTION = 1e-4      # ForceField.run_nvt_langevin's default friction, in 1 / ASE time unit
 
 
 class MDResult(NamedTuple):
@@ -66,20 +73,39 @@ def _host_array(x, name: str, shape) -> np.ndarray:
     return a
 
 
+def _seeds(seed, B: int) -> np.ndarray:
+    """[B] uint64: seed + b for one int in [0, 2^63), or B ints in [0, 2^64)."""
+    def ok(v, hi):
+        return not isinstance(v, (bool, np.bool_)) and isinstance(v, numbers.Integral) and 0 <= int(v) < hi
+    if seed is None:
+        raise ValueError("nvt_langevin and nvt_andersen need a seed: an int in [0, 2^63) or one int per crystal")
+    if np.ndim(seed) == 0:
+        if not ok(seed, 2 ** 63):
+            raise ValueError(f"seed must be an int in [0, 2^63) or {B} ints in [0, 2^64), got {seed!r}")
+        return np.array([int(seed) + b for b in range(B)], dtype=np.uint64)
+    s = list(seed)
+    if len(s) != B or not all(ok(v, 2 ** 64) for v in s):
+        raise ValueError(f"seed must be an int in [0, 2^63) or {B} ints in [0, 2^64), got {seed!r}")
+    return np.array([int(v) for v in s], dtype=np.uint64)
+
+
 def run_md(model, structures, atom_features: torch.Tensor, masses, *, ensemble: str = "nve_velocity_verlet",
            steps: int = 1000, timestep: float = 0.01, temperature_K=300.0, taut: Optional[float] = None, momenta=None,
            trajectory_interval: Optional[int] = None, neighbor_strategy: str = "k-nearest", cutoff: float = 8.0,
-           max_neighbors: int = 12, cutoff_extra: float = 3.5, force_multiplier: float = 1.0) -> MDResult:
+           max_neighbors: int = 12, cutoff_extra: float = 3.5, force_multiplier: float = 1.0,
+           friction: Optional[float] = None, andersen_prob: float = 0.1, seed=None) -> MDResult:
     """Run `steps` steps of molecular dynamics on a batch of crystals, the cells fixed: a batched
     `ForceField.run_nve_velocity_verlet(steps=steps)` (ensemble="nve_velocity_verlet", ASE's VelocityVerlet) or
     `run_nvt_berendsen(temperature_K=..., taut=..., steps=steps)` (ensemble="nvt_berendsen", ASE's NVTBerendsen with
-    fixcm=True).  Returns an `MDResult`.
+    fixcm=True), `run_nvt_langevin(temperature_K=..., friction=...)` (ensemble="nvt_langevin", ASE's Langevin with
+    fixcm=True) or `run_nvt_andersen(temperature_K=..., andersen_prob=...)` (ensemble="nvt_andersen", ASE's Andersen
+    with fixcm=True).  Returns an `MDResult`.
 
     model: an `ALIGNNAtomWise` in eval mode on a CUDA device, with calculate_gradient=True and output_features=1.
     structures: sequence of (lattice [3,3], cart_coords [n,3]), as for `neighbors.crystal_graphs_device`;
     atom_features: [sum n, F] on the model's device, in the same atom order; masses: [sum n] in amu, all > 0.
     timestep in fs (the reference's default 0.01); taut in fs, default 100 * timestep (taken as 100 times the
-    converted timestep, as ForceField does), and not below timestep; temperature_K: the Berendsen target in K, one
+    converted timestep, as ForceField does), and not below timestep; temperature_K: the thermostat's target in K, one
     value or one per crystal (unused by NVE).  momenta: [sum n, 3] in ASE units (amu * A / ASE time), default zero --
     `maxwell_boltzmann_momenta` draws them as `set_momentum_maxwell_boltzmann` does.  Graph options are those of
     `crystal_graphs_device`; force_multiplier as for `relax_structures`.
@@ -87,7 +113,13 @@ def run_md(model, structures, atom_features: torch.Tensor, masses, *, ensemble: 
     MolecularDynamics.irun: evaluate, then `steps` times step and evaluate -- steps + 1 evaluations, and energy, kinetic
     energy and temperature are logged after each.  trajectory_interval=k keeps the positions of evaluations 0, k, 2k,
     ....  Positions are not wrapped into the cell.  A crystal whose positions stop being finite raises RuntimeError
-    naming it and the step."""
+    naming it and the step.
+
+    Langevin and Andersen: friction in 1/fs, finite and >= 0, None for ForceField's 1e-4 in ASE units (exactly);
+    andersen_prob in [0, 1] per component and step (ForceField's 0.1).  seed is required: an int in [0, 2^63), crystal
+    b drawing the stream of seed + b, or B ints in [0, 2^64), one per crystal.  Nothing is drawn from global state: a
+    crystal's trajectory is a function of the arguments and of its own seed, so run alone with that seed it repeats
+    its trajectory in the batch bit for bit.  Langevin (fixcm) divides by n - 1 and rejects one-atom crystals."""
     _check_model("run_md", model)
     if ensemble not in ENSEMBLES:
         raise ValueError(f"ensemble must be one of {sorted(ENSEMBLES)}, got {ensemble!r}")
@@ -111,11 +143,12 @@ def run_md(model, structures, atom_features: torch.Tensor, masses, *, ensemble: 
     dt = float(timestep) * FS
     kind = ENSEMBLES[ensemble]
     T0, taut_ase = None, 0.0
-    if kind == ops.MD_NVT_BERENDSEN:
+    if kind != ops.MD_NVE:
         t = [temperature_K] * B if np.ndim(temperature_K) == 0 else list(temperature_K)
         if len(t) != B or not all(_real(v) and v > 0 for v in t):
             raise ValueError(f"temperature_K must be a finite number > 0 or {B} of them, got {temperature_K!r}")
         T0 = torch.tensor([float(v) for v in t], dtype=torch.float64, device=dev)
+    if kind == ops.MD_NVT_BERENDSEN:
         if taut is None:
             taut_ase = 100 * dt                         # ForceField: taut = 100 * self.timestep, in ASE units
         elif not _real(taut):
@@ -124,6 +157,22 @@ def run_md(model, structures, atom_features: torch.Tensor, masses, *, ensemble: 
             taut_ase = float(taut) * FS
         if not taut_ase >= dt:
             raise ValueError(f"taut must not be smaller than timestep, got taut={taut!r} and timestep={timestep!r}")
+    if kind in STOCHASTIC:
+        seeds = _seeds(seed, B)
+        if friction is None:
+            fr_ase = LANGEVIN_FRICTION
+        elif not _real(friction) or not friction >= 0:
+            raise ValueError(f"friction must be a finite number >= 0 (1/fs) or None, got {friction!r}")
+        else:
+            fr_ase = float(friction) / FS
+        if not _real(andersen_prob) or not 0.0 <= andersen_prob <= 1.0:
+            raise ValueError(f"andersen_prob must be a number in [0, 1], got {andersen_prob!r}")
+        if kind == ops.MD_NVT_LANGEVIN and min(sizes) < 2:
+            raise ValueError(f"nvt_langevin needs at least 2 atoms per crystal (fixcm divides by n - 1); crystal "
+                             f"{sizes.index(min(sizes))} has 1")
+        seeds_d = torch.from_numpy(seeds.view(np.int64)).to(dev)
+        vel = torch.zeros(N, 3, device=dev, dtype=torch.float64)
+        rnd_vel = torch.zeros(N, 3, device=dev, dtype=torch.float64)
 
     pos = torch.from_numpy(np.ascontiguousarray(np.concatenate(Xs))).to(dev)
     mom = torch.from_numpy(np.ascontiguousarray(p0)).to(dev)
@@ -150,13 +199,22 @@ def run_md(model, structures, atom_features: torch.Tensor, masses, *, ensemble: 
         if trajectory_interval is not None and e % trajectory_interval == 0:
             traj.append(pos.clone())                                         # the positions of evaluation e
         with ops._span("md_step", 0):
-            ops.md_step(grad, aoff_d, m_d, T0, pos, mom, forces, ekin[e], temp[e], status, evaluation=e, steps=int(steps),
-                        dt=dt, kB=KB, ensemble=kind, taut=taut_ase, force_multiplier=float(force_multiplier))
+            if kind in STOCHASTIC:
+                ops.md_thermostat_step(grad, aoff_d, m_d, T0, seeds_d, pos, mom, vel, rnd_vel, forces, ekin[e], temp[e],
+                                       status, evaluation=e, steps=int(steps), dt=dt, kB=KB, ensemble=kind,
+                                       friction=fr_ase, andersen_prob=float(andersen_prob),
+                                       force_multiplier=float(force_multiplier))
+            else:
+                ops.md_step(grad, aoff_d, m_d, T0, pos, mom, forces, ekin[e], temp[e], status, evaluation=e,
+                            steps=int(steps), dt=dt, kB=KB, ensemble=kind, taut=taut_ase,
+                            force_multiplier=float(force_multiplier))
         with ops._span("md_readback", 0):
             # one copy: the statuses and, unless this was the last evaluation, the positions of the next one
             back = torch.cat([status.to(torch.float64)] + ([pos.reshape(-1)] if e < steps else [])).cpu().numpy()
         if (back[:B] == ops.MD_BAD_INPUT).any():
             raise RuntimeError("alignn_b200_md_step: the model's forces do not match the crystals' atom counts")
+        if (back[:B] != 0).any():
+            raise RuntimeError(f"run_md: the MD kernel reported statuses {back[:B].astype(int).tolist()}")
         if e == steps:
             break
         new_pos = back[B:].reshape(-1, 3)

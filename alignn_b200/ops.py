@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 import functools
+import math
 import weakref
 from typing import Optional, Tuple
 
@@ -531,6 +532,89 @@ def md_step(grad: torch.Tensor, atom_offsets: torch.Tensor, masses: torch.Tensor
                                        positions.data_ptr(), momenta.data_ptr(), forces.data_ptr(),
                                        kinetic_energy.data_ptr(), temperature.data_ptr(), status.data_ptr(),
                                        stream_ptr()), "alignn_b200_md_step")
+
+
+MD_NVT_LANGEVIN, MD_NVT_ANDERSEN = 2, 3   # alignn_b200_md_thermostat_params.ensemble, also the noise stream's tags
+MD_ONE_ATOM = 6                           # status of a one-atom crystal under Langevin (ASE divides by n - 1)
+
+
+def _md_operands(what, want, device):
+    for t, dt_ in want:
+        if not t.is_cuda or t.device != device:
+            raise RuntimeError(f"{what} needs all operands on one CUDA device; got {t.device} and {device}")
+        ok = t.dtype in dt_ if isinstance(dt_, tuple) else t.dtype == dt_
+        if not ok or not t.is_contiguous():
+            raise RuntimeError(f"{what}: expected a contiguous {dt_} tensor, got {t.dtype}")
+
+
+@_on_tensor_device
+def md_thermostat_step(grad: torch.Tensor, atom_offsets: torch.Tensor, masses: torch.Tensor,
+                       target_temperature: torch.Tensor, seeds: torch.Tensor, positions: torch.Tensor,
+                       momenta: torch.Tensor, velocities: torch.Tensor, rnd_vel: torch.Tensor, forces: torch.Tensor,
+                       kinetic_energy: torch.Tensor, temperature: torch.Tensor, status: torch.Tensor, *,
+                       evaluation: int, steps: int, dt: float, kB: float, ensemble: int, friction: float = 0.0,
+                       andersen_prob: float = 0.0, force_multiplier: float = 1.0) -> None:
+    """Evaluation `evaluation` of an MD run of `steps` steps under ASE 3.22.1's `Langevin` (ensemble=MD_NVT_LANGEVIN)
+    or `Andersen` (MD_NVT_ANDERSEN), fixcm=True, for every crystal, in place, one launch (csrc/md_device.cu,
+    alignn_b200_md_thermostat_step): the forces, the second half of the previous step (evaluation >= 1), ekin and T of
+    this evaluation, and unless evaluation == steps the first half of the next step with the noise of crystal c's seed.
+
+    As `md_step`, plus: target_temperature [B] float64 (K); seeds [B] int64 or uint64 (the 64 bits of each crystal's
+    seed); velocities / rnd_vel [N,3] float64, workspaces the launches of one run pass on (not read at evaluation 0);
+    status MD_ONE_ATOM for a one-atom crystal under Langevin.  dt in ASE time units, friction in 1 / ASE time unit,
+    andersen_prob per component and step.  sqrt(dt), dt ** 1.5 and 2 sqrt(3) are formed here, on the host, as numpy
+    forms them.  Enqueue only: the statuses are the caller's to read back."""
+    lib = _lib.load()
+    _md_operands("md_thermostat_step",
+                 [(grad, torch.float32), (atom_offsets, torch.int64), (masses, torch.float64),
+                  (target_temperature, torch.float64), (seeds, (torch.int64, torch.uint64)), (positions, torch.float64),
+                  (momenta, torch.float64), (velocities, torch.float64), (rnd_vel, torch.float64),
+                  (forces, torch.float32), (kinetic_energy, torch.float64), (temperature, torch.float64),
+                  (status, torch.int32)], grad.device)
+    B = atom_offsets.numel() - 1
+    N = positions.numel() // 3
+    if (B < 1 or positions.numel() != 3 * N or any(t.numel() != 3 * N for t in (momenta, velocities, rnd_vel, forces))
+            or masses.numel() != N or any(t.numel() != B for t in (kinetic_energy, temperature, status,
+                                                                     target_temperature, seeds))
+            or grad.dim() != 2 or grad.shape[1] != 3 or grad.shape[0] > N):
+        raise ValueError("md_thermostat_step: inconsistent operand shapes")
+    if isinstance(steps, bool) or int(steps) != steps or not 1 <= int(steps) <= FIRE_MAX_STEPS:
+        raise ValueError(f"md_thermostat_step: steps must be an integer in [1, {FIRE_MAX_STEPS}], got {steps!r}")
+    if isinstance(evaluation, bool) or int(evaluation) != evaluation or not 0 <= int(evaluation) <= int(steps):
+        raise ValueError(f"md_thermostat_step: evaluation must be an integer in [0, steps], got {evaluation!r}")
+    dt = float(dt)
+    ok = math.isfinite(dt) and dt > 0                  # anything else the library rejects
+    root_dt = math.sqrt(dt) if ok else float("nan")    # np.sqrt(dt): both correctly rounded
+    dt_1_5 = dt ** 1.5 if ok else float("nan")         # Langevin.updatevars' dt**1.5, a Python float power
+    p = _lib.MdThermostatParams(dt, float(kB), float(friction), float(andersen_prob), root_dt, dt_1_5,
+                                2 * math.sqrt(3), int(evaluation), int(steps), int(ensemble), float(force_multiplier))
+    _lib.check(lib.alignn_b200_md_thermostat_step(
+        C.byref(p), atom_offsets.data_ptr(), B, grad.data_ptr(), grad.shape[0], masses.data_ptr(),
+        target_temperature.data_ptr(), seeds.data_ptr(), positions.data_ptr(), momenta.data_ptr(), velocities.data_ptr(),
+        rnd_vel.data_ptr(), forces.data_ptr(), kinetic_energy.data_ptr(), temperature.data_ptr(), status.data_ptr(),
+        stream_ptr()), "alignn_b200_md_thermostat_step")
+
+
+def md_noise(seed: int, step: int, count: int, *, tag: int = MD_NVT_LANGEVIN, atom0: int = 0, blocks: int = 1,
+             device=None):
+    """The thermostats' noise stream (csrc/md_noise.cuh) on the device, for tests: Philox block j of atom index
+    atom0 + a (mod 2^32), a in [0, count), j in [0, blocks), at (seed, step, tag).  Returns (words [count, blocks, 4]
+    int64 holding the uint32 words, uniforms [count, blocks, 2] float64, normals [count, blocks, 2] float64)."""
+    lib = _lib.load()
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    if dev.type != "cuda":
+        raise RuntimeError(f"md_noise needs a CUDA device, got {dev}")
+    if not 0 <= int(seed) < 2 ** 64 or not 0 <= int(atom0) < 2 ** 32:
+        raise ValueError("md_noise: seed must be in [0, 2^64) and atom0 in [0, 2^32)")
+    count, blocks = int(count), int(blocks)
+    words = torch.empty(count, blocks, 4, dtype=torch.int32, device=dev)
+    uniforms = torch.empty(count, blocks, 2, dtype=torch.float64, device=dev)
+    normals = torch.empty(count, blocks, 2, dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.alignn_b200_md_noise(int(seed), int(step), int(tag), int(atom0), count, blocks, words.data_ptr(),
+                                            uniforms.data_ptr(), normals.data_ptr(), stream_ptr()),
+                   "alignn_b200_md_noise")
+    return words.to(torch.int64) & 0xFFFFFFFF, uniforms, normals
 
 
 PHONON_BAD_INPUT = 3              # status of a crystal whose slices do not lie inside the buffers

@@ -682,6 +682,67 @@ int alignn_b200_md_step(const alignn_b200_md_params* params, const int64_t* atom
                         double* positions, double* momenta, float* forces, double* kinetic_energy, double* temperature,
                         int32_t* status, alignn_stream_t stream);
 
+/* Stochastic thermostats (csrc/md_device.cu, csrc/md_noise.cuh): ASE 3.22.1's `Langevin` and `Andersen` (fixcm=True) --
+ * what `ForceField.run_nvt_langevin` / `run_nvt_andersen` (alignn/ff/ff.py:444-508) run one crystal at a time -- with
+ * the run loop of `MolecularDynamics.irun`, for a batch of crystals advanced in lockstep.  Their noise is not numpy's
+ * global RNG but a counter-based Philox4x32-10 stream keyed by each crystal's 64-bit seed, whose layout
+ * csrc/md_noise.cuh fixes: a crystal's trajectory depends on its own seed only, bitwise, in any batch. */
+typedef struct {
+  double dt;                /* time step in ASE time units                                         */
+  double kB;                /* Boltzmann constant, eV/K                                            */
+  double friction;          /* Langevin friction, 1 / ASE time unit, finite and >= 0               */
+  double andersen_prob;     /* Andersen reassignment probability per component and step, [0, 1]   */
+  double sqrt_dt;           /* np.sqrt(dt), formed on the host                                     */
+  double dt_1_5;            /* dt ** 1.5, formed on the host (libm pow)                            */
+  double two_sqrt3;         /* 2 * np.sqrt(3)                                                      */
+  int32_t evaluation;       /* e in [0, steps]: the evaluation whose forces grad holds             */
+  int32_t steps;            /* steps >= 1                                                          */
+  int32_t ensemble;         /* 2 = NVT Langevin, 3 = NVT Andersen                                   */
+  float force_multiplier;   /* F = fp32(grad * force_multiplier)                                   */
+} alignn_b200_md_thermostat_params;
+
+/* One launch per evaluation e = 0, 1, ..., steps, one CTA per crystal, as alignn_b200_md_step.  Per crystal c with
+ * status 0 (n atoms, masses m, kT = kB * target_temperature[c], key seeds[c]):
+ *   F = fp32(grad * force_multiplier), written to forces.  If e >= 1, the second half of the previous step from the
+ *   velocities v (and for Langevin rnd_vel) that the previous launch left in the workspaces: Langevin
+ *   v += c1 F/m - c2 v + rnd_vel; Andersen v += 0.5 F/m dt, v -= (m.v)/M (M = sum m); then p = v m.
+ *   kinetic_energy[c] and temperature[c] as alignn_b200_md_step (the caller passes row e of its logs).
+ *   If e < steps, the first half of the next step with the noise of step index e:
+ *     Langevin (updatevars: sigma = sqrt(2 kT fr/m), c1 = dt/2 - dt^2 fr/8, c2 = dt fr/2 - dt^2 fr^2/8,
+ *     c3 = sqrt(dt) sigma/2 - dt^1.5 fr sigma/8, c5 = dt^1.5 sigma/(2 sqrt 3), c4 = fr/2 c5): v = p/m; xi, eta
+ *     standard normals; rnd_pos = c5 eta, rnd_vel = c3 xi - c4 eta; rnd_pos -= sum(rnd_pos)/n,
+ *     rnd_vel -= sum(rnd_vel m)/(m n), both times sqrt(n/(n - 1)); v += c1 F/m - c2 v + rnd_vel;
+ *     x_new = x + dt v + rnd_pos; v = (x_new - x - rnd_pos)/dt.
+ *     Andersen: v = p/m + kick, kick = boltzmann_random(sqrt(kT/M)) per component, the same for every atom;
+ *     v += 0.5 F/m dt; per component, where the chance draw is <= andersen_prob, v = boltzmann_random(sqrt(kT/m));
+ *     old_com = (m.x)/M; v -= (m.v)/M; x_new = x + v dt; x_new -= (m.x_new)/M - old_com; v = (x_new - x)/dt.
+ *     boltzmann_random(w) = w cos(2 pi u) sqrt(-2 log(1 - u')) on two uniforms.
+ *   positions = x_new; velocities = v (and rnd_vel) for the next launch; momenta are written by the second half only.
+ *   Status 3 (inconsistent input): the slice does not lie inside [0, grad_rows) or is empty; status 6: a one-atom
+ *   crystal under Langevin (ASE divides by n - 1 = 0).  Either way nothing else is read or written for c.  Crystals
+ *   with a nonzero status are not touched.  Sums are in double with fixed-order block reductions; per-element updates
+ *   follow numpy's order with IEEE divisions; no float atomics.
+ *   grad [grad_rows, 3] fp32; atom_offsets [num_crystals+1] int64; masses [>= grad_rows] double (amu, > 0);
+ *   target_temperature [num_crystals] double (K); seeds [num_crystals] uint64; positions / momenta / velocities /
+ *   rnd_vel [>= grad_rows, 3] double (velocities and rnd_vel are workspaces kept between launches; their content
+ *   before evaluation 0 is not read); forces [>= grad_rows, 3] fp32; kinetic_energy / temperature [num_crystals]
+ *   double; status [num_crystals] int32.
+ * Rejected (ALIGNN_ERR_BAD_ARG, nothing enqueued): NULL params or a NULL array, num_crystals < 1, grad_rows < 0,
+ * steps < 1, evaluation outside [0, steps], dt, kB, sqrt_dt, dt_1_5 or two_sqrt3 not finite and > 0, friction not
+ * finite and >= 0, andersen_prob outside [0, 1], a non-finite force_multiplier, an unknown ensemble. */
+int alignn_b200_md_thermostat_step(const alignn_b200_md_thermostat_params* params, const int64_t* atom_offsets,
+                                   int64_t num_crystals, const float* grad, int64_t grad_rows, const double* masses,
+                                   const double* target_temperature, const uint64_t* seeds, double* positions,
+                                   double* momenta, double* velocities, double* rnd_vel, float* forces,
+                                   double* kinetic_energy, double* temperature, int32_t* status, alignn_stream_t stream);
+
+/* The thermostats' noise stream, for tests: item q = a * blocks + j (a in [0, atoms), j in [0, blocks)) is Philox block
+ * j of atom index atom0 + a (mod 2^32) at (seed, step, tag): words [atoms*blocks, 4] uint32, its two uniforms
+ * [atoms*blocks, 2] double and their Box-Muller normals [atoms*blocks, 2] double.  Rejected (ALIGNN_ERR_BAD_ARG):
+ * step < 0, atoms outside [0, INT32_MAX], blocks outside [1, 64], a NULL output. */
+int alignn_b200_md_noise(uint64_t seed, int32_t step, int32_t tag, uint32_t atom0, int64_t atoms, int32_t blocks,
+                         uint32_t* words, double* uniforms, double* normals, alignn_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Phonons (csrc/phonon_device.cu): ASE 3.22.1's finite-displacement `Phonons` (ase/phonons.py) with
  * `read(acoustic=True)` and its defaults (method='frederiksen', symmetrize=3, offset 0) and the Fourier sum of

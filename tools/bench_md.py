@@ -3,12 +3,16 @@
 
 Workload: 64 structures drawn with a seed from tests/golden/sample_structures.npz and jittered, the 4 + 4, d = 256,
 92-feature ALIGNNAtomWise of tools/bench_relax.py (seeded weights, eval mode), k-nearest graphs (8 A, 12 neighbours),
-NVT Berendsen at 300 K (taut = 100 timesteps, the reference's default) from Maxwell-Boltzmann momenta at 300 K, a 1 fs
-timestep and `--steps` steps (steps + 1 evaluations per crystal).  Masses are seeded random values in [1, 200] amu.
+`--ensemble` at 300 K from Maxwell-Boltzmann momenta at 300 K, a 1 fs timestep and `--steps` steps (steps + 1
+evaluations per crystal), with the reference's defaults: NVT Berendsen (the default) with taut = 100 timesteps, NVT
+Langevin with friction 1e-4 per ASE time unit, NVT Andersen with andersen_prob 0.1.  The stochastic ensembles draw
+crystal b's noise from the stream of seed `--seed` + b and draw their structures from the samples with two atoms or
+more (Langevin with fixcm rejects one-atom crystals).  Masses are seeded random values in [1, 200] amu.
 
   batched:     run_md -- per evaluation one device graph build, one model call and one integrator launch for the batch;
   per-crystal: for each crystal, every evaluation runs neighbors.crystal_graph on the host, .to("cuda"), the same model
-               on a one-crystal batch, and the oracle's integrator step in numpy (oracle/md_oracle.py).
+               on a one-crystal batch, and the oracle's integrator step in numpy (oracle/md_oracle.py, or
+               oracle/md_thermostat_oracle.py on the same restated noise stream).
 
 Each arm runs three times (alternating); the median wall time (ending in a synchronise) is reported.  One more batched
 run with CUDA events around its phases gives the per-evaluation split (build, model, step kernel, read-back; each span
@@ -17,7 +21,8 @@ final positions is reported, and per crystal whether its 12th-neighbour cut lies
 (`neighbors.knn_cut_is_tied`) at any structure the host arm evaluated: there rounding picks the images the k-nearest
 graph keeps, and the arms may part.  The device name, power limit and SM clock limit are read in the same run.
 
-    python tools/bench_md.py [--structures 64] [--steps 50] [--seed 0]
+    python tools/bench_md.py [--ensemble nvt_berendsen|nvt_langevin|nvt_andersen] [--structures 64] [--steps 50]
+                             [--seed 0]
 """
 import argparse
 import json
@@ -49,6 +54,7 @@ def main():
     ap.add_argument("--structures", type=int, default=64)
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--ensemble", choices=("nvt_berendsen", "nvt_langevin", "nvt_andersen"), default="nvt_berendsen")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_md.py needs a CUDA device")
@@ -57,12 +63,16 @@ def main():
     from alignn_b200 import maxwell_boltzmann_momenta, neighbors, ops, run_md
     from alignn_b200.alignn_atomwise import ALIGNNAtomWise, ALIGNNAtomWiseConfig
     from oracle import md_oracle as MO
+    from oracle import md_thermostat_oracle as TO
 
     dev = torch.device("cuda:0")
     z = np.load(os.path.join(ROOT, "tests", "golden", "sample_structures.npz"))
     off = z["atom_offsets"]
     rng = np.random.default_rng(a.seed)
-    pick = rng.choice(len(z["ids"]), a.structures, replace=False)
+    pool = np.arange(len(z["ids"]))
+    if a.ensemble != "nvt_berendsen":                          # Langevin (fixcm) rejects one-atom crystals
+        pool = pool[off[1:] - off[:-1] >= 2]
+    pick = rng.choice(pool, min(a.structures, len(pool)), replace=False)
     structs = [(z["lattices"][i], z["cart_coords"][off[i]:off[i + 1]] + rng.normal(scale=0.03, size=(off[i + 1] - off[i], 3)))
                for i in pick]
     sizes = [x.shape[0] for _, x in structs]
@@ -77,8 +87,9 @@ def main():
     timestep, T0 = 1.0, 300.0
 
     def batched():
-        r = run_md(model, structs, feats, masses, ensemble="nvt_berendsen", steps=a.steps, timestep=timestep,
-                   temperature_K=T0, momenta=p0)
+        extra = {} if a.ensemble == "nvt_berendsen" else dict(seed=a.seed)
+        r = run_md(model, structs, feats, masses, ensemble=a.ensemble, steps=a.steps, timestep=timestep,
+                   temperature_K=T0, momenta=p0, **extra)
         torch.cuda.synchronize()
         return r
 
@@ -100,8 +111,13 @@ def main():
                 res = model((g.to(dev), lg.to(dev), lat_t))
                 return float(res["out"].detach() * n), res["grad"].detach().reshape(-1, 3).cpu().numpy()
             dt = timestep * MO.fs
-            out.append(MO.run(evaluate, X, masses[sl], ensemble=MO.NVT_BERENDSEN, steps=a.steps, dt=dt,
-                              temperature_K=T0, taut=100 * dt, momenta=p0[sl]))
+            if a.ensemble == "nvt_berendsen":
+                out.append(MO.run(evaluate, X, masses[sl], ensemble=MO.NVT_BERENDSEN, steps=a.steps, dt=dt,
+                                  temperature_K=T0, taut=100 * dt, momenta=p0[sl]))
+            else:
+                out.append(TO.run(evaluate, X, masses[sl], ensemble=a.ensemble, steps=a.steps, dt=dt, temperature_K=T0,
+                                  noise=TO.PhiloxNoise(a.seed + b), friction=1e-4, andersen_prob=0.1,
+                                  momenta=p0[sl]))
         torch.cuda.synchronize()
         return out
 
@@ -130,7 +146,7 @@ def main():
     split = {k[len("md_"):]: round(summ[k]["total_ms"] / evals, 3) for k in summ if k.startswith("md_")}
     med_b, med_p = statistics.median(ms["batched"]), statistics.median(ms["per_crystal"])
     out = dict(workload=f"{len(structs)} jittered sample structures ({sum(sizes)} atoms), ALIGNNAtomWise 4+4 d=256, "
-                        f"k-nearest 8 A / 12, NVT Berendsen 300 K from Maxwell-Boltzmann 300 K, 1 fs, {a.steps} steps "
+                        f"k-nearest 8 A / 12, {a.ensemble} 300 K from Maxwell-Boltzmann 300 K, 1 fs, {a.steps} steps "
                         f"({evals} evaluations per crystal)",
                batched_ms=[round(v, 1) for v in ms["batched"]], batched_ms_median=round(med_b, 1),
                per_crystal_ms=[round(v, 1) for v in ms["per_crystal"]], per_crystal_ms_median=round(med_p, 1),
