@@ -142,10 +142,6 @@ __device__ void expm_block(const double* A, int n, double* out, ExpmScratch& w) 
   }
 }
 
-// x / 160.21766208 in fp32, correctly rounded: the double quotient of two floats rounded to float is the correctly
-// rounded float quotient (53 >= 2 * 24 + 2), and div_rn is the correctly rounded double quotient in this range
-__device__ __forceinline__ float fdiv_rn(float x, float y) { return __double2float_rn(div_rn((double)x, (double)y)); }
-
 __global__ void __launch_bounds__(kBlock)
 fire_cell_step_kernel(const alignn_b200_fire_cell_params pc, const int32_t* __restrict__ active,
                       const int64_t* __restrict__ atom_off, const int32_t* __restrict__ batch_off, int64_t B,
@@ -193,15 +189,10 @@ fire_cell_step_kernel(const alignn_b200_fire_cell_params pc, const int32_t* __re
     if (bad) {
       st[kStatus] = kCellDegenerate;
     } else {
-      // full_3x3_to_voigt_6_stress (xx, yy, zz, yz, xz, xy) * stress_wt / 160.21766208, fp32 left to right
-      const float* S = stress + 9 * blockIdx.x;
-      float sv[6] = {S[0], S[4], S[8], __fmul_rn(__fadd_rn(S[5], S[7]), 0.5f), __fmul_rn(__fadd_rn(S[2], S[6]), 0.5f),
-                     __fmul_rn(__fadd_rn(S[1], S[3]), 0.5f)};
+      float sv[6];
+      fire::calculator_stress(stress + 9 * blockIdx.x, pc.stress_wt, sv);
 #pragma unroll
-      for (int k = 0; k < 6; ++k) {
-        sv[k] = fdiv_rn(__fmul_rn(sv[k], pc.stress_wt), 160.21766208f);
-        stress_out[6 * c + k] = sv[k];
-      }
+      for (int k = 0; k < 6; ++k) stress_out[6 * c + k] = sv[k];
       // F^-1 = adj(F) / det(F)
       const double* f = F;
       const double a00 = f[4] * f[8] - f[5] * f[7], a01 = f[2] * f[7] - f[1] * f[8], a02 = f[1] * f[5] - f[2] * f[4];

@@ -19,18 +19,24 @@
 // ase/md/langevin.py, ase/md/andersen.py), which `ForceField.run_nvt_langevin` / `run_nvt_andersen`
 // (alignn/ff/ff.py:444-508) run; oracle/md_thermostat_oracle.py is its specification.  Their noise is the
 // counter-based stream of md_noise.cuh, keyed by each crystal's own seed.
+//
+// md_npt_step_kernel runs ASE 3.22.1's `NPTBerendsen` (fixcm=True; ase/md/nptberendsen.py), which
+// `ForceField.run_npt_berendsen` (alignn/ff/ff.py:545-582) runs: the Berendsen thermostat above plus a barostat that
+// rescales each crystal's cell and positions every step on the calculator's stress; oracle/md_npt_oracle.py is its
+// specification.
 #include <math.h>
 #include <stdint.h>
 
 #include "api_common.h"
 #include "alignn_b200.h"
+#include "fire_common.cuh"
 #include "md_noise.cuh"
 
 namespace alignn {
 namespace md {
 
 constexpr int kBlock = 256;
-enum { kOk = 0, kBadInput = 3, kOneAtom = 6 };
+enum { kOk = 0, kBadInput = 3, kCellDegenerate = 4, kOneAtom = 6 };
 enum { kNVE = 0, kBerendsen = 1, kLangevin = 2, kAndersen = 3 };
 
 // sum over the block of three per-thread partials, in a fixed order; every thread returns the totals
@@ -48,6 +54,15 @@ __device__ __forceinline__ void block_sum3(double (*red)[3], double a, double b,
     __syncthreads();
   }
   out[0] = red[0][0]; out[1] = red[0][1]; out[2] = red[0][2];
+}
+
+// NVTBerendsen.scale_velocities' factor sqrt(1 + (T0/T - 1) * (dt/taut)), clipped by two Python ifs (a NaN passes both)
+__device__ __forceinline__ double berendsen_scale(double T0, double T, double dt, double taut) {
+  const double tautscl = __ddiv_rn(dt, taut);
+  double s = __dsqrt_rn(__dadd_rn(1.0, __dmul_rn(__dadd_rn(__ddiv_rn(T0, T), -1.0), tautscl)));
+  if (s > 1.1) s = 1.1;
+  if (s < 0.9) s = 0.9;
+  return s;
 }
 
 __global__ void __launch_bounds__(kBlock)
@@ -102,13 +117,7 @@ md_step_kernel(const alignn_b200_md_params p, const int64_t* __restrict__ atom_o
 
   // ---- 4. the first half of the next step
   if (berendsen) {
-    if (t == 0) {                                               // NVTBerendsen.scale_velocities
-      const double tautscl = __ddiv_rn(dt, p.taut);
-      double s = __dsqrt_rn(__dadd_rn(1.0, __dmul_rn(__dadd_rn(__ddiv_rn(target_T[c], T), -1.0), tautscl)));
-      if (s > 1.1) s = 1.1;                                     // two Python ifs: a NaN passes both
-      if (s < 0.9) s = 0.9;
-      scale = s;
-    }
+    if (t == 0) scale = berendsen_scale(target_T[c], T, dt, p.taut);   // NVTBerendsen.scale_velocities
     __syncthreads();
     const double s = scale;
     double sx = 0.0, sy = 0.0, sz = 0.0;
@@ -370,6 +379,189 @@ md_thermostat_kernel(const alignn_b200_md_thermostat_params p, const int64_t* __
   }
 }
 
+// p_a p_b / m per Voigt component (xx yy zz yz xz xy) added to g: the terms of Atoms.get_stress(include_ideal_gas=True)
+__device__ __forceinline__ void add_ideal_gas_terms(const double q[3], double invm, double g[6]) {
+  g[0] = __dadd_rn(g[0], __dmul_rn(__dmul_rn(q[0], q[0]), invm));
+  g[1] = __dadd_rn(g[1], __dmul_rn(__dmul_rn(q[1], q[1]), invm));
+  g[2] = __dadd_rn(g[2], __dmul_rn(__dmul_rn(q[2], q[2]), invm));
+  g[3] = __dadd_rn(g[3], __dmul_rn(__dmul_rn(q[1], q[2]), invm));
+  g[4] = __dadd_rn(g[4], __dmul_rn(__dmul_rn(q[0], q[2]), invm));
+  g[5] = __dadd_rn(g[5], __dmul_rn(__dmul_rn(q[0], q[1]), invm));
+}
+
+// the ideal-gas-corrected stress, in place on the fp32 array as ASE does it (out_k = fp32(s_k - G_k * invvol)), and its
+// pressure -trace / 3: the trace in fp32, the division in double (numpy 1.x's scalar promotion)
+__device__ __forceinline__ double corrected_pressure(const float sv[6], const double G[6], double invvol, float out[6]) {
+#pragma unroll
+  for (int k = 0; k < 6; ++k) out[k] = __double2float_rn(__dsub_rn((double)sv[k], __dmul_rn(G[k], invvol)));
+  const float trace = __fadd_rn(__fadd_rn(out[0], out[1]), out[2]);
+  return __ddiv_rn(-(double)trace, 3.0);
+}
+
+// ASE 3.22.1's `NPTBerendsen` (fixcm=True), which `ForceField.run_npt_berendsen` (alignn/ff/ff.py:545-582) runs;
+// oracle/md_npt_oracle.py is its specification.  A step needs two evaluations: evaluation A at the rescaled structure,
+// whose forces only drive the half-kick, and the logged evaluation B.  So two launches per step, one CTA per crystal:
+//   phase 0, after logged evaluation e, in three passes over the atoms so that nothing is written before the checks:
+//     1. F = fp32(grad * force_multiplier); e >= 1: p_e = p + (0.5 dt) F (else p_e = p); sums of p_e . (p_e / m) and of
+//        the ideal-gas terms p_a p_b / m; ekin, T and the logged pressure from the calculator's Voigt stress s;
+//     2. e < steps: s_T from T (NVTBerendsen.scale_velocities) and the ideal-gas sums of s_T p_e, the barostat's
+//        pressure P and mu = 1 - (dt/taup) c / 3 (P0 - P);
+//     3. F, p = s_T p_e, x = mu x, C = mu C, and the log rows written.
+//   phase 1, after evaluation A of step e + 1: p += (0.5 dt) F_A, p -= sum_i p_i / n, x += (dt p) / m -- the same
+//   operations as md_step_kernel's Berendsen branch, so with mu = 1 (no barostat) the trajectory is its trajectory.
+// The cell's volume V = |det C| (cofactor expansion) and mu must be finite and > 0: otherwise status 4 and nothing of
+// the crystal is written in phase 0.  ASE would carry on; a run with a collapsed or inverted cell means nothing.
+__global__ void __launch_bounds__(kBlock)
+md_npt_step_kernel(const alignn_b200_md_npt_params p, const int64_t* __restrict__ atom_off,
+                   const float* __restrict__ grad, int64_t grad_rows, const float* __restrict__ stress,
+                   const double* __restrict__ masses, const double* __restrict__ target_T,
+                   const double* __restrict__ target_P, const double* __restrict__ compress, double* __restrict__ cells,
+                   double* __restrict__ x, double* __restrict__ mom, float* __restrict__ forces,
+                   float* __restrict__ stress_out, double* __restrict__ ekin_out, double* __restrict__ temp_out,
+                   double* __restrict__ press_out, int32_t* __restrict__ status) {
+  __shared__ double red[kBlock][3];
+  const int64_t c = blockIdx.x;
+  if (status[c] != kOk) return;
+  const int64_t g0 = atom_off[c], n = atom_off[c + 1] - g0;
+  if (g0 < 0 || n < 1 || atom_off[c + 1] > grad_rows) {
+    if (threadIdx.x == 0) status[c] = kBadInput;
+    return;
+  }
+  const float* gr = grad + 3 * g0;
+  const double* mc = masses + g0;
+  double* xc = x + 3 * g0;
+  double* pc = mom + 3 * g0;
+  const int t = threadIdx.x;
+  const double dt = p.dt;
+  const double half_dt = __dmul_rn(0.5, dt);
+  double tot[3];
+
+  if (p.phase == 1) {
+    double sx = 0.0, sy = 0.0, sz = 0.0;
+    for (int64_t i = t; i < n; i += kBlock) {
+      double q[3];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const double fd = (double)__fmul_rn(gr[3 * i + k], p.force_multiplier);
+        q[k] = __dadd_rn(pc[3 * i + k], __dmul_rn(half_dt, fd));
+        pc[3 * i + k] = q[k];
+      }
+      sx = __dadd_rn(sx, q[0]);
+      sy = __dadd_rn(sy, q[1]);
+      sz = __dadd_rn(sz, q[2]);
+    }
+    block_sum3(red, sx, sy, sz, tot);
+    const double nd = (double)n;
+    const double mean[3] = {__ddiv_rn(tot[0], nd), __ddiv_rn(tot[1], nd), __ddiv_rn(tot[2], nd)};
+    for (int64_t i = t; i < n; i += kBlock) {
+      const double m = mc[i];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const double pd = __dsub_rn(pc[3 * i + k], mean[k]);
+        pc[3 * i + k] = pd;
+        xc[3 * i + k] = __dadd_rn(xc[3 * i + k], __ddiv_rn(__dmul_rn(dt, pd), m));
+      }
+    }
+    return;
+  }
+
+  // ---- phase 0.  The cell of this evaluation (every thread forms the same V)
+  double C[9];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) C[k] = cells[9 * c + k];
+  const double V = fabs(C[0] * (C[4] * C[8] - C[5] * C[7]) - C[1] * (C[3] * C[8] - C[5] * C[6]) +
+                        C[2] * (C[3] * C[7] - C[4] * C[6]));
+  if (!(isfinite(V) && V > 0.0)) {
+    if (t == 0) status[c] = kCellDegenerate;
+    return;
+  }
+  const double invvol = __ddiv_rn(1.0, V);
+  const bool kick = p.evaluation >= 1;
+
+  // ---- 1. p_e, its kinetic energy and ideal-gas sums
+  double kin = 0.0, g[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  for (int64_t i = t; i < n; i += kBlock) {
+    const double m = mc[i];
+    double q[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      double pd = pc[3 * i + k];
+      if (kick) pd = __dadd_rn(pd, __dmul_rn(half_dt, (double)__fmul_rn(gr[3 * i + k], p.force_multiplier)));
+      q[k] = pd;
+      kin = __dadd_rn(kin, __dmul_rn(pd, __ddiv_rn(pd, m)));
+    }
+    add_ideal_gas_terms(q, __ddiv_rn(1.0, m), g);
+  }
+  double G[6], rest[3];
+  block_sum3(red, kin, g[0], g[1], tot);
+  block_sum3(red, g[2], g[3], g[4], G + 2);
+  block_sum3(red, g[5], 0.0, 0.0, rest);
+  G[0] = tot[1];
+  G[1] = tot[2];
+  G[5] = rest[0];
+  const double ekin = __dmul_rn(0.5, tot[0]);
+  const double T = __ddiv_rn(__dmul_rn(2.0, ekin), __dmul_rn((double)(3 * n), p.kB));
+  float sv[6], sc[6];
+  fire::calculator_stress(stress + 9 * c, p.stress_wt, sv);
+  const double P_log = corrected_pressure(sv, G, invvol, sc);
+
+  // ---- 2. the barostat on the scaled momenta
+  const bool step = p.evaluation < p.steps;
+  double s = 1.0, mu = 1.0;
+  if (step) {
+    s = berendsen_scale(target_T[c], T, dt, p.taut);
+    double h[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    for (int64_t i = t; i < n; i += kBlock) {
+      double q[3];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        double pd = pc[3 * i + k];
+        if (kick) pd = __dadd_rn(pd, __dmul_rn(half_dt, (double)__fmul_rn(gr[3 * i + k], p.force_multiplier)));
+        q[k] = __dmul_rn(s, pd);
+      }
+      add_ideal_gas_terms(q, __ddiv_rn(1.0, mc[i]), h);
+    }
+    double H[6];
+    block_sum3(red, h[0], h[1], h[2], H);
+    block_sum3(red, h[3], h[4], h[5], H + 3);
+    const double P = corrected_pressure(sv, H, invvol, sc);
+    const double taupscl = __ddiv_rn(dt, p.taup);
+    mu = __dsub_rn(1.0, __dmul_rn(__ddiv_rn(__dmul_rn(taupscl, compress[c]), 3.0), __dsub_rn(target_P[c], P)));
+    if (!(isfinite(mu) && mu > 0.0)) {
+      if (t == 0) status[c] = kCellDegenerate;
+      return;
+    }
+  }
+
+  // ---- 3. the writes
+  float* fc = forces + 3 * g0;
+  for (int64_t i = t; i < n; i += kBlock) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const float f = __fmul_rn(gr[3 * i + k], p.force_multiplier);
+      fc[3 * i + k] = f;
+      double pd = pc[3 * i + k];
+      if (kick) pd = __dadd_rn(pd, __dmul_rn(half_dt, (double)f));
+      if (step) {
+        pd = __dmul_rn(s, pd);                                  // NVTBerendsen.scale_velocities
+        xc[3 * i + k] = __dmul_rn(mu, xc[3 * i + k]);           // set_cell(mu C, scale_atoms=True)
+      }
+      pc[3 * i + k] = pd;
+    }
+  }
+  if (t == 0) {
+    ekin_out[c] = ekin;
+    temp_out[c] = T;
+    press_out[c] = P_log;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) stress_out[6 * c + k] = sv[k];
+    if (step) {
+#pragma unroll
+      for (int k = 0; k < 9; ++k) cells[9 * c + k] = __dmul_rn(mu, C[k]);
+    }
+  }
+}
+
 // the stream itself, for tests: item (a, j), a in [0, atoms), is block j of atom index atom0 + a (mod 2^32)
 __global__ void __launch_bounds__(kBlock)
 md_noise_kernel(uint64_t seed, uint32_t step, uint32_t tag, uint32_t atom0, int64_t items, int32_t blocks,
@@ -431,6 +623,29 @@ int alignn_b200_md_thermostat_step(const alignn_b200_md_thermostat_params* param
   md_thermostat_kernel<<<(unsigned)num_crystals, kBlock, 0, (cudaStream_t)stream>>>(
       p, atom_offsets, grad, grad_rows, masses, target_temperature, seeds, positions, momenta, velocities, rnd_vel,
       forces, kinetic_energy, temperature, status);
+  return alignn::check_launch();
+}
+
+int alignn_b200_md_npt_step(const alignn_b200_md_npt_params* params, const int64_t* atom_offsets, int64_t num_crystals,
+                            const float* grad, int64_t grad_rows, const float* stress, const double* masses,
+                            const double* target_temperature, const double* target_pressure,
+                            const double* compressibility, double* cells, double* positions, double* momenta,
+                            float* forces, float* stress_out, double* kinetic_energy, double* temperature,
+                            double* pressure, int32_t* status, alignn_stream_t stream) {
+  using namespace alignn::md;
+  if (!params || num_crystals < 1 || num_crystals > INT32_MAX || grad_rows < 0) return ALIGNN_ERR_BAD_ARG;
+  const alignn_b200_md_npt_params p = *params;
+  const auto positive = [](double v) { return isfinite(v) && v > 0.0; };
+  if (p.steps < 1 || p.evaluation < 0 || p.evaluation > p.steps || (p.phase != 0 && p.phase != 1) ||
+      (p.phase == 1 && p.evaluation == p.steps) || !positive(p.dt) || !positive(p.kB) || !positive(p.taut) ||
+      !positive(p.taup) || !(p.taut >= p.dt) || !isfinite(p.force_multiplier) || !isfinite(p.stress_wt))
+    return ALIGNN_ERR_BAD_ARG;
+  if (!atom_offsets || !grad || !stress || !masses || !target_temperature || !target_pressure || !compressibility ||
+      !cells || !positions || !momenta || !forces || !stress_out || !kinetic_energy || !temperature || !pressure || !status)
+    return ALIGNN_ERR_BAD_ARG;
+  md_npt_step_kernel<<<(unsigned)num_crystals, kBlock, 0, (cudaStream_t)stream>>>(
+      p, atom_offsets, grad, grad_rows, stress, masses, target_temperature, target_pressure, compressibility, cells,
+      positions, momenta, forces, stress_out, kinetic_energy, temperature, pressure, status);
   return alignn::check_launch();
 }
 

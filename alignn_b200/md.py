@@ -1,5 +1,5 @@
-"""Molecular dynamics for a batch of crystals with ALIGNN-FF on the GPU: NVE velocity Verlet, NVT Berendsen, NVT Langevin
-and NVT Andersen.
+"""Molecular dynamics for a batch of crystals with ALIGNN-FF on the GPU: NVE velocity Verlet, NVT Berendsen, NVT Langevin,
+NVT Andersen and NPT Berendsen.
 
 The reference runs MD one structure at a time: `ForceField.run_nve_velocity_verlet` and `run_nvt_berendsen`
 (alignn/ff/ff.py:419-443, 510-543) drive ASE's integrators, and every step its calculator (alignn/ff/calculators.py:
@@ -10,7 +10,9 @@ also writes each crystal's kinetic energy and temperature.  Each crystal follows
 alone; `oracle/md_oracle.py` is the specification (ASE 3.22.1 semantics, float64 state).  The stochastic thermostats
 (`ForceField.run_nvt_langevin` / `run_nvt_andersen`, alignn/ff/ff.py:444-508) launch `ops.md_thermostat_step` instead
 and draw their noise from a counter-based stream keyed by each crystal's seed (csrc/md_noise.cuh) rather than numpy's
-global RNG; `oracle/md_thermostat_oracle.py` is their specification.
+global RNG; `oracle/md_thermostat_oracle.py` is their specification.  NPT Berendsen (`ForceField.run_npt_berendsen`,
+alignn/ff/ff.py:545-582) moves the cells too: every step rebuilds the graphs from the rescaled cells, evaluates the
+model twice and launches `ops.md_npt_step` after each evaluation; `oracle/md_npt_oracle.py` is its specification.
 """
 from __future__ import annotations
 
@@ -22,17 +24,20 @@ import numpy as np
 import torch
 
 from . import neighbors, ops
-from .relax import _check_batch, _check_model, _forces_as_alone
+from .relax import _check_batch, _check_model, _forces_and_stress_as_alone, _forces_as_alone
 
 # ase.units (ASE 3.22.1, CODATA 2014): the femtosecond in ASE time units and the Boltzmann constant in eV/K
 _e, _amu, _k = 1.6021766208e-19, 1.660539040e-27, 1.38064852e-23
 FS = 1e-15 * (1e10 * math.sqrt(_e / _amu))     # 0.09822694788464063
 KB = _k / _e                                   # 8.617330337217213e-05
+BAR = 1e5 * ((1 / _e) / 1e30)                  # ase.units: 1e5 * Pascal, the bar in eV/A^3
 
 ENSEMBLES = {"nve_velocity_verlet": ops.MD_NVE, "nvt_berendsen": ops.MD_NVT_BERENDSEN,
-             "nvt_langevin": ops.MD_NVT_LANGEVIN, "nvt_andersen": ops.MD_NVT_ANDERSEN}
+             "nvt_langevin": ops.MD_NVT_LANGEVIN, "nvt_andersen": ops.MD_NVT_ANDERSEN,
+             "npt_berendsen": ops.MD_NPT_BERENDSEN}
 STOCHASTIC = (ops.MD_NVT_LANGEVIN, ops.MD_NVT_ANDERSEN)
 LANGEVIN_FRICTION = 1e-4      # ForceField.run_nvt_langevin's default friction, in 1 / ASE time unit
+NPT_TAUT = 49.11347394232032  # ForceField.run_npt_berendsen's taut literal: 500 fs in ASE units, bitwise
 
 
 class MDResult(NamedTuple):
@@ -44,6 +49,20 @@ class MDResult(NamedTuple):
     temperature: torch.Tensor     # [steps+1,B] float64 temperature per evaluation (K)
     atom_offsets: torch.Tensor    # [B+1] int64: atoms of crystal b are rows atom_offsets[b]:atom_offsets[b+1]
     trajectory: Optional[torch.Tensor]   # [T,N,3] float64 positions at evaluations 0, k, 2k, ... <= steps, or None
+
+
+class NPTResult(NamedTuple):
+    positions: torch.Tensor       # [N,3] float64 final Cartesian positions (not wrapped into the cell)
+    momenta: torch.Tensor         # [N,3] float64 final momenta (ASE units: amu * A / ASE time)
+    forces: torch.Tensor          # [N,3] fp32 forces of the last logged evaluation, grad * force_multiplier
+    energy: torch.Tensor          # [steps+1,B] fp32 potential energy per logged evaluation, out * natoms
+    kinetic_energy: torch.Tensor  # [steps+1,B] float64 kinetic energy per logged evaluation (eV)
+    temperature: torch.Tensor     # [steps+1,B] float64 temperature per logged evaluation (K)
+    atom_offsets: torch.Tensor    # [B+1] int64: atoms of crystal b are rows atom_offsets[b]:atom_offsets[b+1]
+    trajectory: Optional[torch.Tensor]   # [T,N,3] float64 positions at logged evaluations 0, k, 2k, ..., or None
+    cells: torch.Tensor           # [steps+1,B,3,3] float64 the cell of each logged evaluation (rows: lattice vectors)
+    stress: torch.Tensor          # [steps+1,B,6] fp32 the calculator's Voigt stress (eV/A^3; xx yy zz yz xz xy)
+    pressure: torch.Tensor        # [steps+1,B] float64 -trace/3 of that stress less the ideal-gas term (eV/A^3)
 
 
 def maxwell_boltzmann_momenta(masses, temperature_K: float, rng=None) -> np.ndarray:
@@ -93,7 +112,8 @@ def run_md(model, structures, atom_features: torch.Tensor, masses, *, ensemble: 
            steps: int = 1000, timestep: float = 0.01, temperature_K=300.0, taut: Optional[float] = None, momenta=None,
            trajectory_interval: Optional[int] = None, neighbor_strategy: str = "k-nearest", cutoff: float = 8.0,
            max_neighbors: int = 12, cutoff_extra: float = 3.5, force_multiplier: float = 1.0,
-           friction: Optional[float] = None, andersen_prob: float = 0.1, seed=None) -> MDResult:
+           friction: Optional[float] = None, andersen_prob: float = 0.1, seed=None, pressure=None,
+           compressibility=None, taup: float = 1000.0, stress_wt: float = 1.0):
     """Run `steps` steps of molecular dynamics on a batch of crystals, the cells fixed: a batched
     `ForceField.run_nve_velocity_verlet(steps=steps)` (ensemble="nve_velocity_verlet", ASE's VelocityVerlet) or
     `run_nvt_berendsen(temperature_K=..., taut=..., steps=steps)` (ensemble="nvt_berendsen", ASE's NVTBerendsen with
@@ -119,7 +139,19 @@ def run_md(model, structures, atom_features: torch.Tensor, masses, *, ensemble: 
     andersen_prob in [0, 1] per component and step (ForceField's 0.1).  seed is required: an int in [0, 2^63), crystal
     b drawing the stream of seed + b, or B ints in [0, 2^64), one per crystal.  Nothing is drawn from global state: a
     crystal's trajectory is a function of the arguments and of its own seed, so run alone with that seed it repeats
-    its trajectory in the batch bit for bit.  Langevin (fixcm) divides by n - 1 and rejects one-atom crystals."""
+    its trajectory in the batch bit for bit.  Langevin (fixcm) divides by n - 1 and rejects one-atom crystals.
+
+    NPT Berendsen (ensemble="npt_berendsen"): `run_npt_berendsen(temperature_K=..., taut=..., taup=..., pressure=...,
+    compressibility=...)`, ASE's NPTBerendsen with fixcm=True -- the Berendsen thermostat, then the cell and positions
+    scaled by mu = 1 - (dt/taup) compressibility / 3 (pressure - P) every step, P the pressure of the calculator's
+    stress s = fp32(voigt(stress) * stress_wt / 160.21766208) with the ideal-gas term of the momenta.  pressure in bar
+    (any sign) and compressibility in 1/bar (>= 0; 0 switches the barostat off) are required, one value or one per
+    crystal; taup in fs (ForceField's 1000 fs); taut None means ForceField's 500 fs here.  The model must compute stress
+    (stresswise_weight != 0).  Each step evaluates twice, at the rescaled structure (its forces drive the half-kick)
+    and after the drift (logged), so steps + 1 of the 2 steps + 1 evaluations are logged.  Returns an `NPTResult`: the
+    MDResult fields plus the cell, the calculator's stress and the pressure of every logged evaluation.  A cell whose
+    volume or scale factor stops being finite and > 0 raises RuntimeError naming the crystal and the step.  The
+    pressure keywords are ignored by the other ensembles."""
     _check_model("run_md", model)
     if ensemble not in ENSEMBLES:
         raise ValueError(f"ensemble must be one of {sorted(ENSEMBLES)}, got {ensemble!r}")
@@ -148,9 +180,9 @@ def run_md(model, structures, atom_features: torch.Tensor, masses, *, ensemble: 
         if len(t) != B or not all(_real(v) and v > 0 for v in t):
             raise ValueError(f"temperature_K must be a finite number > 0 or {B} of them, got {temperature_K!r}")
         T0 = torch.tensor([float(v) for v in t], dtype=torch.float64, device=dev)
-    if kind == ops.MD_NVT_BERENDSEN:
-        if taut is None:
-            taut_ase = 100 * dt                         # ForceField: taut = 100 * self.timestep, in ASE units
+    if kind in (ops.MD_NVT_BERENDSEN, ops.MD_NPT_BERENDSEN):
+        if taut is None:                                # ForceField: taut = 100 * self.timestep, in ASE units (NVT)
+            taut_ase = NPT_TAUT if kind == ops.MD_NPT_BERENDSEN else 100 * dt
         elif not _real(taut):
             raise ValueError(f"taut must be a finite number (fs), got {taut!r}")
         else:
@@ -177,6 +209,13 @@ def run_md(model, structures, atom_features: torch.Tensor, masses, *, ensemble: 
     pos = torch.from_numpy(np.ascontiguousarray(np.concatenate(Xs))).to(dev)
     mom = torch.from_numpy(np.ascontiguousarray(p0)).to(dev)
     m_d = torch.from_numpy(np.ascontiguousarray(m)).to(dev)
+    if kind == ops.MD_NPT_BERENDSEN:
+        return _run_npt(model, lats, Xs, atom_features, aoff, pos, mom, m_d, T0, dev, steps=int(steps), dt=dt,
+                        taut=taut_ase, pressure=pressure, compressibility=compressibility, taup=taup,
+                        stress_wt=stress_wt, trajectory_interval=trajectory_interval,
+                        graph=dict(neighbor_strategy=neighbor_strategy, cutoff=cutoff, max_neighbors=max_neighbors,
+                                   cutoff_extra=cutoff_extra),
+                        force_multiplier=float(force_multiplier))
     forces = torch.zeros(N, 3, device=dev, dtype=torch.float32)
     energy = torch.zeros(steps + 1, B, device=dev, dtype=torch.float32)
     ekin = torch.zeros(steps + 1, B, device=dev, dtype=torch.float64)
@@ -223,3 +262,99 @@ def run_md(model, structures, atom_features: torch.Tensor, masses, *, ensemble: 
             if not np.isfinite(host_pos[b]).all():
                 raise RuntimeError(f"run_md: the positions of crystal {b} are not finite after step {e + 1}")
     return MDResult(pos, mom, forces, energy, ekin, temp, aoff_d, torch.stack(traj) if traj else None)
+
+
+def _per_crystal(v, B: int, name: str, unit: str, ok) -> list:
+    vals = [v] * B if np.ndim(v) == 0 else list(v)
+    if v is None or len(vals) != B or not all(_real(x) and ok(x) for x in vals):
+        raise ValueError(f"npt_berendsen needs {name} ({unit}): a finite number{'' if name == 'pressure' else ' >= 0'} "
+                         f"or {B} of them, got {v!r}")
+    return [float(x) for x in vals]
+
+
+def _run_npt(model, lats, Xs, atom_features, aoff, pos, mom, m_d, T0, dev, *, steps, dt, taut, pressure,
+             compressibility, taup, stress_wt, trajectory_interval, graph, force_multiplier) -> NPTResult:
+    """run_md's NPT Berendsen loop: per step, phase 0 after the logged evaluation, then evaluation A at the rescaled
+    structure and phase 1 (see csrc/md_device.cu)."""
+    B, N = len(Xs), int(aoff[-1])
+    if model.config.stresswise_weight == 0:
+        raise ValueError("run_md(ensemble='npt_berendsen') needs a model that computes stress (stresswise_weight != 0)")
+    P0 = _per_crystal(pressure, B, "pressure", "bar", lambda x: True)
+    comp = _per_crystal(compressibility, B, "compressibility", "1/bar", lambda x: x >= 0)
+    if not _real(taup) or not taup > 0:
+        raise ValueError(f"taup must be a finite number > 0 (fs), got {taup!r}")
+    if not _real(stress_wt):
+        raise ValueError(f"stress_wt must be a finite real number, got {stress_wt!r}")
+    f64 = dict(dtype=torch.float64, device=dev)
+    P0_d = torch.tensor([v * BAR for v in P0], **f64)          # NPTBerendsen: pressure * (1e5 * units.Pascal)
+    comp_d = torch.tensor([v / BAR for v in comp], **f64)      # compressibility / (1e5 * units.Pascal)
+    cells = torch.from_numpy(np.ascontiguousarray(np.stack(lats))).to(dev)
+    forces = torch.zeros(N, 3, device=dev, dtype=torch.float32)
+    energy = torch.zeros(steps + 1, B, device=dev, dtype=torch.float32)
+    ekin, temp, press = (torch.zeros(steps + 1, B, **f64) for _ in range(3))
+    cell_log = torch.zeros(steps + 1, B, 3, 3, **f64)
+    stress_log = torch.zeros(steps + 1, B, 6, device=dev, dtype=torch.float32)
+    status = torch.zeros(B, device=dev, dtype=torch.int32)
+    aoff_d = torch.from_numpy(aoff).to(dev)
+    host_cells, host_pos = [np.array(c, dtype=np.float64) for c in lats], [x.copy() for x in Xs]
+    kw = dict(steps=steps, dt=dt, kB=KB, taut=taut, taup=float(taup) * FS, force_multiplier=force_multiplier,
+              stress_wt=float(stress_wt))
+    traj = []
+
+    def evaluate(with_stress):
+        with ops._span("md_build", 0):
+            g, lg, lat = neighbors.crystal_graphs_device(list(zip(host_cells, host_pos)), atom_features, device=dev,
+                                                         **graph)
+        with ops._span("md_model", 0):
+            with torch.enable_grad():
+                res = model((g, lg, lat))
+                if with_stress:
+                    return g, res, _forces_and_stress_as_alone(model, g, res, B)
+                return g, res, (_forces_as_alone(model, g, res, B), None)
+
+    def read_back(e, phase, with_cells):
+        with ops._span("md_readback", 0):
+            # one copy: the statuses, then (the cells and) the positions the next graph build needs
+            back = torch.cat([status.to(torch.float64)] + ([cells.reshape(-1)] if with_cells else []) +
+                             [pos.reshape(-1)]).cpu().numpy()
+        st = back[:B]
+        if (st == ops.MD_BAD_INPUT).any():
+            raise RuntimeError("alignn_b200_md_npt_step: the model's forces do not match the crystals' atom counts")
+        bad = np.flatnonzero(st == ops.MD_CELL_DEGENERATE)
+        if bad.size:
+            raise RuntimeError(f"run_md: the cell of crystal {int(bad[0])} became degenerate in step {e + 1} (its volume "
+                               "or the barostat's scale factor is not finite and positive)")
+        if (st != 0).any():
+            raise RuntimeError(f"run_md: the MD kernel reported statuses {st.astype(int).tolist()}")
+        o = B
+        if with_cells:
+            new_cells = back[B:B + 9 * B].reshape(B, 3, 3)
+            o += 9 * B
+            for b in range(B):
+                host_cells[b] = new_cells[b]
+        new_pos = back[o:].reshape(-1, 3)
+        for b in range(B):
+            host_pos[b] = new_pos[aoff[b]:aoff[b + 1]]
+            if phase == 1 and not np.isfinite(host_pos[b]).all():
+                raise RuntimeError(f"run_md: the positions of crystal {b} are not finite after step {e + 1}")
+
+    for e in range(steps + 1):
+        g, res, (grad, stress) = evaluate(True)                     # logged evaluation e (B of step e)
+        out = res["out"].detach().reshape(-1)
+        energy[e] = out * g.batch_num_nodes_on_device().to(out.dtype)
+        if trajectory_interval is not None and e % trajectory_interval == 0:
+            traj.append(pos.clone())
+        cell_log[e] = cells
+        with ops._span("md_step", 0):
+            ops.md_npt_step(grad, stress, aoff_d, m_d, T0, P0_d, comp_d, cells, pos, mom, forces, stress_log[e], ekin[e],
+                            temp[e], press[e], status, evaluation=e, phase=0, **kw)
+        read_back(e, 0, e < steps)
+        if e == steps:
+            break
+        _, _, (grad, _) = evaluate(False)                           # evaluation A of step e + 1
+        with ops._span("md_step", 0):
+            ops.md_npt_step(grad, stress, aoff_d, m_d, T0, P0_d, comp_d, cells, pos, mom, forces, stress_log[e], ekin[e],
+                            temp[e], press[e], status, evaluation=e, phase=1, **kw)
+        read_back(e, 1, False)
+    return NPTResult(pos, mom, forces, energy, ekin, temp, aoff_d, torch.stack(traj) if traj else None, cell_log,
+                     stress_log, press)

@@ -595,6 +595,58 @@ def md_thermostat_step(grad: torch.Tensor, atom_offsets: torch.Tensor, masses: t
         stream_ptr()), "alignn_b200_md_thermostat_step")
 
 
+MD_NPT_BERENDSEN = 4              # run_md's code for NPT Berendsen (its own kernel, alignn_b200_md_npt_step)
+MD_CELL_DEGENERATE = 4            # status of a crystal whose volume or barostat scale is not finite and > 0
+
+
+@_on_tensor_device
+def md_npt_step(grad: torch.Tensor, stress: torch.Tensor, atom_offsets: torch.Tensor, masses: torch.Tensor,
+                target_temperature: torch.Tensor, target_pressure: torch.Tensor, compressibility: torch.Tensor,
+                cells: torch.Tensor, positions: torch.Tensor, momenta: torch.Tensor, forces: torch.Tensor,
+                stress_out: torch.Tensor, kinetic_energy: torch.Tensor, temperature: torch.Tensor,
+                pressure: torch.Tensor, status: torch.Tensor, *, evaluation: int, steps: int, phase: int, dt: float,
+                kB: float, taut: float, taup: float, force_multiplier: float = 1.0, stress_wt: float = 1.0) -> None:
+    """One launch of an MD run of `steps` steps under ASE 3.22.1's `NPTBerendsen` (fixcm=True) for every crystal, in
+    place (csrc/md_device.cu, alignn_b200_md_npt_step).  phase 0, after logged evaluation `evaluation`: the forces, the
+    second half-kick (evaluation >= 1), the log rows, and unless evaluation == steps the velocity scaling and the
+    barostat's rescaling of cells and positions.  phase 1, after evaluation A of the next step: the half-kick on its
+    forces, the mean momentum removed, the drift.
+
+    As `md_step`, plus: stress [B,3,3] fp32, the model's stress (phase 0; not read in phase 1); target_temperature (K),
+    target_pressure (eV/A^3) and compressibility (A^3/eV) [B] float64; cells [B,3,3] float64 (rows are lattice vectors,
+    scaled in place); stress_out [B,6] fp32 (written: the calculator's Voigt stress) and pressure [B] float64 (written:
+    -trace/3 of that stress less the ideal-gas term, eV/A^3), the log rows of this evaluation; status
+    MD_CELL_DEGENERATE for a cell whose volume or barostat scale is not finite and > 0 (nothing of the crystal is
+    written).  dt, taut and taup in ASE time units.  Enqueue only: the statuses are the caller's to read back."""
+    lib = _lib.load()
+    _md_operands("md_npt_step",
+                 [(grad, torch.float32), (stress, torch.float32), (atom_offsets, torch.int64), (masses, torch.float64),
+                  (target_temperature, torch.float64), (target_pressure, torch.float64),
+                  (compressibility, torch.float64), (cells, torch.float64), (positions, torch.float64),
+                  (momenta, torch.float64), (forces, torch.float32), (stress_out, torch.float32),
+                  (kinetic_energy, torch.float64), (temperature, torch.float64), (pressure, torch.float64),
+                  (status, torch.int32)], grad.device)
+    B = atom_offsets.numel() - 1
+    N = positions.numel() // 3
+    if (B < 1 or positions.numel() != 3 * N or momenta.numel() != 3 * N or forces.numel() != 3 * N
+            or masses.numel() != N or stress.numel() != 9 * B or cells.numel() != 9 * B or stress_out.numel() != 6 * B
+            or any(t.numel() != B for t in (target_temperature, target_pressure, compressibility, kinetic_energy,
+                                             temperature, pressure, status))
+            or grad.dim() != 2 or grad.shape[1] != 3 or grad.shape[0] > N):
+        raise ValueError("md_npt_step: inconsistent operand shapes")
+    if isinstance(steps, bool) or int(steps) != steps or not 1 <= int(steps) <= FIRE_MAX_STEPS:
+        raise ValueError(f"md_npt_step: steps must be an integer in [1, {FIRE_MAX_STEPS}], got {steps!r}")
+    if isinstance(evaluation, bool) or int(evaluation) != evaluation or not 0 <= int(evaluation) <= int(steps):
+        raise ValueError(f"md_npt_step: evaluation must be an integer in [0, steps], got {evaluation!r}")
+    p = _lib.MdNptParams(float(dt), float(taut), float(taup), float(kB), int(evaluation), int(steps), int(phase),
+                         float(force_multiplier), float(stress_wt))
+    _lib.check(lib.alignn_b200_md_npt_step(
+        C.byref(p), atom_offsets.data_ptr(), B, grad.data_ptr(), grad.shape[0], stress.data_ptr(), masses.data_ptr(),
+        target_temperature.data_ptr(), target_pressure.data_ptr(), compressibility.data_ptr(), cells.data_ptr(),
+        positions.data_ptr(), momenta.data_ptr(), forces.data_ptr(), stress_out.data_ptr(), kinetic_energy.data_ptr(),
+        temperature.data_ptr(), pressure.data_ptr(), status.data_ptr(), stream_ptr()), "alignn_b200_md_npt_step")
+
+
 def md_noise(seed: int, step: int, count: int, *, tag: int = MD_NVT_LANGEVIN, atom0: int = 0, blocks: int = 1,
              device=None):
     """The thermostats' noise stream (csrc/md_noise.cuh) on the device, for tests: Philox block j of atom index

@@ -736,6 +736,50 @@ int alignn_b200_md_thermostat_step(const alignn_b200_md_thermostat_params* param
                                    double* momenta, double* velocities, double* rnd_vel, float* forces,
                                    double* kinetic_energy, double* temperature, int32_t* status, alignn_stream_t stream);
 
+/* Constant-pressure MD (csrc/md_device.cu): ASE 3.22.1's `NPTBerendsen` (fixcm=True) -- what
+ * `ForceField.run_npt_berendsen` (alignn/ff/ff.py:545-582) runs one crystal at a time -- with the run loop of
+ * `MolecularDynamics.irun`, for a batch of crystals advanced in lockstep.  Each step evaluates the model twice: at the
+ * rescaled structure (evaluation A, forces only) and after the drift (evaluation B, logged). */
+typedef struct {
+  double dt;                /* time step in ASE time units                                         */
+  double taut;              /* Berendsen thermostat coupling time, ASE time units, >= dt           */
+  double taup;              /* barostat coupling time, ASE time units, > 0                         */
+  double kB;                /* Boltzmann constant, eV/K                                            */
+  int32_t evaluation;       /* e in [0, steps]: the logged evaluation, or the step e + 1 of phase 1 */
+  int32_t steps;            /* steps >= 1                                                          */
+  int32_t phase;            /* 0: after logged evaluation e; 1: after evaluation A of step e + 1   */
+  float force_multiplier;   /* F = fp32(grad * force_multiplier)                                   */
+  float stress_wt;          /* s = fp32(voigt(stress) * stress_wt / 160.21766208), as fire_cell     */
+} alignn_b200_md_npt_params;
+
+/* One CTA per crystal c with status 0 (n atoms, masses m, cell C = cells[c] with rows the lattice vectors, V = |det C|):
+ *   phase 0 (grad and stress of logged evaluation e): F = fp32(grad * force_multiplier) to forces; if e >= 1 the
+ *   second half-kick p += (0.5 dt) F; s = the calculator's fp32 Voigt stress of stress[c] (xx yy zz yz xz xy, eV/A^3)
+ *   to stress_out[c]; kinetic_energy[c] and temperature[c] as alignn_b200_md_step; pressure[c] = -tr(s')/3 with
+ *   s'_k = fp32(s_k - sum_i p_a p_b / m / V) (Atoms.get_stress(include_ideal_gas=True), the trace in fp32).  If e < steps:
+ *   p = s_T p (s_T as alignn_b200_md_step's Berendsen scale with T0 = target_temperature[c]); P = -tr(s')/3 of these
+ *   momenta; mu = 1 - (dt/taup) compressibility[c] / 3 (target_pressure[c] - P); C = mu C; x = mu x.
+ *   phase 1 (grad of evaluation A, at the rescaled structure; stress is not read, nothing but momenta and positions
+ *   written): p += (0.5 dt) F; p -= sum_i p_i / n; x = x + (dt p) / m.
+ *   Status 3 (inconsistent input): the slice does not lie inside [0, grad_rows) or is empty.  Status 4 (cell
+ *   degenerate, phase 0): V or, for e < steps, mu is not finite and > 0.  Either way nothing else is read or written for
+ *   c in that launch, and crystals with a nonzero status are not touched.  Sums are in double with fixed-order block
+ *   reductions; per-element updates follow numpy's order with IEEE divisions; no float atomics.
+ *   grad [grad_rows, 3] fp32; stress [num_crystals, 3, 3] fp32 (the model's stress, GPa); atom_offsets
+ *   [num_crystals+1] int64; masses [>= grad_rows] double (amu, > 0); target_temperature (K), target_pressure (eV/A^3),
+ *   compressibility (A^3/eV, >= 0) [num_crystals] double; cells [num_crystals, 3, 3] double; positions / momenta
+ *   [>= grad_rows, 3] double; forces [>= grad_rows, 3] fp32; stress_out [num_crystals, 6] fp32; kinetic_energy /
+ *   temperature / pressure [num_crystals] double (the caller passes row e of its logs); status [num_crystals] int32.
+ * Rejected (ALIGNN_ERR_BAD_ARG, nothing enqueued): NULL params or a NULL array, num_crystals < 1, grad_rows < 0,
+ * steps < 1, evaluation outside [0, steps] (outside [0, steps) for phase 1), a phase other than 0 or 1, dt, kB, taut or
+ * taup not finite and > 0, taut < dt, a non-finite force_multiplier or stress_wt. */
+int alignn_b200_md_npt_step(const alignn_b200_md_npt_params* params, const int64_t* atom_offsets, int64_t num_crystals,
+                            const float* grad, int64_t grad_rows, const float* stress, const double* masses,
+                            const double* target_temperature, const double* target_pressure,
+                            const double* compressibility, double* cells, double* positions, double* momenta,
+                            float* forces, float* stress_out, double* kinetic_energy, double* temperature,
+                            double* pressure, int32_t* status, alignn_stream_t stream);
+
 /* The thermostats' noise stream, for tests: item q = a * blocks + j (a in [0, atoms), j in [0, blocks)) is Philox block
  * j of atom index atom0 + a (mod 2^32) at (seed, step, tag): words [atoms*blocks, 4] uint32, its two uniforms
  * [atoms*blocks, 2] double and their Box-Muller normals [atoms*blocks, 2] double.  Rejected (ALIGNN_ERR_BAD_ARG):

@@ -8,11 +8,17 @@ evaluations per crystal), with the reference's defaults: NVT Berendsen (the defa
 Langevin with friction 1e-4 per ASE time unit, NVT Andersen with andersen_prob 0.1.  The stochastic ensembles draw
 crystal b's noise from the stream of seed `--seed` + b and draw their structures from the samples with two atoms or
 more (Langevin with fixcm rejects one-atom crystals).  Masses are seeded random values in [1, 200] amu.
+NPT Berendsen (`--ensemble npt_berendsen`) runs ForceField's taut = 500 fs and taup = 1000 fs at `--pressure-bar`
+(default 1.01325 bar, one atmosphere: ASE's own NPTBerendsen example) with `--compressibility` (default 1e-6 / bar, a
+solid with a bulk modulus of 100 GPa); the reference passes neither, and its own call cannot run without them.  Its
+model is the same with `stresswise_weight=1` (the other ensembles keep the stress off, so their numbers stay
+comparable), and each step evaluates the model twice.
 
   batched:     run_md -- per evaluation one device graph build, one model call and one integrator launch for the batch;
   per-crystal: for each crystal, every evaluation runs neighbors.crystal_graph on the host, .to("cuda"), the same model
                on a one-crystal batch, and the oracle's integrator step in numpy (oracle/md_oracle.py, or
-               oracle/md_thermostat_oracle.py on the same restated noise stream).
+               oracle/md_thermostat_oracle.py on the same restated noise stream; for NPT the graph is built on the
+               current cell and the integrator is oracle/md_npt_oracle.py).
 
 Each arm runs three times (alternating); the median wall time (ending in a synchronise) is reported.  One more batched
 run with CUDA events around its phases gives the per-evaluation split (build, model, step kernel, read-back; each span
@@ -21,8 +27,8 @@ final positions is reported, and per crystal whether its 12th-neighbour cut lies
 (`neighbors.knn_cut_is_tied`) at any structure the host arm evaluated: there rounding picks the images the k-nearest
 graph keeps, and the arms may part.  The device name, power limit and SM clock limit are read in the same run.
 
-    python tools/bench_md.py [--ensemble nvt_berendsen|nvt_langevin|nvt_andersen] [--structures 64] [--steps 50]
-                             [--seed 0]
+    python tools/bench_md.py [--ensemble nvt_berendsen|nvt_langevin|nvt_andersen|npt_berendsen] [--structures 64]
+                             [--steps 50] [--seed 0] [--pressure-bar 1.01325] [--compressibility 1e-6]
 """
 import argparse
 import json
@@ -54,7 +60,10 @@ def main():
     ap.add_argument("--structures", type=int, default=64)
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--seed", type=int, default=0)
-    ap.add_argument("--ensemble", choices=("nvt_berendsen", "nvt_langevin", "nvt_andersen"), default="nvt_berendsen")
+    ap.add_argument("--ensemble", choices=("nvt_berendsen", "nvt_langevin", "nvt_andersen", "npt_berendsen"),
+                    default="nvt_berendsen")
+    ap.add_argument("--pressure-bar", type=float, default=1.01325)
+    ap.add_argument("--compressibility", type=float, default=1e-6, help="1/bar")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_md.py needs a CUDA device")
@@ -62,6 +71,7 @@ def main():
     __graft_entry__.build()
     from alignn_b200 import maxwell_boltzmann_momenta, neighbors, ops, run_md
     from alignn_b200.alignn_atomwise import ALIGNNAtomWise, ALIGNNAtomWiseConfig
+    from oracle import md_npt_oracle as NO
     from oracle import md_oracle as MO
     from oracle import md_thermostat_oracle as TO
 
@@ -70,7 +80,8 @@ def main():
     off = z["atom_offsets"]
     rng = np.random.default_rng(a.seed)
     pool = np.arange(len(z["ids"]))
-    if a.ensemble != "nvt_berendsen":                          # Langevin (fixcm) rejects one-atom crystals
+    npt = a.ensemble == "npt_berendsen"
+    if a.ensemble in ("nvt_langevin", "nvt_andersen"):         # Langevin (fixcm) rejects one-atom crystals
         pool = pool[off[1:] - off[:-1] >= 2]
     pick = rng.choice(pool, min(a.structures, len(pool)), replace=False)
     structs = [(z["lattices"][i], z["cart_coords"][off[i]:off[i + 1]] + rng.normal(scale=0.03, size=(off[i + 1] - off[i], 3)))
@@ -82,12 +93,14 @@ def main():
     p0 = maxwell_boltzmann_momenta(masses, 300.0, rng)
     torch.manual_seed(1)
     cfg = ALIGNNAtomWiseConfig(name="alignn_atomwise", alignn_layers=4, gcn_layers=4, hidden_features=256,
-                               atom_input_features=92, gradwise_weight=1.0, stresswise_weight=0.0)
+                               atom_input_features=92, gradwise_weight=1.0, stresswise_weight=1.0 if npt else 0.0)
     model = ALIGNNAtomWise(cfg).to(dev).eval()
     timestep, T0 = 1.0, 300.0
 
     def batched():
         extra = {} if a.ensemble == "nvt_berendsen" else dict(seed=a.seed)
+        if npt:
+            extra = dict(pressure=a.pressure_bar, compressibility=a.compressibility)
         r = run_md(model, structs, feats, masses, ensemble=a.ensemble, steps=a.steps, timestep=timestep,
                    temperature_K=T0, momenta=p0, **extra)
         torch.cuda.synchronize()
@@ -106,12 +119,24 @@ def main():
             visited.append(seen)
 
             def evaluate(x, lat=lat, f_b=f_b, lat_t=lat_t, n=X.shape[0], seen=seen):
-                seen.append(x.copy())
+                seen.append((lat, x.copy()))
                 g, lg = neighbors.crystal_graph(lat, x, f_b, cutoff=8.0, neighbor_strategy="k-nearest", max_neighbors=12)
                 res = model((g.to(dev), lg.to(dev), lat_t))
                 return float(res["out"].detach() * n), res["grad"].detach().reshape(-1, 3).cpu().numpy()
+
+            def evaluate_cell(cell, x, f_b=f_b, n=X.shape[0], seen=seen):
+                seen.append((cell, x.copy()))
+                g, lg = neighbors.crystal_graph(cell, x, f_b, cutoff=8.0, neighbor_strategy="k-nearest", max_neighbors=12)
+                g.ndata["V"] = torch.full((n,), abs(float(np.dot(np.cross(cell[0], cell[1]), cell[2]))),
+                                          dtype=torch.float32)
+                res = model((g.to(dev), lg.to(dev), torch.tensor(cell, dtype=torch.float32).view(1, 3, 3).to(dev)))
+                return (float(res["out"].detach() * n), res["grad"].detach().reshape(-1, 3).cpu().numpy(),
+                        res["stresses"].detach().reshape(3, 3).cpu().numpy())
             dt = timestep * MO.fs
-            if a.ensemble == "nvt_berendsen":
+            if npt:
+                out.append(NO.run(evaluate_cell, lat, X, masses[sl], steps=a.steps, dt=dt, temperature_K=T0,
+                                  pressure=a.pressure_bar, compressibility=a.compressibility, momenta=p0[sl]))
+            elif a.ensemble == "nvt_berendsen":
                 out.append(MO.run(evaluate, X, masses[sl], ensemble=MO.NVT_BERENDSEN, steps=a.steps, dt=dt,
                                   temperature_K=T0, taut=100 * dt, momenta=p0[sl]))
             else:
@@ -134,7 +159,7 @@ def main():
     P = got.positions.cpu().numpy()
     T = got.temperature.cpu().numpy()
     dpos = [float(np.abs(P[aoff[b]:aoff[b + 1]] - r["positions"]).max()) for b, r in enumerate(ref)]
-    tied = [any(neighbors.knn_cut_is_tied(lat, x) for x in seen) for (lat, _), seen in zip(structs, visited)]
+    tied = [any(neighbors.knn_cut_is_tied(c, x) for c, x in seen) for seen in visited]
     parted = [b for b in range(len(structs)) if dpos[b] > 1e-5]
     ops.TIMER = ops.KernelTimer()
     try:
@@ -142,12 +167,21 @@ def main():
         summ = ops.TIMER.summary()
     finally:
         ops.TIMER = None
-    evals = a.steps + 1
+    evals = (2 if npt else 1) * a.steps + 1
+    if npt:
+        C = got.cells.cpu().numpy()
+        cells_out = dict(cell_moved_max_A=float(np.abs(C[-1] - C[0]).max()),
+                         max_cell_difference_A=max(float(np.abs(C[-1, b] - r["cell"]).max()) for b, r in enumerate(ref)),
+                         mean_pressure_eV_A3=dict(first=float(got.pressure[0].mean()), last=float(got.pressure[-1].mean())),
+                         target_pressure_eV_A3=NO.pressure_au(a.pressure_bar))
+    else:
+        cells_out = {}
     split = {k[len("md_"):]: round(summ[k]["total_ms"] / evals, 3) for k in summ if k.startswith("md_")}
     med_b, med_p = statistics.median(ms["batched"]), statistics.median(ms["per_crystal"])
     out = dict(workload=f"{len(structs)} jittered sample structures ({sum(sizes)} atoms), ALIGNNAtomWise 4+4 d=256, "
                         f"k-nearest 8 A / 12, {a.ensemble} 300 K from Maxwell-Boltzmann 300 K, 1 fs, {a.steps} steps "
-                        f"({evals} evaluations per crystal)",
+                        f"({evals} evaluations per crystal)"
+                        + (f", {a.pressure_bar} bar, compressibility {a.compressibility} / bar" if npt else ""),
                batched_ms=[round(v, 1) for v in ms["batched"]], batched_ms_median=round(med_b, 1),
                per_crystal_ms=[round(v, 1) for v in ms["per_crystal"]], per_crystal_ms_median=round(med_p, 1),
                speedup_median=round(med_p / med_b, 2), batched_ms_per_evaluation_split=split,
@@ -158,6 +192,7 @@ def main():
                max_difference_on_crystals_without_a_tie_A=max([dpos[b] for b in range(len(structs)) if not tied[b]],
                                                                default=0.0),
                mean_temperature_K=dict(first=round(float(T[0].mean()), 1), last=round(float(T[-1].mean()), 1)),
+               **cells_out,
                device=device_info())
     print(json.dumps(out))
 
