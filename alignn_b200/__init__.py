@@ -9,5 +9,5 @@ __version__ = "0.1.0"
 from .graph import Graph, batch, unbatch, reverse, graph, as_graph, bond_cosines  # noqa: F401
 from .ealignn_atomwise import eALIGNNAtomWise, eALIGNNAtomWiseConfig  # noqa: F401,E402
 from .relax import relax_structures, RelaxResult, CellRelaxResult  # noqa: F401,E402
-from .md import run_md, maxwell_boltzmann_momenta, MDResult, NPTResult  # noqa: F401,E402
+from .md import run_md, maxwell_boltzmann_momenta, upper_triangular, MDResult, NPTResult  # noqa: F401,E402
 from .phonons import phonons, PhononResult  # noqa: F401,E402

@@ -136,6 +136,11 @@ class MdNptParams(C.Structure):
                 ("stress_wt", C.c_float)]
 
 
+class MdNoseHooverParams(C.Structure):
+    _fields_ = [("dt", C.c_double), ("kB", C.c_double), ("evaluation", C.c_int32), ("steps", C.c_int32),
+                ("force_multiplier", C.c_float), ("stress_wt", C.c_float)]
+
+
 class MdThermostatParams(C.Structure):
     _fields_ = [("dt", C.c_double), ("kB", C.c_double), ("friction", C.c_double), ("andersen_prob", C.c_double),
                 ("sqrt_dt", C.c_double), ("dt_1_5", C.c_double), ("two_sqrt3", C.c_double), ("evaluation", C.c_int32),
@@ -218,6 +223,8 @@ _SIGNATURES = {
                                                  _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
     "alignn_b200_md_npt_step": (C.c_int, [C.POINTER(MdNptParams), _fp, C.c_int64, _fp, C.c_int64, _fp, _fp, _fp, _fp, _fp,
                                           _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
+    "alignn_b200_md_nose_hoover_step": (C.c_int, [C.POINTER(MdNoseHooverParams), _fp, C.c_int64, _fp, C.c_int64]
+                                        + [_fp] * 19),
     "alignn_b200_md_noise": (C.c_int, [C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, C.c_int64, C.c_int32, _fp, _fp, _fp,
                                        _fp]),
     "alignn_b200_phonon_force_constants": (C.c_int, [_fp, C.c_double, C.c_float, _fp, C.c_int64, _fp, _fp, C.c_int64, _fp,

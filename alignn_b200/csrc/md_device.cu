@@ -24,6 +24,10 @@
 // `ForceField.run_npt_berendsen` (alignn/ff/ff.py:545-582) runs: the Berendsen thermostat above plus a barostat that
 // rescales each crystal's cell and positions every step on the calculator's stress; oracle/md_npt_oracle.py is its
 // specification.
+//
+// md_nose_hoover_kernel runs ASE 3.22.1's `NPT` (Nose-Hoover thermostat and Parrinello-Rahman barostat;
+// ase/md/npt.py), which `ForceField.run_npt_nose_hoover` (alignn/ff/ff.py:584-617) runs: a central difference in
+// fractional coordinates, one model evaluation per step; oracle/md_nose_hoover_oracle.py is its specification.
 #include <math.h>
 #include <stdint.h>
 
@@ -562,6 +566,350 @@ md_npt_step_kernel(const alignn_b200_md_npt_params p, const int64_t* __restrict_
   }
 }
 
+// ---- ASE's NPT (Nose-Hoover / Parrinello-Rahman).  Row vectors times row-major 3 x 3 matrices, every product and sum
+// rounded on its own in a fixed order (no contraction), so the result depends on the operands only.
+__device__ __forceinline__ void vec_mat3(const double v[3], const double* M, double out[3]) {
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+    out[k] = __dadd_rn(__dadd_rn(__dmul_rn(v[0], M[k]), __dmul_rn(v[1], M[3 + k])), __dmul_rn(v[2], M[6 + k]));
+}
+
+__device__ __forceinline__ void mat3_mul(const double* A, const double* B, double* out) {
+#pragma unroll
+  for (int i = 0; i < 3; ++i) vec_mat3(A + 3 * i, B, out + 3 * i);
+}
+
+__device__ __forceinline__ double det3(const double* A) {
+  const double c0 = __dsub_rn(__dmul_rn(A[4], A[8]), __dmul_rn(A[5], A[7]));
+  const double c1 = __dsub_rn(__dmul_rn(A[3], A[8]), __dmul_rn(A[5], A[6]));
+  const double c2 = __dsub_rn(__dmul_rn(A[3], A[7]), __dmul_rn(A[4], A[6]));
+  return __dadd_rn(__dsub_rn(__dmul_rn(A[0], c0), __dmul_rn(A[1], c1)), __dmul_rn(A[2], c2));
+}
+
+// A^-1 = adj(A) / det, det = det3(A) finite and nonzero
+__device__ __forceinline__ void inv3(const double* A, double det, double* out) {
+  const double adj[9] = {__dsub_rn(__dmul_rn(A[4], A[8]), __dmul_rn(A[5], A[7])),
+                         __dsub_rn(__dmul_rn(A[2], A[7]), __dmul_rn(A[1], A[8])),
+                         __dsub_rn(__dmul_rn(A[1], A[5]), __dmul_rn(A[2], A[4])),
+                         __dsub_rn(__dmul_rn(A[5], A[6]), __dmul_rn(A[3], A[8])),
+                         __dsub_rn(__dmul_rn(A[0], A[8]), __dmul_rn(A[2], A[6])),
+                         __dsub_rn(__dmul_rn(A[2], A[3]), __dmul_rn(A[0], A[5])),
+                         __dsub_rn(__dmul_rn(A[3], A[7]), __dmul_rn(A[4], A[6])),
+                         __dsub_rn(__dmul_rn(A[1], A[6]), __dmul_rn(A[0], A[7])),
+                         __dsub_rn(__dmul_rn(A[0], A[4]), __dmul_rn(A[1], A[3]))};
+#pragma unroll
+  for (int k = 0; k < 9; ++k) out[k] = __ddiv_rn(adj[k], det);
+}
+
+__device__ __forceinline__ bool finite_nonzero(double v) { return isfinite(v) && v != 0.0; }
+
+// the state row of a crystal (ALIGNN_B200_MD_NH_STATE doubles): h_past, eta, eta_past (row-major 3 x 3), zeta, zeta_past
+enum { kHPast = 0, kEta = 9, kEtaPast = 18, kZeta = 27, kZetaPast = 28 };
+// the per-crystal matrices in shared memory
+enum { kH = 0, kInvH = 9, kBetaM = 18, kInvBetaP = 27, kHs = 36, kHFut = 45, kMats = 54 };
+
+// _calculate_q_future for one atom: alpha = (dt dt) ((F/m) h^-1); q_future = (2q + q_past (beta - I) + alpha)(beta + I)^-1
+__device__ __forceinline__ void nh_q_future(const double* M, double dt2, const double f[3], double m, const double q[3],
+                                            const double qp[3], double out[3]) {
+  double fm[3], alpha[3], qb[3], s[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) fm[k] = __ddiv_rn(f[k], m);
+  vec_mat3(fm, M + kInvH, alpha);
+  vec_mat3(qp, M + kBetaM, qb);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) s[k] = __dadd_rn(__dadd_rn(__dmul_rn(2.0, q[k]), qb[k]), __dmul_rn(dt2, alpha[k]));
+  vec_mat3(s, M + kInvBetaP, out);
+}
+
+// p = ((q_future - q_past) (h / (2 dt))) m
+__device__ __forceinline__ void nh_momenta(const double* M, const double qf[3], const double qp[3], double m,
+                                           double p[3]) {
+  const double d[3] = {__dsub_rn(qf[0], qp[0]), __dsub_rn(qf[1], qp[1]), __dsub_rn(qf[2], qp[2])};
+  vec_mat3(d, M + kHs, p);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) p[k] = __dmul_rn(p[k], m);
+}
+
+// q_past = q - dt ((p/m) h^-1)
+__device__ __forceinline__ void nh_q_past(const double* M, double dt, const double q[3], const double p[3], double m,
+                                          double out[3]) {
+  const double v[3] = {__ddiv_rn(p[0], m), __ddiv_rn(p[1], m), __ddiv_rn(p[2], m)};
+  double w[3];
+  vec_mat3(v, M + kInvH, w);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) out[k] = __dsub_rn(q[k], __dmul_rn(dt, w[k]));
+}
+
+// ASE 3.22.1's `NPT` (ase/md/npt.py, mask None, frac_traceless 1), which `ForceField.run_npt_nose_hoover`
+// (alignn/ff/ff.py:584-617) runs; oracle/md_nose_hoover_oracle.py is its specification.  One launch per evaluation e,
+// one CTA per crystal.  Thread 0 forms the crystal's matrices (h, h^-1, beta - I, (beta + I)^-1, h / (2 dt) and, for
+// e < steps, h_future) in shared memory and checks them before anything is written:
+//   e == 0: p -= sum_i p_i / n (zero_center_of_mass_momentum); initialize(): q = r h^-1 - 0.5 and the two passes of
+//           _calculate_q_past_and_future on the forces F of this evaluation -- pass 1 from p0, its mean kinetic energy
+//           per atom (a block reduction), and below 1e-5 eV the first pass stands, else pass 2 from 2 p0 - p'.
+//           The atoms keep p0; q_future goes to the second per-atom array.
+//   e >= 1: the end of step e: that array holds q_past; q_future from F, then p = ((q_future - q_past)(h/(2dt))) m.
+//   always: the forces, ekin, T, the calculator's stress and the ideal-gas pressure, as md_npt_step_kernel logs them.
+//   e < steps: the start of step e + 1 on this evaluation's ideal-gas-corrected stress s and kinetic energy (for e = 0
+//           the past values come from initialize(): h_past = h - dt h eta, eta_past = eta - U(-dt pfact det h (s - s_ext)),
+//           zeta_past = zeta - dt tfact (ekin - desiredEkin)): h_future = h_past + 2dt h eta, eta_future = eta_past +
+//           U(-2dt (pfact det h (s - s_ext))) (U(0) when pfact = 0: pfactor None, s unread), zeta_future = zeta_past +
+//           2dt tfact (ekin - desiredEkin); the shift; q_past <-> q swapped between the two arrays; r = (q + 0.5) h_future.
+// Status 3: the slice is outside grad, or (e == 0) h is not upper triangular.  Status 4: det h, det(beta + I) or, for
+// e < steps, det h_future is not finite and nonzero.  Nothing of the crystal is written then, nor in later launches.
+__global__ void __launch_bounds__(kBlock)
+md_nose_hoover_kernel(const alignn_b200_md_nose_hoover_params p, const int64_t* __restrict__ atom_off,
+                      const float* __restrict__ grad, int64_t grad_rows, const float* __restrict__ stress,
+                      const double* __restrict__ masses, const double* __restrict__ tfact,
+                      const double* __restrict__ pfact, const double* __restrict__ desired_ekin,
+                      const double* __restrict__ ext_stress, double* __restrict__ cells, double* __restrict__ state,
+                      double* __restrict__ x, double* __restrict__ mom, double* __restrict__ qa,
+                      double* __restrict__ qb, float* __restrict__ forces, float* __restrict__ stress_out,
+                      double* __restrict__ ekin_out, double* __restrict__ temp_out, double* __restrict__ press_out,
+                      int32_t* __restrict__ status) {
+  __shared__ double red[kBlock][3];
+  __shared__ double M[kMats];
+  __shared__ double sh_det;
+  __shared__ int verdict;
+  const int64_t c = blockIdx.x;
+  if (status[c] != kOk) return;
+  const int64_t g0 = atom_off[c], n = atom_off[c + 1] - g0;
+  if (g0 < 0 || n < 1 || atom_off[c + 1] > grad_rows) {
+    if (threadIdx.x == 0) status[c] = kBadInput;
+    return;
+  }
+  const int t = threadIdx.x;
+  const double dt = p.dt;
+  const bool init = p.evaluation == 0, step = p.evaluation < p.steps;
+  double* st = state + ALIGNN_B200_MD_NH_STATE * c;
+  if (t == 0) {
+    int v = kOk;
+    double h[9], E[9], T1[9], beta[9];
+#pragma unroll
+    for (int k = 0; k < 9; ++k) h[k] = cells[9 * c + k];
+    if (init && !(h[3] == 0.0 && h[6] == 0.0 && h[7] == 0.0)) v = kBadInput;
+    const double det = det3(h);
+    if (v == kOk && !finite_nonzero(det)) v = kCellDegenerate;
+    if (v == kOk) {
+      inv3(h, det, M + kInvH);
+      // beta = dt (h ((eta + (0.5 zeta) I) h^-1))
+      const double hz = __dmul_rn(0.5, st[kZeta]);
+#pragma unroll
+      for (int k = 0; k < 9; ++k) E[k] = __dadd_rn(st[kEta + k], (k % 4 == 0) ? hz : 0.0);
+      mat3_mul(E, M + kInvH, T1);
+      mat3_mul(h, T1, beta);
+      double bp[9];
+#pragma unroll
+      for (int k = 0; k < 9; ++k) {
+        const double b = __dmul_rn(dt, beta[k]);
+        M[kBetaM + k] = __dsub_rn(b, (k % 4 == 0) ? 1.0 : 0.0);
+        bp[k] = __dadd_rn(b, (k % 4 == 0) ? 1.0 : 0.0);
+      }
+      const double detb = det3(bp);
+      if (!finite_nonzero(detb)) v = kCellDegenerate;
+      else inv3(bp, detb, M + kInvBetaP);
+      const double two_dt = __dmul_rn(2.0, dt);
+#pragma unroll
+      for (int k = 0; k < 9; ++k) {
+        M[kH + k] = h[k];
+        M[kHs + k] = __ddiv_rn(h[k], two_dt);
+      }
+      if (step) {                                               // h_future = h_past + 2dt (h eta)
+        double he[9];
+        mat3_mul(h, st + kEta, he);
+#pragma unroll
+        for (int k = 0; k < 9; ++k) {
+          const double hp = init ? __dsub_rn(h[k], __dmul_rn(dt, he[k])) : st[kHPast + k];
+          M[kHFut + k] = __dadd_rn(hp, __dmul_rn(two_dt, he[k]));
+        }
+        if (!finite_nonzero(det3(M + kHFut))) v = kCellDegenerate;
+      }
+    }
+    sh_det = det;
+    verdict = v;
+  }
+  __syncthreads();
+  if (verdict != kOk) {
+    if (t == 0) status[c] = verdict;
+    return;
+  }
+  const double det = sh_det;
+  const double dt2 = __dmul_rn(dt, dt);
+  const float* gr = grad + 3 * g0;
+  const double* mc = masses + g0;
+  double* xc = x + 3 * g0;
+  double* pc = mom + 3 * g0;
+  double* qac = qa + 3 * g0;
+  double* qbc = qb + 3 * g0;
+  float* fc = forces + 3 * g0;
+  double tot[3];
+
+  // ---- the momenta of this evaluation, their kinetic energy and ideal-gas sums
+  double mean[3] = {0.0, 0.0, 0.0};
+  if (init) {                                                   // zero_center_of_mass_momentum: p - p.sum(0) / n
+    double s[3] = {0.0, 0.0, 0.0};
+    for (int64_t i = t; i < n; i += kBlock) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) s[k] = __dadd_rn(s[k], pc[3 * i + k]);
+    }
+    block_sum3(red, s[0], s[1], s[2], tot);
+    const double nd = (double)n;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) mean[k] = __ddiv_rn(tot[k], nd);
+  }
+  double kin = 0.0, g[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0}, e1 = 0.0;
+  for (int64_t i = t; i < n; i += kBlock) {
+    const double m = mc[i];
+    double f[3], pv[3], q[3], qp[3], qf[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const float fv = __fmul_rn(gr[3 * i + k], p.force_multiplier);
+      fc[3 * i + k] = fv;
+      f[k] = fv;
+    }
+    if (init) {
+      double r[3];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        pv[k] = __dsub_rn(pc[3 * i + k], mean[k]);
+        pc[3 * i + k] = pv[k];
+        r[k] = xc[3 * i + k];
+      }
+      vec_mat3(r, M + kInvH, q);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        q[k] = __dsub_rn(q[k], 0.5);
+        qac[3 * i + k] = q[k];
+      }
+      double p1[3];                                             // the first pass
+      nh_q_past(M, dt, q, pv, m, qp);
+      nh_q_future(M, dt2, f, m, q, qp, qf);
+      nh_momenta(M, qf, qp, m, p1);
+      e1 = __dadd_rn(e1, __ddiv_rn(__dadd_rn(__dadd_rn(__dmul_rn(p1[0], p1[0]), __dmul_rn(p1[1], p1[1])),
+                                             __dmul_rn(p1[2], p1[2])), m));
+    } else {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        q[k] = qac[3 * i + k];
+        qp[k] = qbc[3 * i + k];
+      }
+      nh_q_future(M, dt2, f, m, q, qp, qf);
+      nh_momenta(M, qf, qp, m, pv);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) pc[3 * i + k] = pv[k];
+    }
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      qbc[3 * i + k] = qf[k];
+      kin = __dadd_rn(kin, __dmul_rn(pv[k], __ddiv_rn(pv[k], m)));
+    }
+    add_ideal_gas_terms(pv, __ddiv_rn(1.0, m), g);
+  }
+  double G[6], rest[3];
+  block_sum3(red, kin, g[0], g[1], tot);
+  block_sum3(red, g[2], g[3], g[4], G + 2);
+  block_sum3(red, g[5], e1, 0.0, rest);
+  G[0] = tot[1];
+  G[1] = tot[2];
+  G[5] = rest[0];
+
+  // ---- initialize(): the second pass unless the first one's 0.5 sum(p'^2 / m) / n is below 1e-5 eV
+  if (init && !(__ddiv_rn(__dmul_rn(0.5, rest[1]), (double)n) < 1e-5)) {
+    for (int64_t i = t; i < n; i += kBlock) {
+      const double m = mc[i];
+      double f[3], p0[3], q[3], qp[3], qf[3], p1[3];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        f[k] = fc[3 * i + k];
+        p0[k] = pc[3 * i + k];
+        q[k] = qac[3 * i + k];
+        qf[k] = qbc[3 * i + k];
+      }
+      nh_q_past(M, dt, q, p0, m, qp);                           // pass 1's q_past and p' again
+      nh_momenta(M, qf, qp, m, p1);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) p1[k] = __dadd_rn(__dsub_rn(p0[k], p1[k]), p0[k]);
+      nh_q_past(M, dt, q, p1, m, qp);
+      nh_q_future(M, dt2, f, m, q, qp, qf);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) qbc[3 * i + k] = qf[k];
+    }
+  }
+
+  // ---- the log rows
+  const double ekin = __dmul_rn(0.5, tot[0]);
+  const double T = __ddiv_rn(__dmul_rn(2.0, ekin), __dmul_rn((double)(3 * n), p.kB));
+  float sv[6], sc[6];
+  fire::calculator_stress(stress + 9 * c, p.stress_wt, sv);
+  const double P_log = corrected_pressure(sv, G, __ddiv_rn(1.0, fabs(det)), sc);
+  if (t == 0) {
+    ekin_out[c] = ekin;
+    temp_out[c] = T;
+    press_out[c] = P_log;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) stress_out[6 * c + k] = sv[k];
+  }
+  if (!step) return;
+
+  // ---- the start of step e + 1: the shift of q, and r = (q + 0.5) h_future
+  for (int64_t i = t; i < n; i += kBlock) {
+    double q[3], r[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      q[k] = qbc[3 * i + k];
+      qbc[3 * i + k] = qac[3 * i + k];                          // q_past = q
+      qac[3 * i + k] = q[k];                                    // q = q_future
+      q[k] = __dadd_rn(q[k], 0.5);
+    }
+    vec_mat3(q, M + kHFut, r);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) xc[3 * i + k] = r[k];
+  }
+  if (t == 0) {
+    const double pf = pfact[c], tf = tfact[c];
+    const double dE = __dsub_rn(ekin, desired_ekin[c]);
+    double de[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0}, de0[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    if (pf != 0.0) {                                            // pfactor given: the stress is read
+      const double a = __dmul_rn(pf, det), a0 = __dmul_rn(__dmul_rn(-dt, pf), det);
+#pragma unroll
+      for (int k = 0; k < 6; ++k) {
+        const double ds = __dsub_rn((double)sc[k], ext_stress[6 * c + k]);
+        de[k] = __dmul_rn(__dmul_rn(-2.0, dt), __dmul_rn(a, ds));
+        de0[k] = __dmul_rn(a0, ds);
+      }
+    }
+    // U(v) = [[v0, v5, v4], [0, v1, v3], [0, 0, v2]] as (row-major index, Voigt index) pairs
+    const int ui[6] = {0, 4, 8, 5, 2, 1};
+    double eta[9], eta_past[9], zeta = st[kZeta], zeta_past;
+#pragma unroll
+    for (int k = 0; k < 9; ++k) {
+      eta[k] = st[kEta + k];
+      eta_past[k] = st[kEtaPast + k];
+    }
+    if (init) {                                                 // initialize()'s past values
+#pragma unroll
+      for (int k = 0; k < 9; ++k) eta_past[k] = eta[k];
+#pragma unroll
+      for (int j = 0; j < 6; ++j) eta_past[ui[j]] = __dsub_rn(eta[ui[j]], de0[j]);
+      zeta_past = __dsub_rn(zeta, __dmul_rn(__dmul_rn(dt, tf), dE));
+    } else {
+      zeta_past = st[kZetaPast];
+    }
+#pragma unroll
+    for (int j = 0; j < 6; ++j) eta_past[ui[j]] = __dadd_rn(eta_past[ui[j]], de[j]);   // now eta_future
+    const double zeta_future = __dadd_rn(zeta_past, __dmul_rn(__dmul_rn(__dmul_rn(2.0, dt), tf), dE));
+#pragma unroll
+    for (int k = 0; k < 9; ++k) {
+      st[kHPast + k] = M[kH + k];
+      st[kEtaPast + k] = eta[k];
+      st[kEta + k] = eta_past[k];
+      cells[9 * c + k] = M[kHFut + k];
+    }
+    st[kZetaPast] = zeta;
+    st[kZeta] = zeta_future;
+  }
+}
+
 // the stream itself, for tests: item (a, j), a in [0, atoms), is block j of atom index atom0 + a (mod 2^32)
 __global__ void __launch_bounds__(kBlock)
 md_noise_kernel(uint64_t seed, uint32_t step, uint32_t tag, uint32_t atom0, int64_t items, int32_t blocks,
@@ -646,6 +994,30 @@ int alignn_b200_md_npt_step(const alignn_b200_md_npt_params* params, const int64
   md_npt_step_kernel<<<(unsigned)num_crystals, kBlock, 0, (cudaStream_t)stream>>>(
       p, atom_offsets, grad, grad_rows, stress, masses, target_temperature, target_pressure, compressibility, cells,
       positions, momenta, forces, stress_out, kinetic_energy, temperature, pressure, status);
+  return alignn::check_launch();
+}
+
+int alignn_b200_md_nose_hoover_step(const alignn_b200_md_nose_hoover_params* params, const int64_t* atom_offsets,
+                                    int64_t num_crystals, const float* grad, int64_t grad_rows, const float* stress,
+                                    const double* masses, const double* tfact, const double* pfact,
+                                    const double* desired_ekin, const double* external_stress, double* cells,
+                                    double* state, double* positions, double* momenta, double* q, double* q_future,
+                                    float* forces, float* stress_out, double* kinetic_energy, double* temperature,
+                                    double* pressure, int32_t* status, alignn_stream_t stream) {
+  using namespace alignn::md;
+  if (!params || num_crystals < 1 || num_crystals > INT32_MAX || grad_rows < 0) return ALIGNN_ERR_BAD_ARG;
+  const alignn_b200_md_nose_hoover_params p = *params;
+  const auto positive = [](double v) { return isfinite(v) && v > 0.0; };
+  if (p.steps < 1 || p.evaluation < 0 || p.evaluation > p.steps || !positive(p.dt) || !positive(p.kB) ||
+      !isfinite(p.force_multiplier) || !isfinite(p.stress_wt))
+    return ALIGNN_ERR_BAD_ARG;
+  if (!atom_offsets || !grad || !stress || !masses || !tfact || !pfact || !desired_ekin || !external_stress || !cells ||
+      !state || !positions || !momenta || !q || !q_future || !forces || !stress_out || !kinetic_energy || !temperature ||
+      !pressure || !status)
+    return ALIGNN_ERR_BAD_ARG;
+  md_nose_hoover_kernel<<<(unsigned)num_crystals, kBlock, 0, (cudaStream_t)stream>>>(
+      p, atom_offsets, grad, grad_rows, stress, masses, tfact, pfact, desired_ekin, external_stress, cells, state,
+      positions, momenta, q, q_future, forces, stress_out, kinetic_energy, temperature, pressure, status);
   return alignn::check_launch();
 }
 

@@ -13,6 +13,10 @@ and draw their noise from a counter-based stream keyed by each crystal's seed (c
 global RNG; `oracle/md_thermostat_oracle.py` is their specification.  NPT Berendsen (`ForceField.run_npt_berendsen`,
 alignn/ff/ff.py:545-582) moves the cells too: every step rebuilds the graphs from the rescaled cells, evaluates the
 model twice and launches `ops.md_npt_step` after each evaluation; `oracle/md_npt_oracle.py` is its specification.
+ASE's NPT (Nose-Hoover thermostat and Parrinello-Rahman barostat, `ForceField.run_npt_nose_hoover`, alignn/ff/ff.py:
+584-617) integrates in fractional coordinates with one model call and one `ops.md_nose_hoover_step` launch per step;
+`oracle/md_nose_hoover_oracle.py` is its specification, and `upper_triangular` rotates structures into the cell form it
+needs.
 """
 from __future__ import annotations
 
@@ -34,7 +38,7 @@ BAR = 1e5 * ((1 / _e) / 1e30)                  # ase.units: 1e5 * Pascal, the ba
 
 ENSEMBLES = {"nve_velocity_verlet": ops.MD_NVE, "nvt_berendsen": ops.MD_NVT_BERENDSEN,
              "nvt_langevin": ops.MD_NVT_LANGEVIN, "nvt_andersen": ops.MD_NVT_ANDERSEN,
-             "npt_berendsen": ops.MD_NPT_BERENDSEN}
+             "npt_berendsen": ops.MD_NPT_BERENDSEN, "npt_nose_hoover": ops.MD_NPT_NOSE_HOOVER}
 STOCHASTIC = (ops.MD_NVT_LANGEVIN, ops.MD_NVT_ANDERSEN)
 LANGEVIN_FRICTION = 1e-4      # ForceField.run_nvt_langevin's default friction, in 1 / ASE time unit
 NPT_TAUT = 49.11347394232032  # ForceField.run_npt_berendsen's taut literal: 500 fs in ASE units, bitwise
@@ -113,7 +117,8 @@ def run_md(model, structures, atom_features: torch.Tensor, masses, *, ensemble: 
            trajectory_interval: Optional[int] = None, neighbor_strategy: str = "k-nearest", cutoff: float = 8.0,
            max_neighbors: int = 12, cutoff_extra: float = 3.5, force_multiplier: float = 1.0,
            friction: Optional[float] = None, andersen_prob: float = 0.1, seed=None, pressure=None,
-           compressibility=None, taup: float = 1000.0, stress_wt: float = 1.0):
+           compressibility=None, taup: float = 1000.0, stress_wt: float = 1.0, externalstress=0.0,
+           ttime: Optional[float] = None, pfactor: Optional[float] = None):
     """Run `steps` steps of molecular dynamics on a batch of crystals, the cells fixed: a batched
     `ForceField.run_nve_velocity_verlet(steps=steps)` (ensemble="nve_velocity_verlet", ASE's VelocityVerlet) or
     `run_nvt_berendsen(temperature_K=..., taut=..., steps=steps)` (ensemble="nvt_berendsen", ASE's NVTBerendsen with
@@ -151,7 +156,21 @@ def run_md(model, structures, atom_features: torch.Tensor, masses, *, ensemble: 
     and after the drift (logged), so steps + 1 of the 2 steps + 1 evaluations are logged.  Returns an `NPTResult`: the
     MDResult fields plus the cell, the calculator's stress and the pressure of every logged evaluation.  A cell whose
     volume or scale factor stops being finite and > 0 raises RuntimeError naming the crystal and the step.  The
-    pressure keywords are ignored by the other ensembles."""
+    pressure keywords are ignored by the other ensembles.
+
+    NPT Nose-Hoover (ensemble="npt_nose_hoover"): `run_npt_nose_hoover(temperature_K=..., externalstress=...)`, ASE's
+    NPT -- Melchionna's Nose-Hoover thermostat with a Parrinello-Rahman barostat, a central difference in fractional
+    coordinates of the cell.  externalstress in eV/A^3 as ASE takes it (ForceField's 0.0): a number s (the stress
+    [-s, -s, -s, 0, 0, 0], i.e. a pressure s), a Voigt [6] (xx yy zz yz xz xy) or a symmetric [3,3] for every crystal,
+    or [B,6] / [B,3,3] per crystal.  ttime in fs and pfactor in ASE units (amu/A) switch on the thermostat and the
+    barostat; both default to None, which is the reference's call (it passes neither), so by default the thermostat and
+    barostat are off and the cells do not move.  ASE suggests ttime around 25 fs and pfactor = (ptime * FS)^2 * B, ptime
+    in fs (about 75 fs) and B the bulk modulus in eV/A^3.  taut is ignored here: ForceField computes it and never passes
+    it.  The model must compute stress.  ASE's NPT needs upper triangular cells (rows a, b, c with b in the yz-plane and
+    c along z): another cell raises ValueError naming the crystal; `upper_triangular` rotates structures into that form.
+    One model evaluation per step, all steps + 1 logged; returns an `NPTResult`.  A cell, or the matrix beta + I of the
+    update, that becomes singular or not finite raises RuntimeError naming the crystal and the step.  The other
+    ensembles ignore externalstress, ttime and pfactor."""
     _check_model("run_md", model)
     if ensemble not in ENSEMBLES:
         raise ValueError(f"ensemble must be one of {sorted(ENSEMBLES)}, got {ensemble!r}")
@@ -216,6 +235,13 @@ def run_md(model, structures, atom_features: torch.Tensor, masses, *, ensemble: 
                         graph=dict(neighbor_strategy=neighbor_strategy, cutoff=cutoff, max_neighbors=max_neighbors,
                                    cutoff_extra=cutoff_extra),
                         force_multiplier=float(force_multiplier))
+    if kind == ops.MD_NPT_NOSE_HOOVER:
+        return _run_nose_hoover(model, lats, Xs, atom_features, aoff, pos, mom, m_d, T0, dev, steps=int(steps), dt=dt,
+                                externalstress=externalstress, ttime=ttime, pfactor=pfactor, stress_wt=stress_wt,
+                                trajectory_interval=trajectory_interval,
+                                graph=dict(neighbor_strategy=neighbor_strategy, cutoff=cutoff,
+                                           max_neighbors=max_neighbors, cutoff_extra=cutoff_extra),
+                                force_multiplier=float(force_multiplier))
     forces = torch.zeros(N, 3, device=dev, dtype=torch.float32)
     energy = torch.zeros(steps + 1, B, device=dev, dtype=torch.float32)
     ekin = torch.zeros(steps + 1, B, device=dev, dtype=torch.float64)
@@ -356,5 +382,143 @@ def _run_npt(model, lats, Xs, atom_features, aoff, pos, mom, m_d, T0, dev, *, st
             ops.md_npt_step(grad, stress, aoff_d, m_d, T0, P0_d, comp_d, cells, pos, mom, forces, stress_log[e], ekin[e],
                             temp[e], press[e], status, evaluation=e, phase=1, **kw)
         read_back(e, 1, False)
+    return NPTResult(pos, mom, forces, energy, ekin, temp, aoff_d, torch.stack(traj) if traj else None, cell_log,
+                     stress_log, press)
+
+
+def upper_triangular(structures):
+    """Rotate each (lattice [3,3], cart_coords [n,3]) rigidly into the cell form ASE's NPT needs: rows a, b, c with c
+    along +z, b in the yz-plane (y > 0) and a free, so lattice[1,0] = lattice[2,0] = lattice[2,1] = 0 exactly.  Returns
+    (structures, rotations): the rotated (lattice @ R.T, cart_coords @ R.T) pairs and R [B,3,3], each a proper rotation
+    (orthogonal, det +1), so distances, angles and the energy are unchanged and forces and stresses rotate with R.
+    A cell that is already in this form comes back unchanged (R = I exactly)."""
+    out, rots = [], []
+    for b, (lat, X) in enumerate(structures):
+        L = np.asarray(lat, dtype=np.float64).reshape(3, 3)
+        X = np.asarray(X, dtype=np.float64).reshape(-1, 3)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            ez = L[2] / np.linalg.norm(L[2])
+            yb = L[1] - np.dot(L[1], ez) * ez
+            ey = yb / np.linalg.norm(yb)
+        R = np.stack([np.cross(ey, ez), ey, ez])
+        if not np.isfinite(R).all():
+            raise ValueError(f"upper_triangular: the lattice vectors b and c of crystal {b} are zero or parallel")
+        Lr = L @ R.T
+        Lr[1, 0] = Lr[2, 0] = Lr[2, 1] = 0.0
+        out.append((Lr, X @ R.T))
+        rots.append(R)
+    return out, np.stack(rots)
+
+
+def _external_stress(v, B: int) -> np.ndarray:
+    """ASE's NPT.set_stress for every crystal: [B,6] float64 Voigt (xx yy zz yz xz xy), eV/A^3."""
+    a = v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else v
+    try:
+        a = np.asarray(a, dtype=np.float64)
+    except (TypeError, ValueError):
+        a = None
+    if a is None or not np.isfinite(a).all() or a.shape not in ((), (6,), (3, 3), (B, 6), (B, 3, 3)):
+        raise ValueError(f"externalstress must be a finite number, a [6] or symmetric [3,3] array, or [{B},6] / "
+                         f"[{B},3,3] per crystal (eV/A^3), got {v!r}")
+    if a.ndim == 0:
+        s = float(a)
+        return np.tile(np.array([-s, -s, -s, 0.0, 0.0, 0.0]), (B, 1))
+    if a.shape[-2:] == (3, 3):
+        m = a.reshape(-1, 3, 3)
+        if not all((x - x.T).max() < 1e-10 for x in m):
+            raise ValueError("externalstress: the external stress must be a symmetric tensor")
+        a = np.stack([m[:, 0, 0], m[:, 1, 1], m[:, 2, 2], m[:, 1, 2], m[:, 0, 2], m[:, 0, 1]], axis=1)
+    return np.array(np.broadcast_to(a.reshape(-1, 6), (B, 6)), order="C")
+
+
+def _nose_hoover_constants(sizes, T0, ttime, pfactor, cells):
+    """ASE's NPT._calculateconstants per crystal, in numpy as ASE computes them: (tfact, pfact, desiredEkin) lists for n
+    atoms, kT = kB T0, ttime in ASE time units and pfactor in ASE units (None: 0), pfact frozen at the initial cell."""
+    tf, pf, de = [], [], []
+    for n, t, h in zip(sizes, T0, cells):
+        n, kT = int(n), KB * float(t)
+        tf.append(0.0 if ttime is None else 2.0 / (3 * n * kT * ttime * ttime))
+        pf.append(0.0 if pfactor is None else 1.0 / (pfactor * np.linalg.det(np.asarray(h, dtype=np.float64))))
+        de.append(1.5 * (n - 1) * kT)
+    return tf, pf, de
+
+
+def _run_nose_hoover(model, lats, Xs, atom_features, aoff, pos, mom, m_d, T0, dev, *, steps, dt, externalstress,
+                     ttime, pfactor, stress_wt, trajectory_interval, graph, force_multiplier) -> NPTResult:
+    """run_md's loop for ASE's NPT: per evaluation e one graph build on the current cells, the model with stress and one
+    `md_nose_hoover_step` launch (see csrc/md_device.cu)."""
+    B, N = len(Xs), int(aoff[-1])
+    if model.config.stresswise_weight == 0:
+        raise ValueError("run_md(ensemble='npt_nose_hoover') needs a model that computes stress (stresswise_weight != 0)")
+    for b, lat in enumerate(lats):
+        if not lat[1, 0] == lat[2, 0] == lat[2, 1] == 0.0:
+            raise ValueError(f"run_md(ensemble='npt_nose_hoover'): the cell of crystal {b} is not upper triangular; ASE's "
+                             "NPT needs lattice rows a, b, c with b in the yz-plane and c along z "
+                             "(alignn_b200.upper_triangular rotates structures into that form)")
+    if ttime is not None and not (_real(ttime) and ttime > 0):
+        raise ValueError(f"ttime must be None or a finite number > 0 (fs), got {ttime!r}")
+    if pfactor is not None and not (_real(pfactor) and pfactor > 0):
+        raise ValueError(f"pfactor must be None or a finite number > 0 (ASE units, amu/A), got {pfactor!r}")
+    if not _real(stress_wt):
+        raise ValueError(f"stress_wt must be a finite real number, got {stress_wt!r}")
+    if externalstress is None and pfactor is not None:
+        raise ValueError("run_md(ensemble='npt_nose_hoover'): pfactor needs an externalstress")
+    ext = _external_stress(0.0 if externalstress is None else externalstress, B)
+    tf, pf, de = _nose_hoover_constants(np.diff(aoff), T0.cpu().tolist(), None if ttime is None else float(ttime) * FS,
+                                        None if pfactor is None else float(pfactor), lats)
+    f64 = dict(dtype=torch.float64, device=dev)
+    tf_d, pf_d, de_d = (torch.tensor(v, **f64) for v in (tf, pf, de))
+    ext_d = torch.from_numpy(ext).to(dev)
+    cells = torch.from_numpy(np.ascontiguousarray(np.stack(lats))).to(dev)
+    state = torch.zeros(B, ops.MD_NH_STATE, **f64)
+    q, q_future = torch.zeros(N, 3, **f64), torch.zeros(N, 3, **f64)
+    forces = torch.zeros(N, 3, device=dev, dtype=torch.float32)
+    energy = torch.zeros(steps + 1, B, device=dev, dtype=torch.float32)
+    ekin, temp, press = (torch.zeros(steps + 1, B, **f64) for _ in range(3))
+    cell_log = torch.zeros(steps + 1, B, 3, 3, **f64)
+    stress_log = torch.zeros(steps + 1, B, 6, device=dev, dtype=torch.float32)
+    status = torch.zeros(B, device=dev, dtype=torch.int32)
+    aoff_d = torch.from_numpy(aoff).to(dev)
+    host_cells, host_pos = [np.array(c, dtype=np.float64) for c in lats], [x.copy() for x in Xs]
+    traj = []
+    for e in range(steps + 1):
+        with ops._span("md_build", 0):
+            g, lg, lat = neighbors.crystal_graphs_device(list(zip(host_cells, host_pos)), atom_features, device=dev,
+                                                         **graph)
+        with ops._span("md_model", 0):
+            with torch.enable_grad():
+                res = model((g, lg, lat))
+                grad, stress = _forces_and_stress_as_alone(model, g, res, B)
+            out = res["out"].detach().reshape(-1)
+            energy[e] = out * g.batch_num_nodes_on_device().to(out.dtype)
+        if trajectory_interval is not None and e % trajectory_interval == 0:
+            traj.append(pos.clone())
+        cell_log[e] = cells
+        with ops._span("md_step", 0):
+            ops.md_nose_hoover_step(grad, stress, aoff_d, m_d, tf_d, pf_d, de_d, ext_d, cells, state, pos, mom, q,
+                                    q_future, forces, stress_log[e], ekin[e], temp[e], press[e], status, evaluation=e,
+                                    steps=steps, dt=dt, kB=KB, force_multiplier=force_multiplier,
+                                    stress_wt=float(stress_wt))
+        with ops._span("md_readback", 0):
+            # one copy: the statuses and, unless this was the last evaluation, the next cells and positions
+            back = torch.cat([status.to(torch.float64)] +
+                             ([cells.reshape(-1), pos.reshape(-1)] if e < steps else [])).cpu().numpy()
+        st = back[:B]
+        if (st == ops.MD_BAD_INPUT).any():
+            raise RuntimeError("alignn_b200_md_nose_hoover_step: the model's forces do not match the crystals' atom "
+                               "counts")
+        bad = np.flatnonzero(st == ops.MD_CELL_DEGENERATE)
+        if bad.size:
+            raise RuntimeError(f"run_md: the cell of crystal {int(bad[0])} became degenerate in step {e + 1} (its "
+                               "determinant, or that of the update's beta + I, is not finite and nonzero)")
+        if (st != 0).any():
+            raise RuntimeError(f"run_md: the MD kernel reported statuses {st.astype(int).tolist()}")
+        if e == steps:
+            break
+        new_cells, new_pos = back[B:10 * B].reshape(B, 3, 3), back[10 * B:].reshape(-1, 3)
+        for b in range(B):
+            host_cells[b], host_pos[b] = new_cells[b], new_pos[aoff[b]:aoff[b + 1]]
+            if not np.isfinite(host_pos[b]).all():
+                raise RuntimeError(f"run_md: the positions of crystal {b} are not finite after step {e + 1}")
     return NPTResult(pos, mom, forces, energy, ekin, temp, aoff_d, torch.stack(traj) if traj else None, cell_log,
                      stress_log, press)

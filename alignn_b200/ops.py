@@ -647,6 +647,61 @@ def md_npt_step(grad: torch.Tensor, stress: torch.Tensor, atom_offsets: torch.Te
         temperature.data_ptr(), pressure.data_ptr(), status.data_ptr(), stream_ptr()), "alignn_b200_md_npt_step")
 
 
+MD_NPT_NOSE_HOOVER = 5            # run_md's code for ASE's NPT (its own kernel, alignn_b200_md_nose_hoover_step)
+MD_NH_STATE = 29                  # ALIGNN_B200_MD_NH_STATE: h_past, eta, eta_past (3 x 3 each), zeta, zeta_past
+
+
+@_on_tensor_device
+def md_nose_hoover_step(grad: torch.Tensor, stress: torch.Tensor, atom_offsets: torch.Tensor, masses: torch.Tensor,
+                        tfact: torch.Tensor, pfact: torch.Tensor, desired_ekin: torch.Tensor,
+                        external_stress: torch.Tensor, cells: torch.Tensor, state: torch.Tensor,
+                        positions: torch.Tensor, momenta: torch.Tensor, q: torch.Tensor, q_future: torch.Tensor,
+                        forces: torch.Tensor, stress_out: torch.Tensor, kinetic_energy: torch.Tensor,
+                        temperature: torch.Tensor, pressure: torch.Tensor, status: torch.Tensor, *, evaluation: int,
+                        steps: int, dt: float, kB: float, force_multiplier: float = 1.0, stress_wt: float = 1.0) -> None:
+    """Evaluation `evaluation` of an MD run of `steps` steps under ASE 3.22.1's `NPT` (Nose-Hoover thermostat and
+    Parrinello-Rahman barostat) for every crystal, in place, one launch (csrc/md_device.cu,
+    alignn_b200_md_nose_hoover_step): evaluation 0 initialises (centre-of-mass momentum removed, q from the positions,
+    q_future by ASE's two passes), a later one finishes its step (q_future and the momenta from its forces); then the
+    log rows, and unless evaluation == steps the start of the next step (cell, eta, zeta, the shift of q, the positions
+    of the next evaluation).
+
+    As `md_npt_step`, plus: tfact, pfact, desired_ekin [B] and external_stress [B,6] float64, the constants of ASE's
+    `NPT._calculateconstants` / `set_stress` (pfact 0 means no barostat; the stress then drives nothing); cells [B,3,3]
+    float64, upper triangular, advanced in place; state [B, MD_NH_STATE] float64 (zeroed before evaluation 0); q and
+    q_future [N,3] float64 workspaces the kernel owns between launches.  Status MD_BAD_INPUT also for a cell that is
+    not upper triangular at evaluation 0, MD_CELL_DEGENERATE for a singular or non-finite h, beta + I or next cell.
+    dt in ASE time units.  Enqueue only: the statuses are the caller's to read back."""
+    lib = _lib.load()
+    f64 = torch.float64
+    _md_operands("md_nose_hoover_step",
+                 [(grad, torch.float32), (stress, torch.float32), (atom_offsets, torch.int64), (masses, f64),
+                  (tfact, f64), (pfact, f64), (desired_ekin, f64), (external_stress, f64), (cells, f64), (state, f64),
+                  (positions, f64), (momenta, f64), (q, f64), (q_future, f64), (forces, torch.float32),
+                  (stress_out, torch.float32), (kinetic_energy, f64), (temperature, f64), (pressure, f64),
+                  (status, torch.int32)], grad.device)
+    B = atom_offsets.numel() - 1
+    N = positions.numel() // 3
+    if (B < 1 or positions.numel() != 3 * N or any(t.numel() != 3 * N for t in (momenta, q, q_future, forces))
+            or masses.numel() != N or stress.numel() != 9 * B or cells.numel() != 9 * B or stress_out.numel() != 6 * B
+            or external_stress.numel() != 6 * B or state.numel() != MD_NH_STATE * B
+            or any(t.numel() != B for t in (tfact, pfact, desired_ekin, kinetic_energy, temperature, pressure, status))
+            or grad.dim() != 2 or grad.shape[1] != 3 or grad.shape[0] > N):
+        raise ValueError("md_nose_hoover_step: inconsistent operand shapes")
+    if isinstance(steps, bool) or int(steps) != steps or not 1 <= int(steps) <= FIRE_MAX_STEPS:
+        raise ValueError(f"md_nose_hoover_step: steps must be an integer in [1, {FIRE_MAX_STEPS}], got {steps!r}")
+    if isinstance(evaluation, bool) or int(evaluation) != evaluation or not 0 <= int(evaluation) <= int(steps):
+        raise ValueError(f"md_nose_hoover_step: evaluation must be an integer in [0, steps], got {evaluation!r}")
+    p = _lib.MdNoseHooverParams(float(dt), float(kB), int(evaluation), int(steps), float(force_multiplier),
+                                float(stress_wt))
+    _lib.check(lib.alignn_b200_md_nose_hoover_step(
+        C.byref(p), atom_offsets.data_ptr(), B, grad.data_ptr(), grad.shape[0], stress.data_ptr(), masses.data_ptr(),
+        tfact.data_ptr(), pfact.data_ptr(), desired_ekin.data_ptr(), external_stress.data_ptr(), cells.data_ptr(),
+        state.data_ptr(), positions.data_ptr(), momenta.data_ptr(), q.data_ptr(), q_future.data_ptr(),
+        forces.data_ptr(), stress_out.data_ptr(), kinetic_energy.data_ptr(), temperature.data_ptr(),
+        pressure.data_ptr(), status.data_ptr(), stream_ptr()), "alignn_b200_md_nose_hoover_step")
+
+
 def md_noise(seed: int, step: int, count: int, *, tag: int = MD_NVT_LANGEVIN, atom0: int = 0, blocks: int = 1,
              device=None):
     """The thermostats' noise stream (csrc/md_noise.cuh) on the device, for tests: Philox block j of atom index

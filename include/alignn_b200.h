@@ -780,6 +780,57 @@ int alignn_b200_md_npt_step(const alignn_b200_md_npt_params* params, const int64
                             float* forces, float* stress_out, double* kinetic_energy, double* temperature,
                             double* pressure, int32_t* status, alignn_stream_t stream);
 
+/* Nose-Hoover / Parrinello-Rahman MD (csrc/md_device.cu): ASE 3.22.1's `NPT` (ase/md/npt.py: initialize,
+ * _calculate_q_past_and_future, _calculate_q_future, step; mask None, frac_traceless 1) -- what
+ * `ForceField.run_npt_nose_hoover` (alignn/ff/ff.py:584-617) runs one crystal at a time -- for a batch of crystals in
+ * lockstep, one model evaluation and one launch per step.  The state is kept in fractional coordinates q = r h^-1 - 0.5
+ * of the cell h (rows are the lattice vectors, upper triangular). */
+typedef struct {
+  double dt;                /* time step in ASE time units                                         */
+  double kB;                /* Boltzmann constant, eV/K (the logged temperature only)              */
+  int32_t evaluation;       /* e in [0, steps]: the evaluation whose grad and stress are passed   */
+  int32_t steps;            /* steps >= 1                                                          */
+  float force_multiplier;   /* F = fp32(grad * force_multiplier)                                   */
+  float stress_wt;          /* s = fp32(voigt(stress) * stress_wt / 160.21766208), as fire_cell     */
+} alignn_b200_md_nose_hoover_params;
+
+/* Doubles per crystal of the caller-owned state row: [0, 9) h_past, [9, 18) eta, [18, 27) eta_past (row-major 3 x 3),
+ * [27] zeta, [28] zeta_past.  The caller zeroes it before evaluation 0 (ASE starts from eta = 0, zeta = 0). */
+#define ALIGNN_B200_MD_NH_STATE 29
+
+/* One CTA per crystal c with status 0 (n atoms, masses m, cell h = cells[c], q and q_future rows of its atoms):
+ *   e == 0: p -= sum_i p_i / n; h must be upper triangular (h[1][0] == h[2][0] == h[2][1] == 0); q = r h^-1 - 0.5;
+ *   q_future by the two passes of ASE's initialize (the first alone if its mean kinetic energy per atom is below
+ *   1e-5 eV); the momenta stay p0.  e >= 1: q_future holds q_past on entry; q_future = (2q + q_past (beta - I) +
+ *   alpha)(beta + I)^-1 with alpha = dt^2 (F/m) h^-1, beta = dt h (eta + zeta/2 I) h^-1, and p = ((q_future - q_past)
+ *   (h / (2 dt))) m.  Every e: F = fp32(grad * force_multiplier) to forces, the calculator's fp32 Voigt stress s of
+ *   stress[c] to stress_out[c], kinetic_energy[c] and temperature[c] as alignn_b200_md_step, pressure[c] = -tr(s')/3
+ *   with s' the ideal-gas-corrected stress as alignn_b200_md_npt_step.  e < steps: the start of step e + 1 --
+ *   h_future = h_past + 2dt h eta, eta_future = eta_past + U(-2dt pfact det(h) (s' - external_stress[c])) (U(v) =
+ *   [[v0 v5 v4] [0 v1 v3] [0 0 v2]]; nothing when pfact[c] == 0, i.e. pfactor None), zeta_future = zeta_past +
+ *   2dt tfact[c] (ekin - desired_ekin[c]); the shift (for e == 0 the past values of ASE's initialize first); q and
+ *   q_future exchanged (q = q_future, q_future = q_past); cells[c] = h_future and positions r = (q + 0.5) h_future.
+ *   Status 3: the slice does not lie inside [0, grad_rows) or is empty, or (e == 0) h is not upper triangular.
+ *   Status 4: det h, det(beta + I) or (e < steps) det h_future is not finite and nonzero.  Either way nothing else is
+ *   read or written for c, and crystals with a nonzero status are not touched.  Sums are in double with fixed-order
+ *   block reductions; 3 x 3 inverses in closed form; no float atomics.
+ *   grad [grad_rows, 3] fp32; stress [num_crystals, 3, 3] fp32 (the model's, GPa); masses [>= grad_rows] double (amu);
+ *   tfact = 2 / (3 n kT ttime^2) or 0, pfact = 1 / (pfactor det h0) or 0, desired_ekin = 1.5 (n - 1) kT
+ *   [num_crystals] double and external_stress [num_crystals, 6] double (Voigt, eV/A^3), as ASE's NPT computes them;
+ *   cells [num_crystals, 3, 3] double; state [num_crystals, ALIGNN_B200_MD_NH_STATE] double; positions, momenta, q,
+ *   q_future [>= grad_rows, 3] double; forces [>= grad_rows, 3] fp32; stress_out [num_crystals, 6] fp32;
+ *   kinetic_energy / temperature / pressure [num_crystals] double (the caller passes row e of its logs); status
+ *   [num_crystals] int32.
+ * Rejected (ALIGNN_ERR_BAD_ARG, nothing enqueued): NULL params or a NULL array, num_crystals < 1, grad_rows < 0,
+ * steps < 1, evaluation outside [0, steps], dt or kB not finite and > 0, a non-finite force_multiplier or stress_wt. */
+int alignn_b200_md_nose_hoover_step(const alignn_b200_md_nose_hoover_params* params, const int64_t* atom_offsets,
+                                    int64_t num_crystals, const float* grad, int64_t grad_rows, const float* stress,
+                                    const double* masses, const double* tfact, const double* pfact,
+                                    const double* desired_ekin, const double* external_stress, double* cells,
+                                    double* state, double* positions, double* momenta, double* q, double* q_future,
+                                    float* forces, float* stress_out, double* kinetic_energy, double* temperature,
+                                    double* pressure, int32_t* status, alignn_stream_t stream);
+
 /* The thermostats' noise stream, for tests: item q = a * blocks + j (a in [0, atoms), j in [0, blocks)) is Philox block
  * j of atom index atom0 + a (mod 2^32) at (seed, step, tag): words [atoms*blocks, 4] uint32, its two uniforms
  * [atoms*blocks, 2] double and their Box-Muller normals [atoms*blocks, 2] double.  Rejected (ALIGNN_ERR_BAD_ARG):

@@ -12,13 +12,16 @@ NPT Berendsen (`--ensemble npt_berendsen`) runs ForceField's taut = 500 fs and t
 (default 1.01325 bar, one atmosphere: ASE's own NPTBerendsen example) with `--compressibility` (default 1e-6 / bar, a
 solid with a bulk modulus of 100 GPa); the reference passes neither, and its own call cannot run without them.  Its
 model is the same with `stresswise_weight=1` (the other ensembles keep the stress off, so their numbers stay
-comparable), and each step evaluates the model twice.
+comparable), and each step evaluates the model twice.  NPT Nose-Hoover (`--ensemble npt_nose_hoover`, ASE's NPT) runs
+the same structures rotated by `upper_triangular` into the cell form it needs, ForceField's externalstress 0 and
+`--ttime` (fs) / `--pfactor` (ASE units); both default to None, the reference's call, with thermostat and barostat off.
+Its model also computes stress, and each step evaluates it once.
 
   batched:     run_md -- per evaluation one device graph build, one model call and one integrator launch for the batch;
   per-crystal: for each crystal, every evaluation runs neighbors.crystal_graph on the host, .to("cuda"), the same model
                on a one-crystal batch, and the oracle's integrator step in numpy (oracle/md_oracle.py, or
                oracle/md_thermostat_oracle.py on the same restated noise stream; for NPT the graph is built on the
-               current cell and the integrator is oracle/md_npt_oracle.py).
+               current cell and the integrator is oracle/md_npt_oracle.py or oracle/md_nose_hoover_oracle.py).
 
 Each arm runs three times (alternating); the median wall time (ending in a synchronise) is reported.  One more batched
 run with CUDA events around its phases gives the per-evaluation split (build, model, step kernel, read-back; each span
@@ -27,8 +30,9 @@ final positions is reported, and per crystal whether its 12th-neighbour cut lies
 (`neighbors.knn_cut_is_tied`) at any structure the host arm evaluated: there rounding picks the images the k-nearest
 graph keeps, and the arms may part.  The device name, power limit and SM clock limit are read in the same run.
 
-    python tools/bench_md.py [--ensemble nvt_berendsen|nvt_langevin|nvt_andersen|npt_berendsen] [--structures 64]
-                             [--steps 50] [--seed 0] [--pressure-bar 1.01325] [--compressibility 1e-6]
+    python tools/bench_md.py [--ensemble nvt_berendsen|nvt_langevin|nvt_andersen|npt_berendsen|npt_nose_hoover]
+                             [--structures 64] [--steps 50] [--seed 0] [--pressure-bar 1.01325] [--compressibility 1e-6]
+                             [--ttime FS] [--pfactor AMU_PER_A]
 """
 import argparse
 import json
@@ -60,17 +64,20 @@ def main():
     ap.add_argument("--structures", type=int, default=64)
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--seed", type=int, default=0)
-    ap.add_argument("--ensemble", choices=("nvt_berendsen", "nvt_langevin", "nvt_andersen", "npt_berendsen"),
-                    default="nvt_berendsen")
+    ap.add_argument("--ensemble", default="nvt_berendsen",
+                    choices=("nvt_berendsen", "nvt_langevin", "nvt_andersen", "npt_berendsen", "npt_nose_hoover"))
     ap.add_argument("--pressure-bar", type=float, default=1.01325)
     ap.add_argument("--compressibility", type=float, default=1e-6, help="1/bar")
+    ap.add_argument("--ttime", type=float, default=None, help="fs (npt_nose_hoover; default None: no thermostat)")
+    ap.add_argument("--pfactor", type=float, default=None, help="amu/A (npt_nose_hoover; default None: no barostat)")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_md.py needs a CUDA device")
     import __graft_entry__
     __graft_entry__.build()
-    from alignn_b200 import maxwell_boltzmann_momenta, neighbors, ops, run_md
+    from alignn_b200 import maxwell_boltzmann_momenta, neighbors, ops, run_md, upper_triangular
     from alignn_b200.alignn_atomwise import ALIGNNAtomWise, ALIGNNAtomWiseConfig
+    from oracle import md_nose_hoover_oracle as NH
     from oracle import md_npt_oracle as NO
     from oracle import md_oracle as MO
     from oracle import md_thermostat_oracle as TO
@@ -80,12 +87,14 @@ def main():
     off = z["atom_offsets"]
     rng = np.random.default_rng(a.seed)
     pool = np.arange(len(z["ids"]))
-    npt = a.ensemble == "npt_berendsen"
+    npt, nh = a.ensemble == "npt_berendsen", a.ensemble == "npt_nose_hoover"
     if a.ensemble in ("nvt_langevin", "nvt_andersen"):         # Langevin (fixcm) rejects one-atom crystals
         pool = pool[off[1:] - off[:-1] >= 2]
     pick = rng.choice(pool, min(a.structures, len(pool)), replace=False)
     structs = [(z["lattices"][i], z["cart_coords"][off[i]:off[i + 1]] + rng.normal(scale=0.03, size=(off[i + 1] - off[i], 3)))
                for i in pick]
+    if nh:
+        structs, _ = upper_triangular(structs)
     sizes = [x.shape[0] for _, x in structs]
     aoff = np.concatenate([[0], np.cumsum(sizes)])
     feats = torch.from_numpy(rng.normal(size=(sum(sizes), 92)).astype(np.float32)).to(dev)
@@ -93,7 +102,8 @@ def main():
     p0 = maxwell_boltzmann_momenta(masses, 300.0, rng)
     torch.manual_seed(1)
     cfg = ALIGNNAtomWiseConfig(name="alignn_atomwise", alignn_layers=4, gcn_layers=4, hidden_features=256,
-                               atom_input_features=92, gradwise_weight=1.0, stresswise_weight=1.0 if npt else 0.0)
+                               atom_input_features=92, gradwise_weight=1.0,
+                               stresswise_weight=1.0 if npt or nh else 0.0)
     model = ALIGNNAtomWise(cfg).to(dev).eval()
     timestep, T0 = 1.0, 300.0
 
@@ -101,6 +111,8 @@ def main():
         extra = {} if a.ensemble == "nvt_berendsen" else dict(seed=a.seed)
         if npt:
             extra = dict(pressure=a.pressure_bar, compressibility=a.compressibility)
+        if nh:
+            extra = dict(ttime=a.ttime, pfactor=a.pfactor)
         r = run_md(model, structs, feats, masses, ensemble=a.ensemble, steps=a.steps, timestep=timestep,
                    temperature_K=T0, momenta=p0, **extra)
         torch.cuda.synchronize()
@@ -136,6 +148,10 @@ def main():
             if npt:
                 out.append(NO.run(evaluate_cell, lat, X, masses[sl], steps=a.steps, dt=dt, temperature_K=T0,
                                   pressure=a.pressure_bar, compressibility=a.compressibility, momenta=p0[sl]))
+            elif nh:
+                out.append(NH.run(evaluate_cell, lat, X, masses[sl], steps=a.steps, dt=dt, temperature_K=T0,
+                                  ttime=None if a.ttime is None else a.ttime * MO.fs, pfactor=a.pfactor,
+                                  momenta=p0[sl]))
             elif a.ensemble == "nvt_berendsen":
                 out.append(MO.run(evaluate, X, masses[sl], ensemble=MO.NVT_BERENDSEN, steps=a.steps, dt=dt,
                                   temperature_K=T0, taut=100 * dt, momenta=p0[sl]))
@@ -168,12 +184,12 @@ def main():
     finally:
         ops.TIMER = None
     evals = (2 if npt else 1) * a.steps + 1
-    if npt:
+    if npt or nh:
         C = got.cells.cpu().numpy()
         cells_out = dict(cell_moved_max_A=float(np.abs(C[-1] - C[0]).max()),
                          max_cell_difference_A=max(float(np.abs(C[-1, b] - r["cell"]).max()) for b, r in enumerate(ref)),
                          mean_pressure_eV_A3=dict(first=float(got.pressure[0].mean()), last=float(got.pressure[-1].mean())),
-                         target_pressure_eV_A3=NO.pressure_au(a.pressure_bar))
+                         **({"target_pressure_eV_A3": NO.pressure_au(a.pressure_bar)} if npt else {}))
     else:
         cells_out = {}
     split = {k[len("md_"):]: round(summ[k]["total_ms"] / evals, 3) for k in summ if k.startswith("md_")}
@@ -181,7 +197,8 @@ def main():
     out = dict(workload=f"{len(structs)} jittered sample structures ({sum(sizes)} atoms), ALIGNNAtomWise 4+4 d=256, "
                         f"k-nearest 8 A / 12, {a.ensemble} 300 K from Maxwell-Boltzmann 300 K, 1 fs, {a.steps} steps "
                         f"({evals} evaluations per crystal)"
-                        + (f", {a.pressure_bar} bar, compressibility {a.compressibility} / bar" if npt else ""),
+                        + (f", {a.pressure_bar} bar, compressibility {a.compressibility} / bar" if npt else "")
+                        + (f", upper-triangular cells, ttime {a.ttime} fs, pfactor {a.pfactor}" if nh else ""),
                batched_ms=[round(v, 1) for v in ms["batched"]], batched_ms_median=round(med_b, 1),
                per_crystal_ms=[round(v, 1) for v in ms["per_crystal"]], per_crystal_ms_median=round(med_p, 1),
                speedup_median=round(med_p / med_b, 2), batched_ms_per_evaluation_split=split,
