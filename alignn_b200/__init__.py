@@ -11,3 +11,4 @@ from .ealignn_atomwise import eALIGNNAtomWise, eALIGNNAtomWiseConfig  # noqa: F4
 from .relax import relax_structures, RelaxResult, CellRelaxResult  # noqa: F401,E402
 from .md import run_md, maxwell_boltzmann_momenta, upper_triangular, MDResult, NPTResult  # noqa: F401,E402
 from .phonons import phonons, PhononResult  # noqa: F401,E402
+from .eos import ev_curve, fit_eos, single_point, EOSFit, EVCurveResult, SinglePointResult  # noqa: F401,E402

@@ -231,6 +231,7 @@ _SIGNATURES = {
                                                      _fp, C.c_int64, _fp, _fp, _fp, _fp]),
     "alignn_b200_phonon_dynamical_matrix": (C.c_int, [_fp, C.c_int64, _fp, _fp, C.c_int64, C.c_int64, _fp, _fp, C.c_int64,
                                                       _fp, _fp, _fp]),
+    "alignn_b200_eos_fit": (C.c_int, [C.c_int32, _fp, _fp, C.c_int64, C.c_int32, _fp, _fp, _fp]),
     "alignn_b200_debug_egc_flags": (None, [C.c_int]),
     "alignn_b200_segment_mean": (C.c_int, [_fp, _fp, C.c_int64, C.c_int, _fp, _fp]),
     "alignn_b200_segment_mean_backward": (C.c_int, [_fp, _fp, C.c_int64, C.c_int, _fp, _fp]),

@@ -802,6 +802,35 @@ def phonon_dynamical_matrix(dynamical_matrix: torch.Tensor, fc_offsets: torch.Te
         stream_ptr()), "alignn_b200_phonon_dynamical_matrix")
 
 
+EOS_FORMS = {"murnaghan": 0, "birchmurnaghan": 1, "vinet": 2}    # ALIGNN_B200_EOS_*
+EOS_OK, EOS_OUTSIDE, EOS_NO_FIT, EOS_BAD_INPUT = 0, 1, 2, 3       # per-row statuses of eos_fit
+EOS_MAX_POINTS = 65536            # ALIGNN_B200_EOS_MAX_POINTS
+
+
+@_on_tensor_device
+def eos_fit(volumes: torch.Tensor, energies: torch.Tensor, params: torch.Tensor, status: torch.Tensor, *,
+            form: int) -> None:
+    """ASE 3.22.1's `EquationOfState(v, e, eos).fit()` for every row, one launch (csrc/eos_device.cu,
+    alignn_b200_eos_fit): the parabola seed, then Levenberg-Marquardt to the least-squares optimum.
+
+    volumes / energies [R, S] float64 (A^3, eV), S >= 4; params [R, 4] float64 (written: E0, B0 in eV/A^3, BP, V0);
+    status [R] int32 (written: EOS_OK, EOS_OUTSIDE -- V0 not strictly inside the volumes, parameters kept --,
+    EOS_NO_FIT or EOS_BAD_INPUT -- NaN parameters).  form is one of EOS_FORMS' values.  Enqueue only: the statuses are
+    the caller's to read back."""
+    lib = _lib.load()
+    _phonon_operands("eos_fit", [(volumes, torch.float64), (energies, torch.float64), (params, torch.float64),
+                                 (status, torch.int32)], volumes.device)
+    if (volumes.dim() != 2 or energies.shape != volumes.shape or params.shape != (volumes.shape[0], 4)
+            or status.shape != (volumes.shape[0],)):
+        raise ValueError("eos_fit: inconsistent operand shapes")
+    if form not in EOS_FORMS.values() or not 4 <= volumes.shape[1] <= EOS_MAX_POINTS:
+        raise ValueError(f"eos_fit: form must be one of {sorted(EOS_FORMS.values())} and the rows must have 4 to "
+                         f"{EOS_MAX_POINTS} points, got form={form!r}, {volumes.shape[1]} points")
+    _lib.check(lib.alignn_b200_eos_fit(int(form), volumes.data_ptr(), energies.data_ptr(), volumes.shape[0],
+                                       volumes.shape[1], params.data_ptr(), status.data_ptr(), stream_ptr()),
+               "alignn_b200_eos_fit")
+
+
 class _SegmentMean(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, gptr):

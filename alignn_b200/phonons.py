@@ -20,7 +20,7 @@ import torch
 
 from . import neighbors, ops
 from .md import _host_array, _real
-from .relax import _check_batch, _check_model, _forces_as_alone
+from .relax import _check_batch, _check_model, _evaluate_chunks
 
 # ase.units (ASE 3.22.1, CODATA 2014): Phonons.band_structure's s, sqrt(eV / A^2 / amu) -> eV
 _hbar = 6.626070040e-34 / (2 * math.pi)
@@ -167,25 +167,10 @@ def phonons(model, structures, atom_features: torch.Tensor, masses, *, supercell
         sets = [displaced_supercells(lat, x, sc, delta) for lat, x in zip(lats, Xs)]
         tiled = [atom_features[aoff[b]:aoff[b + 1]].repeat(Nc, 1) for b in range(B)]
     roff = neighbors.ragged_offsets([6 * n * Nc * n for n in sizes])
-    grad_all = torch.empty(int(roff[-1]), 3, device=dev, dtype=torch.float32)
     jobs = [(b, k) for b in range(B) for k in range(6 * sizes[b])]
-    row, j = 0, 0
-    while j < len(jobs):
-        chunk, atoms = [], 0
-        while j < len(jobs) and atoms + Nc * sizes[jobs[j][0]] <= max_batch_atoms:
-            chunk.append(jobs[j])
-            atoms += Nc * sizes[jobs[j][0]]
-            j += 1
-        with ops._span("phonon_build", 0):
-            feats = torch.cat([tiled[b] for b, _ in chunk])
-            g, lg, lat = neighbors.crystal_graphs_device([(sets[b][0], sets[b][1][k]) for b, k in chunk], feats,
-                                                         neighbor_strategy=neighbor_strategy, cutoff=cutoff,
-                                                         max_neighbors=max_neighbors, cutoff_extra=cutoff_extra, device=dev)
-        with ops._span("phonon_model", 0):
-            with torch.enable_grad():
-                res = model((g, lg, lat))
-                grad_all[row:row + atoms] = _forces_as_alone(model, g, res, len(chunk))
-        row += atoms
+    _, grad_all = _evaluate_chunks(model, [(sets[b][0], sets[b][1][k]) for b, k in jobs], lambda j: tiled[jobs[j][0]],
+                                   dev, neighbor_strategy=neighbor_strategy, cutoff=cutoff, max_neighbors=max_neighbors,
+                                   cutoff_extra=cutoff_extra, max_batch_atoms=max_batch_atoms, span="phonon")
 
     # ---- force constants: one launch
     foff = neighbors.ragged_offsets([Nc * 9 * n * n for n in sizes])

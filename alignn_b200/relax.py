@@ -141,6 +141,37 @@ def _forces_and_stress_as_alone(model, g, res, A: int):
     return grad, stress
 
 
+def _evaluate_chunks(model, structures, features, dev, *, neighbor_strategy, cutoff, max_neighbors, cutoff_extra,
+                     max_batch_atoms: int, span: str):
+    """One energy and force evaluation per structure, each as if alone: the structures are packed greedily, in order,
+    into model calls of at most max_batch_atoms atoms (every structure must fit in one), each call's graphs built on the
+    device.  features(j) is structure j's [n_j, F] atom features.  Returns (energy [J] fp32, out * natoms, and grad
+    [sum n_j, 3] fp32, the model's forces with the bond penalty counted once per structure, in structure order).
+    `span` prefixes the `ops._span` names of the graph build and the model call."""
+    sizes = [x.shape[0] for _, x in structures]
+    grad_all = torch.empty(sum(sizes), 3, device=dev, dtype=torch.float32)
+    energy = torch.empty(len(sizes), device=dev, dtype=torch.float32)
+    row, j = 0, 0
+    while j < len(sizes):
+        j0, atoms = j, 0
+        while j < len(sizes) and atoms + sizes[j] <= max_batch_atoms:
+            atoms += sizes[j]
+            j += 1
+        with ops._span(span + "_build", 0):
+            feats = torch.cat([features(k) for k in range(j0, j)])
+            g, lg, lat = neighbors.crystal_graphs_device(structures[j0:j], feats, neighbor_strategy=neighbor_strategy,
+                                                         cutoff=cutoff, max_neighbors=max_neighbors,
+                                                         cutoff_extra=cutoff_extra, device=dev)
+        with ops._span(span + "_model", 0):
+            with torch.enable_grad():
+                res = model((g, lg, lat))
+                grad_all[row:row + atoms] = _forces_as_alone(model, g, res, j - j0)
+            out = res["out"].detach().reshape(-1)                            # 0-d for a one-crystal batch
+            energy[j0:j] = out * g.batch_num_nodes_on_device().to(out.dtype)
+        row += atoms
+    return energy, grad_all
+
+
 def relax_structures(model, structures, atom_features: torch.Tensor, *, fmax: float = 0.1, steps: int = 100,
                      neighbor_strategy: str = "k-nearest", cutoff: float = 8.0, max_neighbors: int = 12,
                      cutoff_extra: float = 3.5, force_multiplier: float = 1.0, optimize_lattice: bool = False,

@@ -882,6 +882,31 @@ int alignn_b200_phonon_dynamical_matrix(const int32_t* supercell, int64_t modes,
                                         const int32_t* crystals, const double* qpoints, int64_t num_q, double* out,
                                         int32_t* status, alignn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Equation of state (csrc/eos_device.cu): ASE 3.22.1's `EquationOfState(v, e, eos).fit()` (ase/eos.py) -- what
+ * `ev_curve` (alignn/ff/ff.py:762-805) fits to one crystal's E(V) points -- for a batch of rows.  Device pointers,
+ * caller-owned buffers, enqueue-only on `stream`.
+ * ---------------------------------------------------------------------------------------- */
+#define ALIGNN_B200_EOS_MURNAGHAN 0         /* E0 + B0 V / BP ((V0/V)^BP / (BP - 1) + 1) - V0 B0 / (BP - 1) */
+#define ALIGNN_B200_EOS_BIRCH_MURNAGHAN 1   /* eta = (V0/V)^(1/3); E0 + 9 B0 V0 / 16 (eta^2-1)^2 (6 + BP (eta^2-1) - 4 eta^2) */
+#define ALIGNN_B200_EOS_VINET 2             /* eta = (V/V0)^(1/3); E0 + 2 B0 V0 / (BP-1)^2 (2 - (5 + 3 BP (eta-1) - 3 eta)
+                                               exp(-3 (BP-1)(eta-1) / 2)) */
+#define ALIGNN_B200_EOS_MAX_ITER 200        /* Levenberg-Marquardt iterations before a row is given up (status 2) */
+#define ALIGNN_B200_EOS_MAX_POINTS 65536    /* points of one row */
+
+/* One warp per row: volumes and energies [rows, points] double (A^3, eV); params [rows, 4] double written as ASE's
+ * (E0 eV, B0 eV/A^3, BP, V0 A^3); status [rows] int32.  Per row: the seed is ASE's -- the least-squares parabola
+ * a + b V + c V^2 (formed in a centred and scaled volume), vmin = -b / 2c, (parabola(vmin), 2 c vmin, 4, vmin) -- and
+ * the fit is Levenberg-Marquardt with the analytic Jacobian and MINPACK's diagonal scaling, run until the step and the
+ * cost decrease have both stalled at fp64 level.  Sums run in a fixed order, so a row's result is bitwise repeatable
+ * and independent of the other rows.  Status 0: ok.  1: V0 not strictly inside (min V, max V) -- ASE warns; the
+ * parameters are written.  2: no fit -- the seed is not finite (c = 0) or ALIGNN_B200_EOS_MAX_ITER iterations did not
+ * converge; NaN parameters.  3: a volume not finite and > 0 or an energy not finite; NaN parameters.
+ * Rejected (ALIGNN_ERR_BAD_ARG, nothing enqueued): an unknown form, rows < 0 or above 4 (2^31 - 1), points outside
+ * [4, ALIGNN_B200_EOS_MAX_POINTS], a NULL pointer.  rows = 0 enqueues nothing. */
+int alignn_b200_eos_fit(int32_t form, const double* volumes, const double* energies, int64_t rows, int32_t points,
+                        double* params, int32_t* status, alignn_stream_t stream);
+
 /* Per-graph mean over node rows (dgl.nn.AvgPooling, alignn.py:325) and its backward. */
 int alignn_b200_segment_mean(const float* x, const int32_t* graph_ptr /*[B+1]*/, int64_t B, int d, float* out,
                              alignn_stream_t stream);
