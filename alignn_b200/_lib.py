@@ -125,6 +125,17 @@ class FireCellParams(C.Structure):
     _fields_ = [("fire", FireParams), ("stress_wt", C.c_float)]
 
 
+class LbfgsParams(C.Structure):
+    _fields_ = [("maxstep", C.c_double), ("alpha", C.c_double), ("damping", C.c_double), ("fmax", C.c_double),
+                ("memory", C.c_int32), ("slots", C.c_int32), ("max_steps", C.c_int32), ("cell", C.c_int32),
+                ("force_multiplier", C.c_float), ("stress_wt", C.c_float)]
+
+
+class BfgsParams(C.Structure):
+    _fields_ = [("maxstep", C.c_double), ("alpha", C.c_double), ("fmax", C.c_double), ("max_steps", C.c_int32),
+                ("cell", C.c_int32), ("force_multiplier", C.c_float), ("stress_wt", C.c_float)]
+
+
 class MdParams(C.Structure):
     _fields_ = [("dt", C.c_double), ("taut", C.c_double), ("kB", C.c_double), ("evaluation", C.c_int32),
                 ("steps", C.c_int32), ("ensemble", C.c_int32), ("force_multiplier", C.c_float)]
@@ -217,6 +228,12 @@ _SIGNATURES = {
                                         _fp, _fp, _fp, _fp]),
     "alignn_b200_fire_cell_step": (C.c_int, [C.POINTER(FireCellParams), _fp, C.c_int64, _fp, _fp, C.c_int64, _fp, C.c_int64,
                                              _fp, C.c_int64, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
+    "alignn_b200_lbfgs_step": (C.c_int, [C.POINTER(LbfgsParams), _fp, C.c_int64, _fp, _fp, C.c_int64, _fp, C.c_int64, _fp,
+                                         C.c_int64] + [_fp] * 15 + [_fp]),
+    "alignn_b200_bfgs_update": (C.c_int, [C.POINTER(BfgsParams), _fp, C.c_int64, _fp, _fp, C.c_int64, C.c_int64, _fp,
+                                          C.c_int64, _fp, C.c_int64] + [_fp] * 16 + [_fp]),
+    "alignn_b200_bfgs_apply": (C.c_int, [C.POINTER(BfgsParams), _fp, C.c_int64, C.c_int64, _fp, _fp, _fp, C.c_int64,
+                                         C.c_int64] + [_fp] * 11 + [_fp]),
     "alignn_b200_md_step": (C.c_int, [C.POINTER(MdParams), _fp, C.c_int64, _fp, C.c_int64, _fp, _fp, _fp, _fp, _fp, _fp, _fp,
                                       _fp, _fp]),
     "alignn_b200_md_thermostat_step": (C.c_int, [C.POINTER(MdThermostatParams), _fp, C.c_int64, _fp, C.c_int64, _fp, _fp,

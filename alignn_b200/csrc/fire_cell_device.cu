@@ -16,18 +16,21 @@
 //   6. positions: x_i = Fn (F^-1 x_i + dr_i).
 // The filter state carried per crystal is C0, L = log F, F and C.  ASE re-derives L = logm(solve(C0, C).T) every step;
 // carrying it differs from that by rounding only.  Matrix exponentials: scaling and squaring of the degree-13 Pade
-// approximant, |A / 2^s|_1 <= 5.37 (Higham 2005), on shared memory.  No floating-point atomics: every result depends on
-// the crystal's own data and the fixed block size only, so it is bitwise repeatable and independent of the batch.
+// approximant, |A / 2^s|_1 <= 5.37 (Higham 2005), on shared memory (filter_common.cuh).  No floating-point atomics:
+// every result depends on the crystal's own data and the fixed block size only, so it is bitwise repeatable and
+// independent of the batch.
 #include <math.h>
 #include <stdint.h>
 
 #include "api_common.h"
 #include "alignn_b200.h"
-#include "fire_common.cuh"
+#include "filter_common.cuh"
 
 namespace alignn {
 namespace fire_cell {
 
+using filter::ExpmScratch;
+using filter::expm_block;
 using fire::div_rn;
 using fire::nan_max;
 
@@ -35,112 +38,6 @@ constexpr int kBlock = 256;
 enum { kRunning = 0, kConverged = 1, kExhausted = 2, kBadInput = 3, kCellDegenerate = 4 };   // istate[c][3]
 enum { kNsteps = 0, kFirst = 1, kTaken = 2, kStatus = 3 };      // istate columns
 enum { kFrozen = 0, kFirstStep = 1, kMix = 2, kReset = 3 };     // what the velocity pass does
-
-// shared scratch of one matrix exponential (n <= 6, row-major n x n)
-struct ExpmScratch {
-  double As[36], A2[36], A4[36], A6[36], X1[36], X2[36], X3[36];
-  double scale;
-  int s;
-};
-
-__device__ __forceinline__ double mm_entry(const double* A, const double* B, int n, int i, int j) {
-  double acc = 0.0;
-  for (int k = 0; k < n; ++k) acc += A[i * n + k] * B[k * n + j];
-  return acc;
-}
-
-// out = expm(A) for an n x n matrix in shared memory (n <= 6); every thread of the block calls it.  A and out must not
-// alias each other or the scratch.
-__device__ void expm_block(const double* A, int n, double* out, ExpmScratch& w) {
-  // Pade 13 coefficients b_0 .. b_13
-  constexpr double b0 = 64764752532480000.0, b1 = 32382376266240000.0, b2 = 7771770303897600.0,
-                   b3 = 1187353796428800.0, b4 = 129060195264000.0, b5 = 10559470521600.0, b6 = 670442572800.0,
-                   b7 = 33522128640.0, b8 = 1323241920.0, b9 = 40840800.0, b10 = 960960.0, b11 = 16380.0, b12 = 182.0,
-                   b13 = 1.0;
-  constexpr double theta13 = 5.371920351148152;
-  const int t = threadIdx.x, nn = n * n;
-  const int i = t / n, j = t - (t / n) * n;
-  const double eye = (i == j) ? 1.0 : 0.0;
-  if (t == 0) {
-    double norm = 0.0;                                          // 1-norm: the largest absolute column sum
-    for (int c = 0; c < n; ++c) {
-      double col = 0.0;
-      for (int r = 0; r < n; ++r) col += fabs(A[r * n + c]);
-      norm = nan_max(norm, col);
-    }
-    double sc = 1.0;
-    int s = 0;
-    while (norm > theta13 && s < 1000) {                        // halvings are exact; an infinite norm stops at 1000
-      norm *= 0.5;
-      sc *= 0.5;
-      ++s;
-    }
-    w.scale = sc;
-    w.s = s;
-  }
-  __syncthreads();
-  if (t < nn) w.As[t] = A[t] * w.scale;
-  __syncthreads();
-  if (t < nn) w.A2[t] = mm_entry(w.As, w.As, n, i, j);
-  __syncthreads();
-  if (t < nn) w.A4[t] = mm_entry(w.A2, w.A2, n, i, j);
-  __syncthreads();
-  if (t < nn) {
-    w.A6[t] = mm_entry(w.A4, w.A2, n, i, j);
-  }
-  __syncthreads();
-  if (t < nn) {
-    w.X1[t] = b13 * w.A6[t] + b11 * w.A4[t] + b9 * w.A2[t];
-    w.X2[t] = b12 * w.A6[t] + b10 * w.A4[t] + b8 * w.A2[t];
-  }
-  __syncthreads();
-  if (t < nn) {
-    w.X3[t] = mm_entry(w.A6, w.X1, n, i, j) + b7 * w.A6[t] + b5 * w.A4[t] + b3 * w.A2[t] + b1 * eye;
-    out[t] = mm_entry(w.A6, w.X2, n, i, j) + b6 * w.A6[t] + b4 * w.A4[t] + b2 * w.A2[t] + b0 * eye;   // V
-  }
-  __syncthreads();
-  if (t < nn) w.X1[t] = mm_entry(w.As, w.X3, n, i, j);                                                    // U
-  __syncthreads();
-  if (t < nn) {
-    const double u = w.X1[t], v = out[t];
-    w.X2[t] = v - u;                                            // Q = V - U
-    out[t] = v + u;                                             // P = V + U
-  }
-  __syncthreads();
-  if (t == 0) {                                                 // Q X = P: Gaussian elimination, partial pivoting
-    double* Q = w.X2;
-    for (int k = 0; k < n; ++k) {
-      int piv = k;
-      for (int r = k + 1; r < n; ++r)
-        if (fabs(Q[r * n + k]) > fabs(Q[piv * n + k])) piv = r;
-      if (piv != k) {
-        for (int c = 0; c < n; ++c) {
-          const double q = Q[k * n + c]; Q[k * n + c] = Q[piv * n + c]; Q[piv * n + c] = q;
-          const double p = out[k * n + c]; out[k * n + c] = out[piv * n + c]; out[piv * n + c] = p;
-        }
-      }
-      for (int r = k + 1; r < n; ++r) {
-        const double m = div_rn(Q[r * n + k], Q[k * n + k]);
-        for (int c = k + 1; c < n; ++c) Q[r * n + c] -= m * Q[k * n + c];
-        for (int c = 0; c < n; ++c) out[r * n + c] -= m * out[k * n + c];
-      }
-    }
-    for (int k = n - 1; k >= 0; --k) {
-      for (int c = 0; c < n; ++c) {
-        double acc = out[k * n + c];
-        for (int r = k + 1; r < n; ++r) acc -= Q[k * n + r] * out[r * n + c];
-        out[k * n + c] = div_rn(acc, Q[k * n + k]);
-      }
-    }
-  }
-  __syncthreads();
-  for (int q = 0; q < w.s; ++q) {                               // undo the scaling: s squarings
-    if (t < nn) w.X1[t] = mm_entry(out, out, n, i, j);
-    __syncthreads();
-    if (t < nn) out[t] = w.X1[t];
-    __syncthreads();
-  }
-}
 
 __global__ void __launch_bounds__(kBlock)
 fire_cell_step_kernel(const alignn_b200_fire_cell_params pc, const int32_t* __restrict__ active,

@@ -481,6 +481,144 @@ def fire_cell_step(grad: torch.Tensor, stress: torch.Tensor, active: torch.Tenso
                                               istate.data_ptr(), stream_ptr()), "alignn_b200_fire_cell_step")
 
 
+LBFGS_DEFAULTS = dict(maxstep=0.2, memory=100, damping=1.0, alpha=70.0)   # ase LBFGS defaults (no line search)
+BFGS_DEFAULTS = dict(maxstep=0.2, alpha=70.0)                             # ase BFGS defaults
+QN_BREAKDOWN = 5              # istate status of a crystal whose quasi-Newton update or step is not finite
+
+
+def _qn_operands(name, grad, stress, active, batch_offsets, atom_offsets, positions, forces, cell_ops, rows_ops, istate,
+                 steps):
+    """The operand checks lbfgs_step and bfgs_update share.  Returns (B, A, N, rows, cell)."""
+    cell = stress is not None
+    want = [(grad, torch.float32), (active, torch.int32), (batch_offsets, torch.int32), (atom_offsets, torch.int64),
+            (positions, torch.float64), (forces, torch.float32), (istate, torch.int32)]
+    want += [(t, torch.float64) for t in rows_ops]
+    if cell:
+        want += [(stress, torch.float32), (cell_ops[-1], torch.float32)] + [(t, torch.float64) for t in cell_ops[:-1]]
+    for t, dt in want:
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != grad.device:
+            raise RuntimeError(f"{name} needs all operands on one CUDA device")
+        if t.dtype != dt or not t.is_contiguous():
+            raise RuntimeError(f"{name}: expected a contiguous {dt} tensor, got {t.dtype}")
+    B, A = atom_offsets.numel() - 1, active.numel()
+    N = positions.numel() // 3
+    rows = N + 3 * B if cell else N
+    if (forces.numel() != 3 * N or istate.numel() != 4 * B or batch_offsets.numel() != A + 1 or grad.dim() != 2
+            or grad.shape[1] != 3 or any(t.numel() != 3 * rows for t in rows_ops[:4])
+            or (cell and (stress.numel() != 9 * A or cell_ops[-1].numel() != 6 * B
+                          or any(t.numel() != 9 * B for t in cell_ops[:-1])))):
+        raise ValueError(f"{name}: inconsistent operand shapes")
+    if isinstance(steps, bool) or int(steps) != steps or not 1 <= int(steps) <= FIRE_MAX_STEPS:
+        raise ValueError(f"{name}: steps must be an integer in [1, {FIRE_MAX_STEPS}], got {steps!r}")
+    return B, A, N, rows, cell
+
+
+def _cell_ptrs(cell, cell_ops):
+    return [t.data_ptr() for t in cell_ops] if cell else [None] * 6
+
+
+@_on_tensor_device
+def lbfgs_step(grad: torch.Tensor, stress, active: torch.Tensor, batch_offsets: torch.Tensor, atom_offsets: torch.Tensor,
+               positions: torch.Tensor, forces: torch.Tensor, cells0, logdef, defgrad, cells, cell_forces, stress_out,
+               r0: torch.Tensor, f0: torch.Tensor, work: torch.Tensor, s_ring: torch.Tensor, y_ring: torch.Tensor,
+               history: torch.Tensor, istate: torch.Tensor, *, fmax: float, steps: int, force_multiplier: float = 1.0,
+               stress_wt: float = 1.0, **lbfgs) -> None:
+    """One LBFGS step (ASE 3.22.1 `LBFGS.step` with `Optimizer.converged` and the step limit of `Dynamics.irun`) for the
+    running crystals listed in `active`, in place, one launch (csrc/qn_device.cu, alignn_b200_lbfgs_step).
+
+    As `fire_step` for grad, active, batch_offsets, atom_offsets, positions and forces.  stress None: the atoms alone;
+    else ExpCellFilter as `fire_cell_step` (stress, cells0, logdef, defgrad, cells, cell_forces, stress_out; no cell
+    velocities).  Per-row state, [rows, 3] float64 with rows = N (+ 3B with the filter): r0, f0, work; the history ring
+    s_ring, y_ring [slots * rows * 3] float64 and history [B, 2 * slots] float64, slots >= min(memory, steps); istate
+    [B,4] int32 = {iteration, pairs used, steps taken, status (0 running, 1 converged, 2 step limit, FIRE_BAD_INPUT,
+    FIRE_CELL_DEGENERATE, QN_BREAKDOWN)}, initially zero.  `lbfgs` overrides LBFGS_DEFAULTS."""
+    lib = _lib.load()
+    par = dict(LBFGS_DEFAULTS, **lbfgs)
+    cell_ops = (cells0, logdef, defgrad, cells, cell_forces, stress_out)
+    B, A, N, rows, cell = _qn_operands("lbfgs_step", grad, stress, active, batch_offsets, atom_offsets, positions, forces,
+                                       cell_ops, (r0, f0, work, work, s_ring, y_ring, history), istate, steps)
+    slots = s_ring.numel() // max(3 * rows, 1)
+    if (s_ring.numel() != slots * 3 * rows or y_ring.numel() != s_ring.numel() or history.numel() != 2 * slots * B
+            or slots < 1):
+        raise ValueError("lbfgs_step: inconsistent operand shapes")
+    memory = par["memory"]
+    if isinstance(memory, bool) or int(memory) != memory or not 1 <= int(memory) <= FIRE_MAX_STEPS:
+        raise ValueError(f"lbfgs_step: memory must be an integer >= 1, got {memory!r}")
+    p = _lib.LbfgsParams(float(par["maxstep"]), float(par["alpha"]), float(par["damping"]), float(fmax), int(memory),
+                         int(slots), int(steps), int(cell), float(force_multiplier), float(stress_wt))
+    c0, ld, dg, ce, cf, so = _cell_ptrs(cell, cell_ops)
+    _lib.check(lib.alignn_b200_lbfgs_step(C.byref(p), active.data_ptr(), A, atom_offsets.data_ptr(), batch_offsets.data_ptr(),
+                                          B, grad.data_ptr(), grad.shape[0], stress.data_ptr() if cell else None,
+                                          A if cell else 0, positions.data_ptr(), forces.data_ptr(), c0, ld, dg, ce, cf, so,
+                                          r0.data_ptr(), f0.data_ptr(), work.data_ptr(), s_ring.data_ptr(),
+                                          y_ring.data_ptr(), history.data_ptr(), istate.data_ptr(), stream_ptr()),
+               "alignn_b200_lbfgs_step")
+
+
+@_on_tensor_device
+def bfgs_update(grad: torch.Tensor, stress, active: torch.Tensor, batch_offsets: torch.Tensor, atom_offsets: torch.Tensor,
+                positions: torch.Tensor, forces: torch.Tensor, cells0, logdef, defgrad, cells, cell_forces, stress_out,
+                h_offsets: torch.Tensor, H: torch.Tensor, r0: torch.Tensor, f0: torch.Tensor, r: torch.Tensor,
+                f: torch.Tensor, work: torch.Tensor, istate: torch.Tensor, *, max_dim: int, fmax: float, steps: int,
+                force_multiplier: float = 1.0, stress_wt: float = 1.0, **bfgs) -> None:
+    """The first half of a BFGS step (ASE 3.22.1 `BFGS.step` up to `update`), in place (csrc/qn_device.cu,
+    alignn_b200_bfgs_update): forces, decision, this evaluation's rows r and f, and H's rank-2 update.
+
+    Operands as `lbfgs_step`, plus: h_offsets [B+1] int64 (crystal c's H, [3m, 3m] row-major, at H[h_offsets[c]:]),
+    H float64, initially alpha I per crystal; r, f [rows, 3] float64; work [3, rows, 3] float64; istate = {r0 and f0 set,
+    update pending, steps taken, status}, initially zero; max_dim >= 3m for every crystal of `active`.  `bfgs`
+    overrides BFGS_DEFAULTS."""
+    lib = _lib.load()
+    par = dict(BFGS_DEFAULTS, **bfgs)
+    cell_ops = (cells0, logdef, defgrad, cells, cell_forces, stress_out)
+    B, A, N, rows, cell = _qn_operands("bfgs_update", grad, stress, active, batch_offsets, atom_offsets, positions, forces,
+                                       cell_ops, (r0, f0, r, f, work, H), istate, steps)
+    if work.numel() != 9 * rows or h_offsets.dtype != torch.int64 or h_offsets.numel() != B + 1 or not h_offsets.is_cuda:
+        raise ValueError("bfgs_update: inconsistent operand shapes")
+    p = _lib.BfgsParams(float(par["maxstep"]), float(par["alpha"]), float(fmax), int(steps), int(cell),
+                        float(force_multiplier), float(stress_wt))
+    c0, ld, dg, ce, cf, so = _cell_ptrs(cell, cell_ops)
+    _lib.check(lib.alignn_b200_bfgs_update(C.byref(p), active.data_ptr(), A, atom_offsets.data_ptr(), batch_offsets.data_ptr(),
+                                           B, int(max_dim), grad.data_ptr(), grad.shape[0],
+                                           stress.data_ptr() if cell else None, A if cell else 0, positions.data_ptr(),
+                                           forces.data_ptr(), c0, ld, dg, ce, cf, so, h_offsets.data_ptr(), H.data_ptr(),
+                                           r0.data_ptr(), f0.data_ptr(), r.data_ptr(), f.data_ptr(), work.data_ptr(),
+                                           istate.data_ptr(), stream_ptr()), "alignn_b200_bfgs_update")
+
+
+@_on_tensor_device
+def bfgs_apply(group: torch.Tensor, omega: torch.Tensor, eigenvectors: torch.Tensor, atom_offsets: torch.Tensor,
+               positions: torch.Tensor, cells0, logdef, defgrad, cells, r0: torch.Tensor, f0: torch.Tensor,
+               r: torch.Tensor, f: torch.Tensor, work: torch.Tensor, istate: torch.Tensor, *, cell: bool, **bfgs) -> None:
+    """The second half of a BFGS step (csrc/qn_device.cu, alignn_b200_bfgs_apply) for a group of crystals with the same
+    3m, after omega, V = torch.linalg.eigh(H) of their blocks (row g: crystal group[g]): dr = V ((f V) / |omega|), the
+    longest-row cap, set_positions, r0 = r, f0 = f.  Crystals of the group that are not running are ignored; a
+    crystal whose update broke down gets QN_BREAKDOWN.  Operands as `bfgs_update`."""
+    lib = _lib.load()
+    par = dict(BFGS_DEFAULTS, **bfgs)
+    G, dim = group.numel(), int(omega.shape[-1]) if omega.dim() == 2 else 0
+    B = atom_offsets.numel() - 1
+    rows = r.numel() // 3
+    want = [(group, torch.int32), (omega, torch.float64), (eigenvectors, torch.float64), (atom_offsets, torch.int64),
+            (positions, torch.float64), (r0, torch.float64), (f0, torch.float64), (r, torch.float64), (f, torch.float64),
+            (work, torch.float64), (istate, torch.int32)]
+    want += [(t, torch.float64) for t in (cells0, logdef, defgrad, cells)] if cell else []
+    for t, dt in want:
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != r.device:
+            raise RuntimeError("bfgs_apply needs all operands on one CUDA device")
+        if t.dtype != dt or not t.is_contiguous():
+            raise RuntimeError(f"bfgs_apply: expected a contiguous {dt} tensor, got {t.dtype}")
+    if (omega.dim() != 2 or omega.shape[0] != G or tuple(eigenvectors.shape) != (G, dim, dim) or work.numel() != 9 * rows
+            or any(t.numel() != 3 * rows for t in (r0, f0, f)) or istate.numel() != 4 * B):
+        raise ValueError("bfgs_apply: inconsistent operand shapes")
+    p = _lib.BfgsParams(float(par["maxstep"]), float(par["alpha"]), 0.0, 1, int(bool(cell)), 1.0, 1.0)
+    cp = [t.data_ptr() for t in (cells0, logdef, defgrad, cells)] if cell else [None] * 4
+    _lib.check(lib.alignn_b200_bfgs_apply(C.byref(p), group.data_ptr(), G, dim, omega.data_ptr(), eigenvectors.data_ptr(),
+                                          atom_offsets.data_ptr(), B, rows, positions.data_ptr(), *cp, r0.data_ptr(),
+                                          f0.data_ptr(), r.data_ptr(), f.data_ptr(), work.data_ptr(), istate.data_ptr(),
+                                          stream_ptr()), "alignn_b200_bfgs_apply")
+
+
 MD_NVE, MD_NVT_BERENDSEN = 0, 1   # alignn_b200_md_params.ensemble
 MD_BAD_INPUT = 3                  # status of a crystal whose atom slice does not lie inside the batch
 

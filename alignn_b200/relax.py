@@ -12,6 +12,10 @@ With `optimize_lattice=True` the cells relax with the atoms, as the reference's 
 optimize_lattice=True)` does with ASE's `ExpCellFilter`: each step builds the graphs from the current cells, and
 `ops.fire_cell_step` (csrc/fire_cell_device.cu) moves atoms and cells on the forces and the calculator's Voigt stress;
 `oracle/cell_filter_oracle.py` is its specification.
+
+`optimizer="LBFGS"` or `"BFGS"` runs ASE's quasi-Newton optimizers instead, in either lattice mode, through the same
+loop: only the optimizer state and the step enqueued differ (`ops.lbfgs_step`, or `ops.bfgs_update`, torch's batched
+`eigh` of each crystal's H and `ops.bfgs_apply`; csrc/qn_device.cu).  `oracle/qn_oracle.py` is their specification.
 """
 from __future__ import annotations
 
@@ -30,7 +34,7 @@ class RelaxResult(NamedTuple):
     positions: torch.Tensor      # [N,3] float64 final Cartesian positions (not wrapped into the cell)
     energy: torch.Tensor         # [B] fp32 energy at the final positions, out * natoms (without the bond penalty)
     forces: torch.Tensor         # [N,3] fp32 forces at the final positions, grad * force_multiplier
-    nsteps: torch.Tensor         # [B] int32 FIRE steps taken
+    nsteps: torch.Tensor         # [B] int32 steps taken by the optimizer that ran
     converged: torch.Tensor      # [B] bool: max_i |F_i| < fmax at the final positions
     atom_offsets: torch.Tensor   # [B+1] int64: atoms of crystal b are rows atom_offsets[b]:atom_offsets[b+1]
 
@@ -39,7 +43,7 @@ class CellRelaxResult(NamedTuple):
     positions: torch.Tensor      # [N,3] float64 final Cartesian positions (not wrapped into the cell)
     energy: torch.Tensor         # [B] fp32 energy at the final structure, out * natoms (without the bond penalty)
     forces: torch.Tensor         # [N,3] fp32 Cartesian forces at the final structure, grad * force_multiplier
-    nsteps: torch.Tensor         # [B] int32 FIRE steps taken
+    nsteps: torch.Tensor         # [B] int32 steps taken by the optimizer that ran
     converged: torch.Tensor      # [B] bool: the filter's test, max over atom and cell rows of |row| < fmax
     atom_offsets: torch.Tensor   # [B+1] int64: atoms of crystal b are rows atom_offsets[b]:atom_offsets[b+1]
     cells: torch.Tensor          # [B,3,3] float64 final lattices, rows are lattice vectors as given
@@ -172,10 +176,72 @@ def _evaluate_chunks(model, structures, features, dev, *, neighbor_strategy, cut
     return energy, grad_all
 
 
+OPTIMIZERS = ("FIRE", "LBFGS", "BFGS")
+# the other optimizers `ForceField.optimize_atoms` accepts (alignn/ff/ff.py:385-398), which this package does not build
+NOT_BUILT_OPTIMIZERS = ("MDMin", "GPMin", "LBFGSLineSearch", "BFGSLineSearch", "SciPyFminCG", "SciPyFminBFGS")
+
+
+def _check_optimizer(optimizer) -> str:
+    if not isinstance(optimizer, str) or optimizer not in OPTIMIZERS + NOT_BUILT_OPTIMIZERS:
+        raise ValueError(f"optimizer must be one of {', '.join(OPTIMIZERS)}, got {optimizer!r}")
+    if optimizer in NOT_BUILT_OPTIMIZERS:
+        raise NotImplementedError(f"relax_structures: optimizer {optimizer!r} is not implemented; "
+                                  f"use one of {', '.join(OPTIMIZERS)}")
+    return optimizer
+
+
+class _QuasiNewton:
+    """The optimizer state of a batched LBFGS or BFGS relaxation (csrc/qn_device.cu) and its step: the rows of crystal b
+    start at row aoff[b] (+ 3b under the filter) of every per-row array."""
+
+    def __init__(self, optimizer, sizes, aoff, steps, cell, dev):
+        self.optimizer, self.cell, self.sizes = optimizer, cell, sizes
+        B = len(sizes)
+        rows = int(aoff[-1]) + (3 * B if cell else 0)
+        self.rows = rows
+        f64 = dict(device=dev, dtype=torch.float64)
+        self.r0, self.f0 = torch.zeros(rows, 3, **f64), torch.zeros(rows, 3, **f64)
+        self.istate = torch.zeros(B, 4, device=dev, dtype=torch.int32)
+        if optimizer == "LBFGS":
+            slots = min(ops.LBFGS_DEFAULTS["memory"], int(steps))
+            self.work = torch.zeros(rows, 3, **f64)
+            self.s_ring, self.y_ring = torch.zeros(slots * rows * 3, **f64), torch.zeros(slots * rows * 3, **f64)
+            self.history = torch.zeros(B, 2 * slots, **f64)
+        else:
+            self.dims = [3 * (n + 3 if cell else n) for n in sizes]
+            self.h_off = np.concatenate([[0], np.cumsum([d * d for d in self.dims])]).astype(np.int64)
+            self.h_off_d = torch.from_numpy(self.h_off).to(dev)
+            H = torch.zeros(int(self.h_off[-1]), **f64)
+            for b, d in enumerate(self.dims):                  # H0 = alpha I
+                H[int(self.h_off[b]):int(self.h_off[b + 1])].view(d, d).diagonal().fill_(ops.BFGS_DEFAULTS["alpha"])
+            self.H = H
+            self.r, self.f = torch.zeros(rows, 3, **f64), torch.zeros(rows, 3, **f64)
+            self.work = torch.zeros(3, rows, 3, **f64)
+
+    def step(self, grad, stress, act, active, batch_offsets, aoff_d, pos, forces, cell_ops, kw):
+        if self.optimizer == "LBFGS":
+            ops.lbfgs_step(grad, stress, act, batch_offsets, aoff_d, pos, forces, *cell_ops, self.r0, self.f0, self.work,
+                           self.s_ring, self.y_ring, self.history, self.istate, **kw)
+            return
+        max_dim = max(self.dims[b] for b in active)
+        ops.bfgs_update(grad, stress, act, batch_offsets, aoff_d, pos, forces, *cell_ops, self.h_off_d, self.H, self.r0,
+                        self.f0, self.r, self.f, self.work, self.istate, max_dim=max_dim, **kw)
+        groups = {}
+        for b in active:
+            groups.setdefault(self.dims[b], []).append(b)
+        dev = pos.device
+        for d, ids in groups.items():                          # eigh of every running crystal's H, d x d at a time
+            base = torch.from_numpy(self.h_off[ids]).to(dev)
+            idx = base.unsqueeze(1) + torch.arange(d * d, device=dev).unsqueeze(0)
+            omega, V = torch.linalg.eigh(self.H[idx].view(len(ids), d, d))
+            ops.bfgs_apply(torch.tensor(ids, dtype=torch.int32).to(dev), omega.contiguous(), V.contiguous(), aoff_d, pos,
+                           *cell_ops[:4], self.r0, self.f0, self.r, self.f, self.work, self.istate, cell=self.cell)
+
+
 def relax_structures(model, structures, atom_features: torch.Tensor, *, fmax: float = 0.1, steps: int = 100,
                      neighbor_strategy: str = "k-nearest", cutoff: float = 8.0, max_neighbors: int = 12,
                      cutoff_extra: float = 3.5, force_multiplier: float = 1.0, optimize_lattice: bool = False,
-                     stress_wt: float = 1.0):
+                     stress_wt: float = 1.0, optimizer: str = "FIRE"):
     """Relax the atomic positions of a batch of crystals with FIRE (ASE 3.22.1 defaults), the cells fixed: a batched
     `optimize_atoms(optimizer="FIRE", optimize_lattice=False, fmax=fmax, steps=steps)`.  Returns a `RelaxResult`.
     With optimize_lattice=True the cells relax too (see below) and a `CellRelaxResult` is returned.
@@ -198,7 +264,15 @@ def relax_structures(model, structures, atom_features: torch.Tensor, *, fmax: fl
     filter's forces (atom rows f_i F and the three cell rows) is below fmax.  The model must compute stress
     (stresswise_weight != 0); optimize_lattice must be a bool.  Every step builds the graphs from the current cells.  The returned forces stay
     Cartesian; `cells` and `stress` are the final lattices and the stress of the last evaluation.  A cell that loses
-    its volume raises RuntimeError naming the crystal."""
+    its volume raises RuntimeError naming the crystal.
+
+    optimizer: "FIRE" (the default), "LBFGS" or "BFGS" -- ASE 3.22.1's optimizers with the defaults the reference passes
+    (LBFGS: maxstep 0.2, memory 100, damping 1, alpha 70, no line search; BFGS: maxstep 0.2, alpha 70), with either
+    value of optimize_lattice; oracle/qn_oracle.py is their specification.  nsteps counts the steps of the optimizer
+    that ran.  The other names optimize_atoms accepts raise NotImplementedError, anything else ValueError.  Where ASE
+    would carry on with positions that are not finite (a zero or non-finite curvature y.s, a or b, or a step that is
+    not finite) a RuntimeError names the crystal and the optimizer."""
+    optimizer = _check_optimizer(optimizer)
     lats, Xs, dev = _check(model, structures, atom_features, fmax, steps, neighbor_strategy, max_neighbors)
     if not isinstance(optimize_lattice, (bool, np.bool_)):
         raise ValueError(f"optimize_lattice must be a bool, got {optimize_lattice!r}")
@@ -230,6 +304,9 @@ def relax_structures(model, structures, atom_features: torch.Tensor, *, fmax: fl
         cvel, cforces = torch.zeros_like(cells0), torch.zeros_like(cells0)
         stress_out = torch.zeros(B, 6, device=dev, dtype=torch.float32)
         host_cells = [lat.copy() for lat in lats]
+    qn = None if optimizer == "FIRE" else _QuasiNewton(optimizer, sizes, aoff, steps, cell, dev)
+    if qn is not None:
+        istate = qn.istate
     active = list(range(B))
     while active:
         A = len(active)
@@ -249,8 +326,13 @@ def relax_structures(model, structures, atom_features: torch.Tensor, *, fmax: fl
                     grad = _forces_as_alone(model, g, res, A)
             out = res["out"].detach().reshape(-1)                            # 0-d for a one-crystal batch
             energy[act.long()] = out * g.batch_num_nodes_on_device().to(out.dtype)
-        with ops._span("relax_fire", 0):
-            if cell:
+        with ops._span("relax_fire" if qn is None else "relax_" + optimizer.lower(), 0):
+            if qn is not None:
+                cell_ops = (cells0, logdef, defgrad, cells, cforces, stress_out) if cell else (None,) * 6
+                qn.step(grad, stress if cell else None, act, active, g.node_graph_offsets(), aoff_d, pos, forces, cell_ops,
+                        dict(fmax=float(fmax), steps=int(steps), force_multiplier=float(force_multiplier),
+                             stress_wt=float(stress_wt)))
+            elif cell:
                 ops.fire_cell_step(grad, stress, act, g.node_graph_offsets(), aoff_d, pos, vel, forces, cells0, logdef,
                                    defgrad, cells, cvel, cforces, stress_out, fstate, istate, fmax=float(fmax),
                                    steps=int(steps), force_multiplier=float(force_multiplier), stress_wt=float(stress_wt))
@@ -273,8 +355,12 @@ def relax_structures(model, structures, atom_features: torch.Tensor, *, fmax: fl
             host_pos[b] = new_pos[o:o + sizes[b]]
             o += sizes[b]
         if (status == ops.FIRE_BAD_INPUT).any():
-            raise RuntimeError(f"alignn_b200_{'fire_cell_step' if cell else 'fire_step'}: the model's forces do not match "
-                               "the crystals' atom counts")
+            what = {"FIRE": "fire_cell_step" if cell else "fire_step", "LBFGS": "lbfgs_step", "BFGS": "bfgs_update"}
+            raise RuntimeError(f"alignn_b200_{what[optimizer]}: the model's forces do not match the crystals' atom counts")
+        broke = [b for b, s in zip(active, status) if s == ops.QN_BREAKDOWN]
+        if broke:
+            raise RuntimeError(f"relax_structures: {optimizer} broke down on crystal {broke[0]} (a curvature y.s, a or b "
+                               "that is zero or not finite, or a step that is not finite)")
         bad = [b for b, s in zip(active, status) if s == ops.FIRE_CELL_DEGENERATE]
         if cell and bad:
             raise RuntimeError(f"relax_structures: the cell of crystal {bad[0]} became degenerate (its volume or "

@@ -644,6 +644,94 @@ int alignn_b200_fire_cell_step(const alignn_b200_fire_cell_params* params, const
                                float* stress_out, double* fstate, int32_t* istate, alignn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Quasi-Newton relaxation (csrc/qn_device.cu): ASE 3.22.1's `LBFGS` and `BFGS` (ase/optimize/lbfgs.py, bfgs.py) with
+ * the convergence test and step limit of `Optimizer.converged` / `Dynamics.irun`, on the atoms or (cell = 1) on
+ * `ExpCellFilter` as alignn_b200_fire_cell_step -- what `ForceField.optimize_atoms(optimizer="LBFGS" / "BFGS", ...)`
+ * (alignn/ff/ff.py:385-412) runs one crystal at a time.  Device pointers, caller-owned buffers, enqueue-only.
+ *
+ * Rows: a crystal with n atoms has m = n rows (r = x_i, f = F_i widened) or, with cell = 1, m = n + 3 (atom rows
+ * F^-1 x_i and f_i F, then the three rows of L and of the filter's cell forces).  Its rows start at row
+ * atom_offsets[c] + 3c (cell = 1) or atom_offsets[c] of every [rows, 3] double array below, rows = N + 3B or N.
+ * istate [num_crystals, 4] int32: columns 2 and 3 are the steps taken and the status -- 0 running, 1 converged, 2 step
+ * limit, 3 inconsistent input (the batch slice is not the crystal's atoms, or a size does not match), 4 degenerate cell
+ * (as alignn_b200_fire_cell_step), 5 breakdown (y.s, a or b zero or not finite, or a step that is not finite; the
+ * positions and cell are not moved).  Crystals with a nonzero status, and ids outside [0, num_crystals), are not
+ * touched.  grad, batch_offsets, stress, stress_out, cell_forces and the filter state are as alignn_b200_fire_cell_step;
+ * with cell = 0 stress and the filter arrays may be NULL.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct {
+  double maxstep;           /* 0.2: the longest row of dr is capped (>=) at maxstep                    */
+  double alpha;             /* 70: H0 = 1 / alpha                                                     */
+  double damping;           /* 1.0: dr is multiplied by it after the cap                              */
+  double fmax;              /* converged when the largest |row|^2 < fmax^2 (strict)                    */
+  int32_t memory;           /* 100: pairs the two-loop recursion uses, >= 1                          */
+  int32_t slots;            /* ring slots per crystal, >= min(memory, max_steps)                      */
+  int32_t max_steps;        /* steps >= 1                                                             */
+  int32_t cell;             /* 0: atoms only; 1: ExpCellFilter                                        */
+  float force_multiplier;   /* F = fp32(grad * force_multiplier)                                      */
+  float stress_wt;          /* s = fp32(voigt(stress) * stress_wt / 160.21766208) (cell = 1)          */
+} alignn_b200_lbfgs_params;
+
+/* One LBFGS launch per step, one CTA per entry of active.  Per running crystal: forces (and the filter's rows), the
+ * decision, then at iteration k > 0 the pair s = r - r0, y = f0 - f, rho = 1 / y.s into slot (k - 1) % slots, the
+ * two-loop recursion over the last min(k, memory) pairs, dr = the longest-row cap of -z times damping, set_positions
+ * (r + dr), r0 = r, f0 = f.
+ *   r0, f0, work [rows, 3] double (work: q and then dr of the last step); s_ring, y_ring [slots * rows * 3] double,
+ *   crystal c's slot j at 3 (slots * row0(c) + j m); history [num_crystals, 2 * slots] double (rho, then the
+ *   two-loop's a); istate = {iteration, pairs used by the last step, steps taken, status}, initially {0, 0, 0, 0}.
+ * Rejected (ALIGNN_ERR_BAD_ARG, nothing enqueued): a NULL array that is needed, num_active outside [0, num_crystals],
+ * maxstep or alpha not finite and > 0, a non-finite damping, force_multiplier or (cell = 1) stress_wt, fmax negative or
+ * not finite, memory < 1, max_steps < 1, slots < min(memory, max_steps), cell not 0 or 1, or (cell = 1) stress_rows
+ * != num_active. */
+int alignn_b200_lbfgs_step(const alignn_b200_lbfgs_params* params, const int32_t* active, int64_t num_active,
+                           const int64_t* atom_offsets, const int32_t* batch_offsets, int64_t num_crystals,
+                           const float* grad, int64_t grad_rows, const float* stress, int64_t stress_rows,
+                           double* positions, float* forces, const double* cells0, double* logdef, double* defgrad,
+                           double* cells, double* cell_forces, float* stress_out, double* r0, double* f0, double* work,
+                           double* s_ring, double* y_ring, double* history, int32_t* istate, alignn_stream_t stream);
+
+typedef struct {
+  double maxstep;           /* 0.2: the longest row of dr is capped (>=) at maxstep */
+  double alpha;             /* 70: H0 = alpha I                                     */
+  double fmax;
+  int32_t max_steps;
+  int32_t cell;             /* 0: atoms only; 1: ExpCellFilter                      */
+  float force_multiplier;
+  float stress_wt;
+} alignn_b200_bfgs_params;
+
+/* The first half of a BFGS step: per running crystal of active, forces (and the filter's rows) and the decision; for a
+ * crystal that steps, its rows r and f of this evaluation are stored, and unless this is its first step or
+ * max |r - r0| < 1e-7, H -= outer(df, df) / a + outer(dg, dg) / b with dr = r - r0, df = f - f0, a = dr.df,
+ * dg = H dr, b = dr.dg.  H, [3m, 3m] row-major per crystal, starts at H[h_offsets[c]]; h_offsets [num_crystals + 1]
+ * int64 with h_offsets[c+1] - h_offsets[c] = (3m)^2, initially alpha I.  dg = H dr and the update run with
+ * ceil(max_dim / 32) CTAs per crystal; max_dim >= 3m for every crystal of active (else status 3).  When a or b is zero
+ * or not finite H is left as it is and alignn_b200_bfgs_apply sets status 5.
+ *   r0, f0, r, f [rows, 3] double; work [3, rows, 3] double (dg, w, dr); istate = {r0 and f0 hold a step's rows,
+ *   update pending, steps taken, status}, initially {0, 0, 0, 0}.
+ * Rejected: as alignn_b200_lbfgs_step where it applies, and max_dim < 3 or max_dim > 32 * 65535. */
+int alignn_b200_bfgs_update(const alignn_b200_bfgs_params* params, const int32_t* active, int64_t num_active,
+                            const int64_t* atom_offsets, const int32_t* batch_offsets, int64_t num_crystals,
+                            int64_t max_dim, const float* grad, int64_t grad_rows, const float* stress,
+                            int64_t stress_rows, double* positions, float* forces, const double* cells0,
+                            const double* logdef, const double* defgrad, const double* cells, double* cell_forces,
+                            float* stress_out, const int64_t* h_offsets, double* H, double* r0, double* f0, double* r,
+                            double* f, double* work, int32_t* istate, alignn_stream_t stream);
+
+/* The second half, after omega, V = eigh(H) for a group of crystals with the same dim = 3m: omega [group_size, dim] and
+ * eigenvectors [group_size, dim, dim] (row-major, eigenvectors in the columns) of crystal group[g] in row g.  For every
+ * running crystal of the group: status 5 if its update broke down; dr = V ((f V) / |omega|) with several CTAs per
+ * crystal; the longest-row cap; set_positions(r + dr) (cell = 1: L = L + dr_cell, F = expm(L), C = C0 F^T, status 4
+ * when expm is not finite, x_i = F (r_i + dr_i)); r0 = r, f0 = f.  A crystal that is not running is ignored, so a
+ * group may hold crystals that converged in this evaluation.  num_rows = rows (N + 3B or N).
+ * Rejected: as alignn_b200_bfgs_update where it applies, and dim < 3 or num_rows < 1. */
+int alignn_b200_bfgs_apply(const alignn_b200_bfgs_params* params, const int32_t* group, int64_t group_size, int64_t dim,
+                           const double* omega, const double* eigenvectors, const int64_t* atom_offsets,
+                           int64_t num_crystals, int64_t num_rows, double* positions, const double* cells0,
+                           double* logdef, double* defgrad, double* cells, double* r0, double* f0, const double* r,
+                           const double* f, double* work, int32_t* istate, alignn_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Molecular dynamics (csrc/md_device.cu): ASE 3.22.1's `VelocityVerlet` (NVE) and `NVTBerendsen` (fixcm=True) with the
  * run loop of `MolecularDynamics.irun` -- what `ForceField.run_nve_velocity_verlet` / `run_nvt_berendsen`
  * (alignn/ff/ff.py:419-443, 510-543) run one crystal at a time -- for a batch of crystals advanced in lockstep.
