@@ -224,6 +224,9 @@ _SIGNATURES = {
                                                _fp]),
     "alignn_b200_remove_net_torque_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "alignn_b200_remove_net_torque": (C.c_int, [_fp, _fp, _fp, C.c_int64, C.c_int64, C.c_int, _fp, _fp, C.c_size_t, _fp]),
+    "alignn_b200_remove_net_torque_per_crystal_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),
+    "alignn_b200_remove_net_torque_per_crystal": (C.c_int, [_fp, _fp, _fp, C.c_int64, C.c_int64, _fp, _fp, C.c_size_t,
+                                                            _fp]),
     "alignn_b200_fire_step": (C.c_int, [C.POINTER(FireParams), _fp, C.c_int64, _fp, _fp, C.c_int64, _fp, C.c_int64, _fp, _fp,
                                         _fp, _fp, _fp, _fp]),
     "alignn_b200_fire_cell_step": (C.c_int, [C.POINTER(FireCellParams), _fp, C.c_int64, _fp, _fp, C.c_int64, _fp, C.c_int64,

@@ -150,8 +150,14 @@ class eALIGNNAtomWise(nn.Module):
                 return self._forward(g, True)
         return self._forward(g, False)
 
-    def _forward(self, inputs, second: bool):
+    def _forward(self, inputs, second: bool, per_crystal: bool = False):
+        """per_crystal=True evaluates every crystal of the batch as if it were alone (what the reference calculator
+        computes for one structure; the batched drivers use it): the energies and the bond penalty are differentiated
+        once, as sum_b en_b + sum(penalty), each bond's pair force is scaled by its own crystal's atom count, and the net
+        torque is removed per crystal (`ops.remove_net_torque_per_crystal`).  Inference only (second=False)."""
         c = self.config
+        if per_crystal and second:
+            raise ValueError("eALIGNNAtomWise: the per-crystal evaluation is inference only")
         g, lat = as_graph(inputs[0]), inputs[-1]
         x = self.atom_embedding(g.ndata["atom_features"])
         lg = z = None
@@ -196,9 +202,19 @@ class eALIGNNAtomWise(nn.Module):
         result = {}
         if c.calculate_gradient:
             with ops.input_grads_only():
-                (dr,) = torch.autograd.grad(en_out, r, grad_outputs=torch.ones_like(en_out),
-                                            create_graph=second, retain_graph=second or self.training)
-            pair_forces = -dr * g.num_nodes()                           # :384-394: the batch's total atom count
+                if per_crystal:                        # one crystal's en_out alone, summed over the batch: each term once
+                    en0 = out * natoms if c.energy_mult_natoms else out
+                    total = en0.sum() + pen.sum() if c.use_penalty else en0.sum()
+                    (dr,) = torch.autograd.grad(total, r, retain_graph=self.training)
+                else:
+                    (dr,) = torch.autograd.grad(en_out, r, grad_outputs=torch.ones_like(en_out),
+                                                create_graph=second, retain_graph=second or self.training)
+            if per_crystal:                                             # each bond scaled by its own crystal's atoms
+                n_e = torch.repeat_interleave(natoms.to(torch.float32), g.batch_num_edges().to(dr.device),
+                                              output_size=dr.shape[0])
+                pair_forces = -dr * n_e.unsqueeze(1)
+            else:
+                pair_forces = -dr * g.num_nodes()                       # :384-394: the batch's total atom count
             if second:
                 src, dst = g.index.src.long(), g.index.dst.long()
                 zeros = torch.zeros(g.num_nodes(), 3, device=r.device, dtype=r.dtype)
@@ -208,6 +224,8 @@ class eALIGNNAtomWise(nn.Module):
             if c.remove_torque:                                         # :409-412
                 if second:
                     forces = remove_net_torque_torch(pos.detach(), forces, g.batch_num_nodes())
+                elif per_crystal:
+                    forces = ops.remove_net_torque_per_crystal(pos.detach(), forces, g.node_graph_offsets().long())
                 else:
                     forces = ops.remove_net_torque(pos.detach(), forces, g.node_graph_offsets().long())
             forces = torch.squeeze(forces)

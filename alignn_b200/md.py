@@ -28,7 +28,7 @@ import numpy as np
 import torch
 
 from . import neighbors, ops
-from .relax import _check_batch, _check_model, _forces_and_stress_as_alone, _forces_as_alone
+from .relax import _check_batch, _check_model, _evaluate, _forces_and_stress_as_alone, _forces_as_alone, _graphs
 
 # ase.units (ASE 3.22.1, CODATA 2014): the femtosecond in ASE time units and the Boltzmann constant in eV/K
 _e, _amu, _k = 1.6021766208e-19, 1.660539040e-27, 1.38064852e-23
@@ -126,7 +126,8 @@ def run_md(model, structures, atom_features: torch.Tensor, masses, *, ensemble: 
     fixcm=True) or `run_nvt_andersen(temperature_K=..., andersen_prob=...)` (ensemble="nvt_andersen", ASE's Andersen
     with fixcm=True).  Returns an `MDResult`.
 
-    model: an `ALIGNNAtomWise` in eval mode on a CUDA device, with calculate_gradient=True and output_features=1.
+    model: an `ALIGNNAtomWise` or `eALIGNNAtomWise` in eval mode on a CUDA device, with calculate_gradient=True and
+    output_features=1; each crystal gets what it would get run alone.
     structures: sequence of (lattice [3,3], cart_coords [n,3]), as for `neighbors.crystal_graphs_device`;
     atom_features: [sum n, F] on the model's device, in the same atom order; masses: [sum n] in amu, all > 0.
     timestep in fs (the reference's default 0.01); taut in fs, default 100 * timestep (taken as 100 times the
@@ -252,12 +253,12 @@ def run_md(model, structures, atom_features: torch.Tensor, masses, *, ensemble: 
     traj = []
     for e in range(steps + 1):
         with ops._span("md_build", 0):
-            g, lg, lat = neighbors.crystal_graphs_device(list(zip(lats, host_pos)), atom_features,
-                                                         neighbor_strategy=neighbor_strategy, cutoff=cutoff,
-                                                         max_neighbors=max_neighbors, cutoff_extra=cutoff_extra, device=dev)
+            g, lg, lat = _graphs(model, list(zip(lats, host_pos)), atom_features, dev,
+                                 neighbor_strategy=neighbor_strategy, cutoff=cutoff, max_neighbors=max_neighbors,
+                                 cutoff_extra=cutoff_extra)
         with ops._span("md_model", 0):
             with torch.enable_grad():
-                res = model((g, lg, lat))
+                res = _evaluate(model, g, lg, lat)
                 grad = _forces_as_alone(model, g, res, B)
             out = res["out"].detach().reshape(-1)                            # 0-d for a one-crystal batch
             energy[e] = out * g.batch_num_nodes_on_device().to(out.dtype)
@@ -329,11 +330,10 @@ def _run_npt(model, lats, Xs, atom_features, aoff, pos, mom, m_d, T0, dev, *, st
 
     def evaluate(with_stress):
         with ops._span("md_build", 0):
-            g, lg, lat = neighbors.crystal_graphs_device(list(zip(host_cells, host_pos)), atom_features, device=dev,
-                                                         **graph)
+            g, lg, lat = _graphs(model, list(zip(host_cells, host_pos)), atom_features, dev, **graph)
         with ops._span("md_model", 0):
             with torch.enable_grad():
-                res = model((g, lg, lat))
+                res = _evaluate(model, g, lg, lat)
                 if with_stress:
                     return g, res, _forces_and_stress_as_alone(model, g, res, B)
                 return g, res, (_forces_as_alone(model, g, res, B), None)
@@ -483,11 +483,10 @@ def _run_nose_hoover(model, lats, Xs, atom_features, aoff, pos, mom, m_d, T0, de
     traj = []
     for e in range(steps + 1):
         with ops._span("md_build", 0):
-            g, lg, lat = neighbors.crystal_graphs_device(list(zip(host_cells, host_pos)), atom_features, device=dev,
-                                                         **graph)
+            g, lg, lat = _graphs(model, list(zip(host_cells, host_pos)), atom_features, dev, **graph)
         with ops._span("md_model", 0):
             with torch.enable_grad():
-                res = model((g, lg, lat))
+                res = _evaluate(model, g, lg, lat)
                 grad, stress = _forces_and_stress_as_alone(model, g, res, B)
             out = res["out"].detach().reshape(-1)
             energy[e] = out * g.batch_num_nodes_on_device().to(out.dtype)

@@ -199,7 +199,8 @@ def knn_graph_device(lattice_mat, cart_coords, max_neighbors: int = 12, cutoff: 
 
 
 def crystal_graphs_device(structures, atom_features: torch.Tensor, neighbor_strategy: str = "k-nearest",
-                          cutoff: float = 8.0, max_neighbors: int = 12, cutoff_extra: float = 3.5, device="cuda"):
+                          cutoff: float = 8.0, max_neighbors: int = 12, cutoff_extra: float = 3.5, device="cuda",
+                          line_graph: bool = True):
     """(g, lg, lat) of a batch of periodic structures, built on the GPU: what `dgl.batch` of `atom_dgl_multigraph`
     outputs (graphs.py:472-589) plus the stacked lattices give the models (`ALIGNN`, `ALIGNNAtomWise`,
     `eALIGNNAtomWise`).
@@ -208,7 +209,8 @@ def crystal_graphs_device(structures, atom_features: torch.Tensor, neighbor_stra
     order (the caller's embedding table).  `neighbor_strategy` "k-nearest" (the reference default: `knn_graph` per
     crystal) or "radius_graph" (`radius_graph` per crystal with this `cutoff_extra`; atom_dgl_multigraph's 3.5).
     g.ndata: atom_features, V (the cell volume |a . (b x c)| on every atom), frac_coords (fp32); g.edata: r, images
-    (fp32); lg = L(g) with lg.edata["h"] = bond cosines; lat [B,3,3] fp32."""
+    (fp32); lg = L(g) with lg.edata["h"] = bond cosines; lat [B,3,3] fp32.  line_graph=False skips L(g) and the
+    cosines and returns lg = None (eALIGNN builds its own L(g) inside forward); g is the same."""
     dev = torch.device(device)
     u, v, r, img, bne, lats, fracs, sizes = _neighbors_device(structures, neighbor_strategy, cutoff, max_neighbors,
                                                               cutoff_extra, dev)
@@ -224,8 +226,10 @@ def crystal_graphs_device(structures, atom_features: torch.Tensor, neighbor_stra
     g.ndata["frac_coords"] = host[N:4 * N].view(N, 3)
     g.edata["r"] = r
     g.edata["images"] = img
-    lg = g.line_graph(shared=True)
-    lg.edata["h"] = bond_cosines(r, lg)
+    lg = None
+    if line_graph:
+        lg = g.line_graph(shared=True)
+        lg.edata["h"] = bond_cosines(r, lg)
     return g, lg, host[4 * N:].view(len(lats), 3, 3)
 
 

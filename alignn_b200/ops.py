@@ -383,6 +383,29 @@ def remove_net_torque(pos: torch.Tensor, forces: torch.Tensor, node_offsets64: t
     return out
 
 
+@_on_tensor_device
+def remove_net_torque_per_crystal(pos: torch.Tensor, forces: torch.Tensor, node_offsets64: torch.Tensor) -> torch.Tensor:
+    """Forces with each crystal's own net torque removed, the crystal's centre and torque taken over its atoms only:
+    bit for bit `remove_net_torque` of every crystal as a one-crystal batch (a 3-atom crystal crosses along dim 0), in
+    one set of launches for the batch and without a read-back.  node_offsets64 [B+1] int64 on the device; offsets that
+    do not start at 0, decrease or do not end at N give NaN forces."""
+    lib = _lib.load()
+    pos, forces = pos.contiguous(), forces.contiguous()
+    require_cuda(pos, forces)
+    if node_offsets64.dtype != torch.int64 or node_offsets64.device != forces.device:
+        raise ValueError("node_offsets64 must be an int64 tensor on the forces' device")
+    N, B = forces.shape[0], node_offsets64.numel() - 1
+    if pos.shape != (N, 3) or forces.shape != (N, 3):
+        raise ValueError(f"pos and forces must both be [N,3], got {tuple(pos.shape)} and {tuple(forces.shape)}")
+    out = torch.empty(N, 3, device=forces.device, dtype=torch.float32)
+    nb = int(lib.alignn_b200_remove_net_torque_per_crystal_workspace_bytes(B, N))
+    ws = torch.empty(max(nb, 1), device=forces.device, dtype=torch.uint8)
+    _lib.check(lib.alignn_b200_remove_net_torque_per_crystal(ptr(pos), ptr(forces), node_offsets64.contiguous().data_ptr(),
+                                                             B, N, ptr(out), ptr(ws), nb, stream_ptr()),
+               "alignn_b200_remove_net_torque_per_crystal")
+    return out
+
+
 FIRE_DEFAULTS = dict(maxstep=0.2, dtmax=1.0, n_min=5, finc=1.1, fdec=0.5, astart=0.1, fa=0.99)   # ase FIRE defaults
 FIRE_DT0, FIRE_A0 = 0.1, 0.1                                                                    # its initial dt and a
 FIRE_BAD_INPUT = 3            # istate status of a crystal whose batch slice does not match its atom count

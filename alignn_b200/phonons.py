@@ -135,7 +135,8 @@ def phonons(model, structures, atom_features: torch.Tensor, masses, *, supercell
     supercell, delta)`, `run()`, `read(acoustic=True)`, `band_structure(q)` and `get_dos(kpts).sample_grid(npts,
     width)`.  Returns a `PhononResult`.
 
-    model: an `ALIGNNAtomWise` in eval mode on a CUDA device, with calculate_gradient=True and output_features=1.
+    model: an `ALIGNNAtomWise` or `eALIGNNAtomWise` in eval mode on a CUDA device, with calculate_gradient=True and
+    output_features=1.
     structures: sequence of (lattice [3,3], cart_coords [n,3]) unit cells, as for `neighbors.crystal_graphs_device`;
     atom_features: [sum n, F] on the model's device, in the same atom order; masses: [sum n] in amu, all > 0.
     supercell: one (N0, N1, N2) for the batch, at most ops.PHONON_MAX_CELLS cells; delta: the displacement in A.

@@ -16,6 +16,10 @@ optimize_lattice=True)` does with ASE's `ExpCellFilter`: each step builds the gr
 `optimizer="LBFGS"` or `"BFGS"` runs ASE's quasi-Newton optimizers instead, in either lattice mode, through the same
 loop: only the optimizer state and the step enqueued differ (`ops.lbfgs_step`, or `ops.bfgs_update`, torch's batched
 `eigh` of each crystal's H and `ops.bfgs_apply`; csrc/qn_device.cu).  `oracle/qn_oracle.py` is their specification.
+
+The model is an `ALIGNNAtomWise` or an `eALIGNNAtomWise`.  `_graphs`, `_evaluate` and the `_forces*_as_alone` helpers
+are the only model-specific code the batched drivers (here, md.py, phonons.py, eos.py) share: eALIGNN is evaluated
+through its per-crystal mode (DESIGN section 19), ALIGNNAtomWise through its forward plus the penalty correction.
 """
 from __future__ import annotations
 
@@ -28,6 +32,7 @@ import torch
 
 from . import neighbors, ops
 from .alignn_atomwise import ALIGNNAtomWise, bond_penalty, cutoff_function_based_edges
+from .ealignn_atomwise import eALIGNNAtomWise
 
 
 class RelaxResult(NamedTuple):
@@ -51,9 +56,9 @@ class CellRelaxResult(NamedTuple):
 
 
 def _check_model(caller: str, model) -> None:
-    """The model checks `relax_structures` and `run_md` share; `caller` names the call in the messages."""
-    if not isinstance(model, ALIGNNAtomWise):
-        raise ValueError(f"{caller} takes an ALIGNNAtomWise model")
+    """The model checks the batched drivers share; `caller` names the call in the messages."""
+    if not isinstance(model, (ALIGNNAtomWise, eALIGNNAtomWise)):
+        raise ValueError(f"{caller} takes an ALIGNNAtomWise or eALIGNNAtomWise model")
     c = model.config
     if model.training:
         raise ValueError(f"{caller} needs the model in eval mode (model.eval())")
@@ -66,6 +71,13 @@ def _check_model(caller: str, model) -> None:
         # energy would depend on the other crystals in the batch
         raise NotImplementedError(f"{caller}: energy_mult_natoms=False with use_penalty=True mixes the batch's "
                                   "penalty into every crystal's energy")
+    if isinstance(model, eALIGNNAtomWise):
+        # eALIGNN ignores force_mult_natoms, as the reference does.  Without ALIGNN layers its torque removal reads
+        # ndata["cart_coords"], which no graph builder provides (the reference calculator fails with a KeyError there)
+        if c.alignn_layers == 0 and c.remove_torque:
+            raise ValueError(f"{caller}: an eALIGNNAtomWise with alignn_layers=0 and remove_torque=True needs "
+                             "ndata['cart_coords'], which the crystal graphs do not carry")
+        return
     if c.force_mult_natoms:
         # the model multiplies the pair forces by the atoms of the whole batch (alignn_atomwise.py:530-539); the
         # calculator's natoms factor goes into force_multiplier instead
@@ -110,6 +122,21 @@ def _penalty_pair_grad(model, r: torch.Tensor) -> torch.Tensor:
     return d
 
 
+def _graphs(model, structures, feats, dev, **graph):
+    """The device graphs (g, lg, lat) a driver hands `model`: eALIGNN builds L(g) of its filtered graph itself, so its
+    lg is None and the build skips L(g)."""
+    return neighbors.crystal_graphs_device(structures, feats, device=dev,
+                                           line_graph=not isinstance(model, eALIGNNAtomWise), **graph)
+
+
+def _evaluate(model, g, lg, lat) -> dict:
+    """One model call over a batch: eALIGNN through its per-crystal evaluation (every crystal as if alone, DESIGN
+    section 19); ALIGNNAtomWise through its forward, corrected afterwards by `_forces_as_alone`."""
+    if isinstance(model, eALIGNNAtomWise):
+        return model._forward((g, lat), False, per_crystal=True)
+    return model((g, lg, lat))
+
+
 def _pair_forces_as_alone(model, g, res, A: int) -> torch.Tensor:
     """The model's pair forces with the bond penalty's gradient counted once per crystal (see `_forces_as_alone`)."""
     c = model.config
@@ -126,7 +153,7 @@ def _forces_as_alone(model, g, res, A: int) -> torch.Tensor:
     bit for bit.  No read-back: the correction and the scatter run whether or not any bond is penalised."""
     c = model.config
     grad = res["grad"].detach().reshape(-1, 3)
-    if A == 1 or not c.use_penalty:
+    if A == 1 or not c.use_penalty or isinstance(model, eALIGNNAtomWise):     # eALIGNN: already per crystal
         return grad.contiguous()
     return ops.pair_force_scatter(_pair_forces_as_alone(model, g, res, A), g.index, c.add_reverse_forces)
 
@@ -136,7 +163,7 @@ def _forces_and_stress_as_alone(model, g, res, A: int):
     it A times too, so the per-crystal virial (the model's own, `ops.virial_stress`) is taken again from the corrected
     pair forces.  Without one the model's `stresses` are used as they are."""
     c = model.config
-    if A == 1 or not c.use_penalty:
+    if A == 1 or not c.use_penalty or isinstance(model, eALIGNNAtomWise):
         return res["grad"].detach().reshape(-1, 3).contiguous(), res["stresses"].detach().reshape(-1, 3, 3).contiguous()
     pf = _pair_forces_as_alone(model, g, res, A)
     grad = ops.pair_force_scatter(pf, g.index, c.add_reverse_forces)
@@ -163,12 +190,11 @@ def _evaluate_chunks(model, structures, features, dev, *, neighbor_strategy, cut
             j += 1
         with ops._span(span + "_build", 0):
             feats = torch.cat([features(k) for k in range(j0, j)])
-            g, lg, lat = neighbors.crystal_graphs_device(structures[j0:j], feats, neighbor_strategy=neighbor_strategy,
-                                                         cutoff=cutoff, max_neighbors=max_neighbors,
-                                                         cutoff_extra=cutoff_extra, device=dev)
+            g, lg, lat = _graphs(model, structures[j0:j], feats, dev, neighbor_strategy=neighbor_strategy,
+                                 cutoff=cutoff, max_neighbors=max_neighbors, cutoff_extra=cutoff_extra)
         with ops._span(span + "_model", 0):
             with torch.enable_grad():
-                res = model((g, lg, lat))
+                res = _evaluate(model, g, lg, lat)
                 grad_all[row:row + atoms] = _forces_as_alone(model, g, res, j - j0)
             out = res["out"].detach().reshape(-1)                            # 0-d for a one-crystal batch
             energy[j0:j] = out * g.batch_num_nodes_on_device().to(out.dtype)
@@ -246,7 +272,8 @@ def relax_structures(model, structures, atom_features: torch.Tensor, *, fmax: fl
     `optimize_atoms(optimizer="FIRE", optimize_lattice=False, fmax=fmax, steps=steps)`.  Returns a `RelaxResult`.
     With optimize_lattice=True the cells relax too (see below) and a `CellRelaxResult` is returned.
 
-    model: an `ALIGNNAtomWise` in eval mode on a CUDA device, with calculate_gradient=True and output_features=1.
+    model: an `ALIGNNAtomWise` or `eALIGNNAtomWise` in eval mode on a CUDA device, with calculate_gradient=True and
+    output_features=1; each crystal gets what it would get relaxed alone.
     structures: sequence of (lattice [3,3], cart_coords [n,3]), as for `neighbors.crystal_graphs_device`;
     atom_features: [sum n, F] on the model's device, in the same atom order.
     Graph options are those of `crystal_graphs_device` (defaults: the reference's k-nearest, 8 A, 12 neighbours).
@@ -314,12 +341,12 @@ def relax_structures(model, structures, atom_features: torch.Tensor, *, fmax: fl
         act = torch.tensor(active, dtype=torch.int32).to(dev)
         with ops._span("relax_build", 0):
             feats = atom_features if A == B else atom_features[rows]
-            g, lg, lat = neighbors.crystal_graphs_device([(host_cells[b], host_pos[b]) for b in active], feats,
-                                                         neighbor_strategy=neighbor_strategy, cutoff=cutoff,
-                                                         max_neighbors=max_neighbors, cutoff_extra=cutoff_extra, device=dev)
+            g, lg, lat = _graphs(model, [(host_cells[b], host_pos[b]) for b in active], feats, dev,
+                                 neighbor_strategy=neighbor_strategy, cutoff=cutoff, max_neighbors=max_neighbors,
+                                 cutoff_extra=cutoff_extra)
         with ops._span("relax_model", 0):
             with torch.enable_grad():
-                res = model((g, lg, lat))
+                res = _evaluate(model, g, lg, lat)
                 if cell:
                     grad, stress = _forces_and_stress_as_alone(model, g, res, A)
                 else:

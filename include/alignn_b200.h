@@ -573,6 +573,22 @@ int alignn_b200_remove_net_torque(const float* pos, const float* forces, const i
                                   int64_t num_nodes, int cross_dim0, float* out, void* workspace, size_t workspace_bytes,
                                   alignn_stream_t stream);
 
+/* Per-crystal net-torque removal: `remove_net_torque` (alignn/models/utils.py:295-398) applied to each crystal of the
+ * batch as if it were alone -- what the reference calculator computes for one structure.  For crystal c (atoms
+ * node_offsets[c] .. node_offsets[c+1], n_c of them): com_c = mean of c's positions, tau_c = sum over c's atoms of
+ * r_i x F_i, mu_c = M_c^{-1} (-tau_c) as above (LU, pseudo-inverse on an exactly zero pivot), out_i = F_i + r_i x mu_c;
+ * the column-wise cross of cross_dim0 is used exactly for the crystals with n_c == 3.  Every crystal's rows are bit for
+ * bit what alignn_b200_remove_net_torque gives that crystal as a one-crystal batch: its sums use part_blocks(n_c)
+ * partials with the same striding, block tree and index-order total as such a launch.  One set of five launches for
+ * the whole batch, no float atomics, no host reads.  pos / forces / out [N,3] fp32, node_offsets [B+1] int64 (device).
+ * BAD_ARG: batch_size < 1, num_nodes < 0, a batch too large for the partial-block grid (workspace_bytes() returns 0
+ * then), or a NULL pointer.  The offsets are checked on the device: unless node_offsets[0] == 0, they never decrease
+ * and node_offsets[B] == num_nodes, every row of out is NaN. */
+size_t alignn_b200_remove_net_torque_per_crystal_workspace_bytes(int64_t batch_size, int64_t num_nodes);
+int alignn_b200_remove_net_torque_per_crystal(const float* pos, const float* forces, const int64_t* node_offsets,
+                                              int64_t batch_size, int64_t num_nodes, float* out, void* workspace,
+                                              size_t workspace_bytes, alignn_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Structure relaxation (csrc/fire_device.cu): one step of ASE 3.22.1's FIRE (`FIRE.step`, ase/optimize/fire.py) with
  * the convergence test and step limit of `Optimizer.converged` / `Dynamics.irun` (ase/optimize/optimize.py), for a

@@ -49,6 +49,17 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 
+def _kept_bonds(lat, X, dev, cutoff=4.0):
+    """Bonds eALIGNN keeps in this structure alone: its filter recomputes each bond with the image added as Angstrom
+    (DESIGN section 8) and drops those longer than the 4 A inner cutoff, which can drop them all."""
+    from alignn_b200 import neighbors
+    from alignn_b200.ealignn_atomwise import cartesian_coordinates
+    from alignn_b200.graph import lightweight_graph
+    g, _, lat_t = neighbors.crystal_graphs_device([(lat, X)], torch.zeros(X.shape[0], 1, device=dev), device=dev,
+                                                  neighbor_strategy="radius_graph", cutoff=cutoff, line_graph=False)
+    return lightweight_graph(g, cartesian_coordinates(g, lat_t), cutoff)[0].num_edges()
+
+
 def device_info():
     q = "name,power.limit,clocks.max.sm"
     try:
@@ -64,6 +75,9 @@ def main():
     ap.add_argument("--structures", type=int, default=64)
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--model", choices=("alignn_atomwise", "ealignn"), default="alignn_atomwise",
+                    help="ealignn: a 2+2, d=64 eALIGNNAtomWise on radius_graph 4 A / 12 (the reference's eALIGNN example "
+                         "config); the host arm builds each crystal's graph with crystal_graphs_device")
     ap.add_argument("--ensemble", default="nvt_berendsen",
                     choices=("nvt_berendsen", "nvt_langevin", "nvt_andersen", "npt_berendsen", "npt_nose_hoover"))
     ap.add_argument("--pressure-bar", type=float, default=1.01325)
@@ -77,6 +91,7 @@ def main():
     __graft_entry__.build()
     from alignn_b200 import maxwell_boltzmann_momenta, neighbors, ops, run_md, upper_triangular
     from alignn_b200.alignn_atomwise import ALIGNNAtomWise, ALIGNNAtomWiseConfig
+    from alignn_b200.ealignn_atomwise import eALIGNNAtomWise, eALIGNNAtomWiseConfig
     from oracle import md_nose_hoover_oracle as NH
     from oracle import md_npt_oracle as NO
     from oracle import md_oracle as MO
@@ -90,6 +105,9 @@ def main():
     npt, nh = a.ensemble == "npt_berendsen", a.ensemble == "npt_nose_hoover"
     if a.ensemble in ("nvt_langevin", "nvt_andersen"):         # Langevin (fixcm) rejects one-atom crystals
         pool = pool[off[1:] - off[:-1] >= 2]
+    if a.model == "ealignn":
+        # a crystal whose filtered graph keeps no bond cannot run alone (the one-crystal forward has no edges)
+        pool = np.array([i for i in pool if _kept_bonds(z["lattices"][i], z["cart_coords"][off[i]:off[i + 1]], dev) >= 2 * (off[i + 1] - off[i])])
     pick = rng.choice(pool, min(a.structures, len(pool)), replace=False)
     structs = [(z["lattices"][i], z["cart_coords"][off[i]:off[i + 1]] + rng.normal(scale=0.03, size=(off[i + 1] - off[i], 3)))
                for i in pick]
@@ -101,10 +119,27 @@ def main():
     masses = rng.uniform(1.0, 200.0, sum(sizes))
     p0 = maxwell_boltzmann_momenta(masses, 300.0, rng)
     torch.manual_seed(1)
-    cfg = ALIGNNAtomWiseConfig(name="alignn_atomwise", alignn_layers=4, gcn_layers=4, hidden_features=256,
-                               atom_input_features=92, gradwise_weight=1.0,
-                               stresswise_weight=1.0 if npt or nh else 0.0)
-    model = ALIGNNAtomWise(cfg).to(dev).eval()
+    ea = a.model == "ealignn"
+    if ea:
+        model = eALIGNNAtomWise(eALIGNNAtomWiseConfig(name="ealignn_atomwise", atom_input_features=92,
+                                                      stresswise_weight=1.0 if npt or nh else 0.0)).to(dev).eval()
+        graph = dict(neighbor_strategy="radius_graph", cutoff=4.0, max_neighbors=12)
+    else:
+        cfg = ALIGNNAtomWiseConfig(name="alignn_atomwise", alignn_layers=4, gcn_layers=4, hidden_features=256,
+                                   atom_input_features=92, gradwise_weight=1.0,
+                                   stresswise_weight=1.0 if npt or nh else 0.0)
+        model = ALIGNNAtomWise(cfg).to(dev).eval()
+        graph = dict(neighbor_strategy="k-nearest", cutoff=8.0, max_neighbors=12)
+
+    def one_crystal(cell, x, f_b):
+        """(g, lg, lat) of one crystal as the calculator builds it: on the host for ALIGNNAtomWise; on the device for
+        eALIGNN, which needs the graph's frac_coords and images"""
+        if ea:
+            return neighbors.crystal_graphs_device([(cell, x)], f_b.to(dev), device=dev, **graph)
+        g, lg = neighbors.crystal_graph(cell, x, f_b, **graph)
+        g.ndata["V"] = torch.full((x.shape[0],), abs(float(np.dot(np.cross(cell[0], cell[1]), cell[2]))),
+                                  dtype=torch.float32)
+        return g.to(dev), lg.to(dev), torch.tensor(cell, dtype=torch.float32).view(1, 3, 3).to(dev)
     timestep, T0 = 1.0, 300.0
 
     def batched():
@@ -114,7 +149,7 @@ def main():
         if nh:
             extra = dict(ttime=a.ttime, pfactor=a.pfactor)
         r = run_md(model, structs, feats, masses, ensemble=a.ensemble, steps=a.steps, timestep=timestep,
-                   temperature_K=T0, momenta=p0, **extra)
+                   temperature_K=T0, momenta=p0, **graph, **extra)
         torch.cuda.synchronize()
         return r
 
@@ -126,22 +161,17 @@ def main():
         for b, (lat, X) in enumerate(structs):
             sl = slice(aoff[b], aoff[b + 1])
             f_b = feats[sl].cpu()
-            lat_t = torch.tensor(lat, dtype=torch.float32).view(1, 3, 3).to(dev)
             seen = []
             visited.append(seen)
 
-            def evaluate(x, lat=lat, f_b=f_b, lat_t=lat_t, n=X.shape[0], seen=seen):
+            def evaluate(x, lat=lat, f_b=f_b, n=X.shape[0], seen=seen):
                 seen.append((lat, x.copy()))
-                g, lg = neighbors.crystal_graph(lat, x, f_b, cutoff=8.0, neighbor_strategy="k-nearest", max_neighbors=12)
-                res = model((g.to(dev), lg.to(dev), lat_t))
+                res = model(one_crystal(lat, x, f_b))
                 return float(res["out"].detach() * n), res["grad"].detach().reshape(-1, 3).cpu().numpy()
 
             def evaluate_cell(cell, x, f_b=f_b, n=X.shape[0], seen=seen):
                 seen.append((cell, x.copy()))
-                g, lg = neighbors.crystal_graph(cell, x, f_b, cutoff=8.0, neighbor_strategy="k-nearest", max_neighbors=12)
-                g.ndata["V"] = torch.full((n,), abs(float(np.dot(np.cross(cell[0], cell[1]), cell[2]))),
-                                          dtype=torch.float32)
-                res = model((g.to(dev), lg.to(dev), torch.tensor(cell, dtype=torch.float32).view(1, 3, 3).to(dev)))
+                res = model(one_crystal(cell, x, f_b))
                 return (float(res["out"].detach() * n), res["grad"].detach().reshape(-1, 3).cpu().numpy(),
                         res["stresses"].detach().reshape(3, 3).cpu().numpy())
             dt = timestep * MO.fs
@@ -175,7 +205,7 @@ def main():
     P = got.positions.cpu().numpy()
     T = got.temperature.cpu().numpy()
     dpos = [float(np.abs(P[aoff[b]:aoff[b + 1]] - r["positions"]).max()) for b, r in enumerate(ref)]
-    tied = [any(neighbors.knn_cut_is_tied(c, x) for c, x in seen) for seen in visited]
+    tied = [not ea and any(neighbors.knn_cut_is_tied(c, x) for c, x in seen) for seen in visited]
     parted = [b for b in range(len(structs)) if dpos[b] > 1e-5]
     ops.TIMER = ops.KernelTimer()
     try:
@@ -194,8 +224,9 @@ def main():
         cells_out = {}
     split = {k[len("md_"):]: round(summ[k]["total_ms"] / evals, 3) for k in summ if k.startswith("md_")}
     med_b, med_p = statistics.median(ms["batched"]), statistics.median(ms["per_crystal"])
-    out = dict(workload=f"{len(structs)} jittered sample structures ({sum(sizes)} atoms), ALIGNNAtomWise 4+4 d=256, "
-                        f"k-nearest 8 A / 12, {a.ensemble} 300 K from Maxwell-Boltzmann 300 K, 1 fs, {a.steps} steps "
+    what = "eALIGNNAtomWise 2+2 d=64, radius_graph 4 A / 12" if ea else "ALIGNNAtomWise 4+4 d=256, k-nearest 8 A / 12"
+    out = dict(workload=f"{len(structs)} jittered sample structures ({sum(sizes)} atoms), {what}, "
+                        f"{a.ensemble} 300 K from Maxwell-Boltzmann 300 K, 1 fs, {a.steps} steps "
                         f"({evals} evaluations per crystal)"
                         + (f", {a.pressure_bar} bar, compressibility {a.compressibility} / bar" if npt else "")
                         + (f", upper-triangular cells, ttime {a.ttime} fs, pfactor {a.pfactor}" if nh else ""),

@@ -43,6 +43,17 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 
+def _kept_bonds(lat, X, dev, cutoff=4.0):
+    """Bonds eALIGNN keeps in this structure alone: its filter recomputes each bond with the image added as Angstrom
+    (DESIGN section 8) and drops those longer than the 4 A inner cutoff, which can drop them all."""
+    from alignn_b200 import neighbors
+    from alignn_b200.ealignn_atomwise import cartesian_coordinates
+    from alignn_b200.graph import lightweight_graph
+    g, _, lat_t = neighbors.crystal_graphs_device([(lat, X)], torch.zeros(X.shape[0], 1, device=dev), device=dev,
+                                                  neighbor_strategy="radius_graph", cutoff=cutoff, line_graph=False)
+    return lightweight_graph(g, cartesian_coordinates(g, lat_t), cutoff)[0].num_edges()
+
+
 def device_info():
     q = "name,power.limit,clocks.max.sm"
     try:
@@ -137,6 +148,9 @@ def main():
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--optimize-lattice", action="store_true", help="relax the cells too (ExpCellFilter)")
     ap.add_argument("--optimizer", choices=("FIRE", "LBFGS", "BFGS"), default="FIRE")
+    ap.add_argument("--model", choices=("alignn_atomwise", "ealignn"), default="alignn_atomwise",
+                    help="ealignn: a 2+2, d=64 eALIGNNAtomWise on radius_graph 4 A / 12 (the reference's eALIGNN example "
+                         "config); the host arm builds each crystal's graph with crystal_graphs_device")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_relax.py needs a CUDA device")
@@ -144,6 +158,7 @@ def main():
     __graft_entry__.build()
     from alignn_b200 import neighbors, ops, relax_structures
     from alignn_b200.alignn_atomwise import ALIGNNAtomWise, ALIGNNAtomWiseConfig
+    from alignn_b200.ealignn_atomwise import eALIGNNAtomWise, eALIGNNAtomWiseConfig
     from oracle import cell_filter_oracle as CF
     from oracle import fire_oracle as FO
     from oracle import qn_oracle as QN
@@ -152,7 +167,11 @@ def main():
     z = np.load(os.path.join(ROOT, "tests", "golden", "sample_structures.npz"))
     off = z["atom_offsets"]
     rng = np.random.default_rng(a.seed)
-    pick = rng.choice(len(z["ids"]), a.structures, replace=False)
+    pool = np.arange(len(z["ids"]))
+    if a.model == "ealignn":
+        # a crystal whose filtered graph keeps no bond cannot run alone (the one-crystal forward has no edges)
+        pool = np.array([i for i in pool if _kept_bonds(z["lattices"][i], z["cart_coords"][off[i]:off[i + 1]], dev) >= 2 * (off[i + 1] - off[i])])
+    pick = rng.choice(pool, min(a.structures, len(pool)), replace=False)
     structs = [(z["lattices"][i], z["cart_coords"][off[i]:off[i + 1]] + rng.normal(scale=0.03, size=(off[i + 1] - off[i], 3)))
                for i in pick]
     sizes = [x.shape[0] for _, x in structs]
@@ -166,12 +185,29 @@ def main():
         Ds = [np.eye(3) + np.diag(srng.uniform(-0.04, 0.04, 3)) + srng.uniform(-0.03, 0.03, (3, 3)) for _ in structs]
         structs = [(lat @ D.T, X @ D.T) for (lat, X), D in zip(structs, Ds)]
     torch.manual_seed(1)
-    cfg = ALIGNNAtomWiseConfig(name="alignn_atomwise", alignn_layers=4, gcn_layers=4, hidden_features=256,
-                               atom_input_features=92, gradwise_weight=1.0, stresswise_weight=1.0 if cell else 0.0)
-    model = ALIGNNAtomWise(cfg).to(dev).eval()
+    ea = a.model == "ealignn"
+    if ea:
+        model = eALIGNNAtomWise(eALIGNNAtomWiseConfig(name="ealignn_atomwise", atom_input_features=92,
+                                                      stresswise_weight=1.0 if cell else 0.0)).to(dev).eval()
+        graph = dict(neighbor_strategy="radius_graph", cutoff=4.0, max_neighbors=12)
+    else:
+        cfg = ALIGNNAtomWiseConfig(name="alignn_atomwise", alignn_layers=4, gcn_layers=4, hidden_features=256,
+                                   atom_input_features=92, gradwise_weight=1.0, stresswise_weight=1.0 if cell else 0.0)
+        model = ALIGNNAtomWise(cfg).to(dev).eval()
+        graph = dict(neighbor_strategy="k-nearest", cutoff=8.0, max_neighbors=12)
+
+    def one_crystal(c, x, f_b):
+        """(g, lg, lat) of one crystal as the calculator builds it: on the host for ALIGNNAtomWise; on the device for
+        eALIGNN, which needs the graph's frac_coords and images"""
+        if ea:
+            return neighbors.crystal_graphs_device([(c, x)], f_b.to(dev), device=dev, **graph)
+        g, lg = neighbors.crystal_graph(c, x, f_b, **graph)
+        g.ndata["V"] = torch.full((x.shape[0],), abs(float(np.dot(np.cross(c[0], c[1]), c[2]))), dtype=torch.float32)
+        return g.to(dev), lg.to(dev), torch.tensor(c, dtype=torch.float32).view(1, 3, 3).to(dev)
 
     def batched():
-        r = relax_structures(model, structs, feats, fmax=fmax, steps=a.steps, optimize_lattice=cell, optimizer=a.optimizer)
+        r = relax_structures(model, structs, feats, fmax=fmax, steps=a.steps, optimize_lattice=cell, optimizer=a.optimizer,
+                             **graph)
         torch.cuda.synchronize()
         return r
 
@@ -183,11 +219,9 @@ def main():
         for lat, X in structs:
             n = X.shape[0]
             f_b = feats[o:o + n].cpu()
-            lat_t = torch.tensor(lat, dtype=torch.float32).view(1, 3, 3).to(dev)
 
-            def evaluate(x, lat=lat, f_b=f_b, lat_t=lat_t, n=n):
-                g, lg = neighbors.crystal_graph(lat, x, f_b, cutoff=8.0, neighbor_strategy="k-nearest", max_neighbors=12)
-                res = model((g.to(dev), lg.to(dev), lat_t))
+            def evaluate(x, lat=lat, f_b=f_b, n=n):
+                res = model(one_crystal(lat, x, f_b))
                 return float(res["out"].detach() * n), res["grad"].detach().reshape(-1, 3).cpu().numpy()
 
             seen = []
@@ -195,9 +229,7 @@ def main():
 
             def evaluate_cell(c, x, f_b=f_b, n=n, seen=seen):
                 seen.append((c, x))
-                g, lg = neighbors.crystal_graph(c, x, f_b, cutoff=8.0, neighbor_strategy="k-nearest", max_neighbors=12)
-                g.ndata["V"] = torch.full((n,), abs(float(np.dot(np.cross(c[0], c[1]), c[2]))), dtype=torch.float32)
-                res = model((g.to(dev), lg.to(dev), torch.tensor(c, dtype=torch.float32).view(1, 3, 3).to(dev)))
+                res = model(one_crystal(c, x, f_b))
                 return (float(res["out"].detach() * n), res["grad"].detach().reshape(-1, 3).cpu().numpy(),
                         res["stresses"].detach().reshape(3, 3).cpu().numpy())
             if a.optimizer != "FIRE":
@@ -247,7 +279,7 @@ def main():
         moved = max(float(np.abs(r["cell"] - lat).max()) for r, (lat, _) in zip(ref, structs))
         agree = sum(p <= 1e-5 and c <= 1e-5 for p, c in zip(dpos, dcell))
         # per crystal: does its 12th-neighbour cut fall inside a distance tie at any structure the host arm evaluated?
-        tied = [any(neighbors.knn_cut_is_tied(c, x) for c, x in seen) for seen in visited]
+        tied = [not ea and any(neighbors.knn_cut_is_tied(c, x) for c, x in seen) for seen in visited]
         parted = [b for b in range(len(structs)) if dpos[b] > 1e-5 or dcell[b] > 1e-5]
         extra = {"max_cell_difference_A": max(dcell), "crystals_within_1e-5_A": f"{agree}/{len(structs)}",
                  "crystals_with_a_knn_tie": sum(tied),
@@ -270,8 +302,9 @@ def main():
     what = f"ExpCellFilter {a.optimizer} on atoms and strained, sheared cells" if cell else a.optimizer
     if a.optimizer != "FIRE":
         extra["kernels_alone_ms"] = qn_kernels_alone(a.optimizer, sizes, cell, dev)
-    out = dict(workload=f"{len(structs)} jittered sample structures ({sum(sizes)} atoms), ALIGNNAtomWise 4+4 d=256, "
-                        f"k-nearest 8 A / 12, fmax={fmax}, at most {a.steps} {what} steps",
+    model_s = "eALIGNNAtomWise 2+2 d=64, radius_graph 4 A / 12" if ea else "ALIGNNAtomWise 4+4 d=256, k-nearest 8 A / 12"
+    out = dict(workload=f"{len(structs)} jittered sample structures ({sum(sizes)} atoms), {model_s}, "
+                        f"fmax={fmax}, at most {a.steps} {what} steps",
                batched_ms=[round(v, 1) for v in ms["batched"]], batched_ms_median=round(med_b, 1),
                per_crystal_ms=[round(v, 1) for v in ms["per_crystal"]], per_crystal_ms_median=round(med_p, 1),
                speedup_median=round(med_p / med_b, 2), batched_ms_per_evaluation_split=split,
