@@ -10,16 +10,14 @@ curve (`fit_eos`).  `oracle/eos_oracle.py` is the specification of the fit.
 """
 from __future__ import annotations
 
-import numbers
 from typing import NamedTuple, Optional
 
 import numpy as np
 import torch
 
-from . import neighbors, ops
-from .md import _real
+from . import calculator, neighbors, ops
 from .phonons import DEFAULT_MAX_BATCH_ATOMS
-from .relax import CellRelaxResult, _check_batch, _check_model, _evaluate_chunks, relax_structures
+from .relax import CellRelaxResult, relax_structures
 
 # ase.units (ASE 3.22.1, CODATA 2014): the reference's kv = B / kJ * 1.0e24
 _e = 1.6021766208e-19
@@ -93,9 +91,8 @@ def fit_eos(volumes, energies, eos: str = "murnaghan") -> EOSFit:
 
 
 def _check_options(force_multiplier, max_batch_atoms):
-    if not _real(force_multiplier):
-        raise ValueError(f"force_multiplier must be a finite real number, got {force_multiplier!r}")
-    if isinstance(max_batch_atoms, bool) or not isinstance(max_batch_atoms, numbers.Integral) or max_batch_atoms < 1:
+    calculator.check_real("force_multiplier", force_multiplier)
+    if not calculator.integer(max_batch_atoms) or max_batch_atoms < 1:
         raise ValueError(f"max_batch_atoms must be an integer >= 1, got {max_batch_atoms!r}")
 
 
@@ -109,17 +106,19 @@ def single_point(model, structures, atom_features: torch.Tensor, *, neighbor_str
     The structures are packed greedily, in order, into model calls of at most max_batch_atoms atoms, which must hold
     the largest structure.  energy is out * natoms without the bond penalty; the forces count the penalty once per
     structure."""
-    _check_model("single_point", model)
-    lats, Xs, dev = _check_batch("single_point", model, structures, atom_features, neighbor_strategy, max_neighbors)
+    calculator.check_model("single_point", model)
+    lats, Xs, dev = calculator.check_batch("single_point", model, structures, atom_features, neighbor_strategy,
+                                           max_neighbors)
     _check_options(force_multiplier, max_batch_atoms)
     sizes = [x.shape[0] for x in Xs]
     if max_batch_atoms < max(sizes):
         raise ValueError(f"max_batch_atoms must be at least the largest structure, {max(sizes)} atoms, "
                          f"got {max_batch_atoms!r}")
     aoff = neighbors.ragged_offsets(sizes)
-    energy, grad = _evaluate_chunks(model, list(zip(lats, Xs)), lambda j: atom_features[aoff[j]:aoff[j + 1]], dev,
-                                    neighbor_strategy=neighbor_strategy, cutoff=cutoff, max_neighbors=max_neighbors,
-                                    cutoff_extra=cutoff_extra, max_batch_atoms=max_batch_atoms, span="single_point")
+    graph = dict(neighbor_strategy=neighbor_strategy, cutoff=cutoff, max_neighbors=max_neighbors,
+                 cutoff_extra=cutoff_extra)
+    energy, grad = calculator.evaluate_chunks(model, list(zip(lats, Xs)), lambda j: atom_features[aoff[j]:aoff[j + 1]],
+                                              dev, graph, max_batch_atoms=max_batch_atoms, span="single_point")
     forces = grad * torch.tensor(float(force_multiplier), dtype=torch.float32, device=dev)
     return SinglePointResult(energy, forces, torch.from_numpy(aoff).to(dev))
 
@@ -161,12 +160,11 @@ def ev_curve(model, structures, atom_features: torch.Tensor, *, strains=DEFAULT_
     Non-finite energies raise RuntimeError naming the crystal.  A crystal whose fit has V0 outside its volumes
     (status 1) or no fit (status 2) does not stop the batch: its status says so."""
     _eos_form(eos)
-    _check_model("ev_curve", model)
-    lats, Xs, dev = _check_batch("ev_curve", model, structures, atom_features, neighbor_strategy, max_neighbors)
+    calculator.check_model("ev_curve", model)
+    lats, Xs, dev = calculator.check_batch("ev_curve", model, structures, atom_features, neighbor_strategy, max_neighbors)
     _check_options(force_multiplier, max_batch_atoms)
     st = _strains(strains)
-    if not isinstance(on_relaxed_struct, (bool, np.bool_)):
-        raise ValueError(f"on_relaxed_struct must be a bool, got {on_relaxed_struct!r}")
+    calculator.check_bool("on_relaxed_struct", on_relaxed_struct)
     B, S = len(Xs), st.shape[0]
     sizes = [x.shape[0] for x in Xs]
     if max_batch_atoms < max(sizes):

@@ -22,13 +22,12 @@ from __future__ import annotations
 
 import math
 import numbers
-from typing import NamedTuple, Optional
+from typing import Callable, NamedTuple, Optional
 
 import numpy as np
 import torch
 
-from . import neighbors, ops
-from .relax import _check_batch, _check_model, _evaluate, _forces_and_stress_as_alone, _forces_as_alone, _graphs
+from . import calculator, neighbors, ops
 
 # ase.units (ASE 3.22.1, CODATA 2014): the femtosecond in ASE time units and the Boltzmann constant in eV/K
 _e, _amu, _k = 1.6021766208e-19, 1.660539040e-27, 1.38064852e-23
@@ -79,21 +78,6 @@ def maxwell_boltzmann_momenta(masses, temperature_K: float, rng=None) -> np.ndar
     masses = np.asarray(masses, dtype=np.float64)
     xi = rng.standard_normal((len(masses), 3))
     return xi * np.sqrt(masses * (KB * temperature_K))[:, np.newaxis]
-
-
-def _real(x) -> bool:
-    return not isinstance(x, bool) and isinstance(x, numbers.Real) and math.isfinite(x)
-
-
-def _host_array(x, name: str, shape) -> np.ndarray:
-    a = x.detach().cpu().numpy() if isinstance(x, torch.Tensor) else x
-    try:
-        a = np.asarray(a, dtype=np.float64)
-    except (TypeError, ValueError):
-        raise ValueError(f"{name} must be a real array of shape {list(shape)}") from None
-    if a.shape != tuple(shape) or not np.isfinite(a).all():
-        raise ValueError(f"{name} must be a finite array of shape {list(shape)}, got shape {list(a.shape)}")
-    return a
 
 
 def _seeds(seed, B: int) -> np.ndarray:
@@ -172,38 +156,32 @@ def run_md(model, structures, atom_features: torch.Tensor, masses, *, ensemble: 
     One model evaluation per step, all steps + 1 logged; returns an `NPTResult`.  A cell, or the matrix beta + I of the
     update, that becomes singular or not finite raises RuntimeError naming the crystal and the step.  The other
     ensembles ignore externalstress, ttime and pfactor."""
-    _check_model("run_md", model)
+    calculator.check_model("run_md", model)
     if ensemble not in ENSEMBLES:
         raise ValueError(f"ensemble must be one of {sorted(ENSEMBLES)}, got {ensemble!r}")
-    if isinstance(steps, bool) or not isinstance(steps, numbers.Integral) or not 1 <= steps <= ops.FIRE_MAX_STEPS:
-        raise ValueError(f"steps must be an integer in [1, {ops.FIRE_MAX_STEPS}], got {steps!r}")
-    if not _real(timestep) or not timestep > 0:
-        raise ValueError(f"timestep must be a finite number > 0 (fs), got {timestep!r}")
-    if trajectory_interval is not None and (isinstance(trajectory_interval, bool) or
-                                            not isinstance(trajectory_interval, numbers.Integral) or
-                                            trajectory_interval < 1):
+    calculator.check_steps(steps)
+    calculator.check_positive("timestep", timestep, "fs")
+    if trajectory_interval is not None and (not calculator.integer(trajectory_interval) or trajectory_interval < 1):
         raise ValueError(f"trajectory_interval must be None or an integer >= 1, got {trajectory_interval!r}")
-    lats, Xs, dev = _check_batch("run_md", model, structures, atom_features, neighbor_strategy, max_neighbors)
+    lats, Xs, dev = calculator.check_batch("run_md", model, structures, atom_features, neighbor_strategy, max_neighbors)
     B = len(Xs)
     sizes = [x.shape[0] for x in Xs]
     aoff = neighbors.ragged_offsets(sizes)
     N = int(aoff[-1])
-    m = _host_array(masses, "masses", (N,))
-    if not (m > 0).all():
-        raise ValueError("masses must all be > 0 (amu)")
-    p0 = np.zeros((N, 3)) if momenta is None else _host_array(momenta, "momenta", (N, 3))
+    m = calculator.host_masses(masses, N)
+    p0 = np.zeros((N, 3)) if momenta is None else calculator.host_array(momenta, "momenta", (N, 3))
     dt = float(timestep) * FS
     kind = ENSEMBLES[ensemble]
     T0, taut_ase = None, 0.0
     if kind != ops.MD_NVE:
         t = [temperature_K] * B if np.ndim(temperature_K) == 0 else list(temperature_K)
-        if len(t) != B or not all(_real(v) and v > 0 for v in t):
+        if len(t) != B or not all(calculator.real(v) and v > 0 for v in t):
             raise ValueError(f"temperature_K must be a finite number > 0 or {B} of them, got {temperature_K!r}")
         T0 = torch.tensor([float(v) for v in t], dtype=torch.float64, device=dev)
     if kind in (ops.MD_NVT_BERENDSEN, ops.MD_NPT_BERENDSEN):
         if taut is None:                                # ForceField: taut = 100 * self.timestep, in ASE units (NVT)
             taut_ase = NPT_TAUT if kind == ops.MD_NPT_BERENDSEN else 100 * dt
-        elif not _real(taut):
+        elif not calculator.real(taut):
             raise ValueError(f"taut must be a finite number (fs), got {taut!r}")
         else:
             taut_ase = float(taut) * FS
@@ -213,11 +191,11 @@ def run_md(model, structures, atom_features: torch.Tensor, masses, *, ensemble: 
         seeds = _seeds(seed, B)
         if friction is None:
             fr_ase = LANGEVIN_FRICTION
-        elif not _real(friction) or not friction >= 0:
+        elif not calculator.real(friction) or not friction >= 0:
             raise ValueError(f"friction must be a finite number >= 0 (1/fs) or None, got {friction!r}")
         else:
             fr_ase = float(friction) / FS
-        if not _real(andersen_prob) or not 0.0 <= andersen_prob <= 1.0:
+        if not calculator.real(andersen_prob) or not 0.0 <= andersen_prob <= 1.0:
             raise ValueError(f"andersen_prob must be a number in [0, 1], got {andersen_prob!r}")
         if kind == ops.MD_NVT_LANGEVIN and min(sizes) < 2:
             raise ValueError(f"nvt_langevin needs at least 2 atoms per crystal (fixcm divides by n - 1); crystal "
@@ -229,161 +207,132 @@ def run_md(model, structures, atom_features: torch.Tensor, masses, *, ensemble: 
     pos = torch.from_numpy(np.ascontiguousarray(np.concatenate(Xs))).to(dev)
     mom = torch.from_numpy(np.ascontiguousarray(p0)).to(dev)
     m_d = torch.from_numpy(np.ascontiguousarray(m)).to(dev)
-    if kind == ops.MD_NPT_BERENDSEN:
-        return _run_npt(model, lats, Xs, atom_features, aoff, pos, mom, m_d, T0, dev, steps=int(steps), dt=dt,
-                        taut=taut_ase, pressure=pressure, compressibility=compressibility, taup=taup,
-                        stress_wt=stress_wt, trajectory_interval=trajectory_interval,
-                        graph=dict(neighbor_strategy=neighbor_strategy, cutoff=cutoff, max_neighbors=max_neighbors,
-                                   cutoff_extra=cutoff_extra),
-                        force_multiplier=float(force_multiplier))
-    if kind == ops.MD_NPT_NOSE_HOOVER:
-        return _run_nose_hoover(model, lats, Xs, atom_features, aoff, pos, mom, m_d, T0, dev, steps=int(steps), dt=dt,
-                                externalstress=externalstress, ttime=ttime, pfactor=pfactor, stress_wt=stress_wt,
-                                trajectory_interval=trajectory_interval,
-                                graph=dict(neighbor_strategy=neighbor_strategy, cutoff=cutoff,
-                                           max_neighbors=max_neighbors, cutoff_extra=cutoff_extra),
-                                force_multiplier=float(force_multiplier))
     forces = torch.zeros(N, 3, device=dev, dtype=torch.float32)
-    energy = torch.zeros(steps + 1, B, device=dev, dtype=torch.float32)
-    ekin = torch.zeros(steps + 1, B, device=dev, dtype=torch.float64)
-    temp = torch.zeros(steps + 1, B, device=dev, dtype=torch.float64)
     status = torch.zeros(B, device=dev, dtype=torch.int32)
     aoff_d = torch.from_numpy(aoff).to(dev)
-    host_pos = [x.copy() for x in Xs]
+    npt = kind in (ops.MD_NPT_BERENDSEN, ops.MD_NPT_NOSE_HOOVER)
+    f64 = dict(dtype=torch.float64, device=dev)
+    log = _Log(torch.zeros(steps + 1, B, device=dev, dtype=torch.float32), torch.zeros(steps + 1, B, **f64),
+               torch.zeros(steps + 1, B, **f64), torch.zeros(steps + 1, B, 3, 3, **f64) if npt else None,
+               torch.zeros(steps + 1, B, 6, device=dev, dtype=torch.float32) if npt else None,
+               torch.zeros(steps + 1, B, **f64) if npt else None)
+    run = (aoff_d, m_d, T0, pos, mom, forces, status, log)
+    kw = dict(steps=int(steps), dt=dt, kB=KB, force_multiplier=float(force_multiplier))
+    if kind == ops.MD_NPT_BERENDSEN:
+        ens = _npt_berendsen(model, lats, run, taut=taut_ase, pressure=pressure, compressibility=compressibility,
+                             taup=taup, stress_wt=stress_wt, **kw)
+    elif kind == ops.MD_NPT_NOSE_HOOVER:
+        ens = _nose_hoover(model, lats, sizes, run, externalstress=externalstress, ttime=ttime, pfactor=pfactor,
+                           stress_wt=stress_wt, **kw)
+    elif kind in STOCHASTIC:
+        ens = _Ensemble(lambda e, phase, grad, stress: ops.md_thermostat_step(
+            grad, aoff_d, m_d, T0, seeds_d, pos, mom, vel, rnd_vel, forces, log.kinetic_energy[e], log.temperature[e],
+            status, evaluation=e, ensemble=kind, friction=fr_ase, andersen_prob=float(andersen_prob), **kw),
+            False, None, 1, "md_step", None)
+    else:
+        ens = _Ensemble(lambda e, phase, grad, stress: ops.md_step(
+            grad, aoff_d, m_d, T0, pos, mom, forces, log.kinetic_energy[e], log.temperature[e], status, evaluation=e,
+            ensemble=kind, taut=taut_ase, **kw), False, None, 1, "md_step", None)
+    graph = dict(neighbor_strategy=neighbor_strategy, cutoff=cutoff, max_neighbors=max_neighbors,
+                 cutoff_extra=cutoff_extra)
+    traj = _run(model, lats, Xs, atom_features, dev, graph, ens, pos, status, log, int(steps), trajectory_interval)
+    base = (pos, mom, forces, log.energy, log.kinetic_energy, log.temperature, aoff_d, traj)
+    return MDResult(*base) if ens.cells is None else NPTResult(*base, log.cells, log.stress, log.pressure)
+
+
+class _Log(NamedTuple):
+    """run_md's per-evaluation log, [steps+1, B, ...]: the last three only when the cells move."""
+    energy: torch.Tensor
+    kinetic_energy: torch.Tensor
+    temperature: torch.Tensor
+    cells: Optional[torch.Tensor]
+    stress: Optional[torch.Tensor]
+    pressure: Optional[torch.Tensor]
+
+
+class _Ensemble(NamedTuple):
+    """What run_md's loop needs of an ensemble."""
+    launch: Callable          # launch(e, phase, grad, stress): the step kernel after evaluation e (or its phase 1)
+    stress: bool              # the logged evaluations need the model's stress
+    cells: Optional[torch.Tensor]   # [B,3,3] float64 cells the launches move, or None for fixed cells
+    phases: int               # 2: each step also evaluates, unlogged, at the rescaled structure (NPT Berendsen)
+    kernel: str               # the kernel the MD_BAD_INPUT message names
+    degenerate: Optional[str]   # why a cell is MD_CELL_DEGENERATE, or None where the ensemble has no such status
+
+
+def _run(model, lats, Xs, atom_features, dev, graph, ens: _Ensemble, pos, status, log: _Log, steps: int,
+         trajectory_interval) -> Optional[torch.Tensor]:
+    """run_md's loop for every ensemble: per evaluation e one graph build on the current cells and positions, the model
+    and the ensemble's launch, then one read-back of the statuses and, unless e == steps, the cells and positions of
+    the next evaluation (with `ens.phases` == 2 the step's unlogged evaluation and launch follow, and a second
+    read-back).  Returns the trajectory, or None."""
+    B = len(Xs)
+    sizes = [x.shape[0] for x in Xs]
+    host_cells, host_pos = [np.array(c, dtype=np.float64) for c in lats], [x.copy() for x in Xs]
     traj = []
     for e in range(steps + 1):
-        with ops._span("md_build", 0):
-            g, lg, lat = _graphs(model, list(zip(lats, host_pos)), atom_features, dev,
-                                 neighbor_strategy=neighbor_strategy, cutoff=cutoff, max_neighbors=max_neighbors,
-                                 cutoff_extra=cutoff_extra)
-        with ops._span("md_model", 0):
-            with torch.enable_grad():
-                res = _evaluate(model, g, lg, lat)
-                grad = _forces_as_alone(model, g, res, B)
-            out = res["out"].detach().reshape(-1)                            # 0-d for a one-crystal batch
-            energy[e] = out * g.batch_num_nodes_on_device().to(out.dtype)
+        log.energy[e], grad, stress, _ = calculator.evaluate(model, list(zip(host_cells, host_pos)), atom_features, dev,
+                                                             graph, span="md", stress=ens.stress)
         if trajectory_interval is not None and e % trajectory_interval == 0:
             traj.append(pos.clone())                                         # the positions of evaluation e
-        with ops._span("md_step", 0):
-            if kind in STOCHASTIC:
-                ops.md_thermostat_step(grad, aoff_d, m_d, T0, seeds_d, pos, mom, vel, rnd_vel, forces, ekin[e], temp[e],
-                                       status, evaluation=e, steps=int(steps), dt=dt, kB=KB, ensemble=kind,
-                                       friction=fr_ase, andersen_prob=float(andersen_prob),
-                                       force_multiplier=float(force_multiplier))
-            else:
-                ops.md_step(grad, aoff_d, m_d, T0, pos, mom, forces, ekin[e], temp[e], status, evaluation=e,
-                            steps=int(steps), dt=dt, kB=KB, ensemble=kind, taut=taut_ase,
-                            force_multiplier=float(force_multiplier))
-        with ops._span("md_readback", 0):
-            # one copy: the statuses and, unless this was the last evaluation, the positions of the next one
-            back = torch.cat([status.to(torch.float64)] + ([pos.reshape(-1)] if e < steps else [])).cpu().numpy()
-        if (back[:B] == ops.MD_BAD_INPUT).any():
-            raise RuntimeError("alignn_b200_md_step: the model's forces do not match the crystals' atom counts")
-        if (back[:B] != 0).any():
-            raise RuntimeError(f"run_md: the MD kernel reported statuses {back[:B].astype(int).tolist()}")
+        if ens.cells is not None:
+            log.cells[e] = ens.cells
+        for phase in range(ens.phases if e < steps else 1):
+            if phase == 1:                                                   # evaluation A of step e + 1
+                _, grad, _, _ = calculator.evaluate(model, list(zip(host_cells, host_pos)), atom_features, dev, graph,
+                                                    span="md")
+            with ops._span("md_step", 0):
+                ens.launch(e, phase, grad, stress)
+            # one copy: the statuses and, unless this was the last evaluation, the (cells and) positions of the next
+            st = calculator.read_back("md_readback", status, range(B), sizes, host_pos, pos if e < steps else None,
+                                      host_cells, ens.cells if phase == 0 and e < steps else None)
+            if (st == ops.MD_BAD_INPUT).any():
+                raise RuntimeError(f"alignn_b200_{ens.kernel}: the model's forces do not match the crystals' atom counts")
+            bad = np.flatnonzero(st == ops.MD_CELL_DEGENERATE)
+            if ens.degenerate is not None and bad.size:
+                raise RuntimeError(f"run_md: the cell of crystal {int(bad[0])} became degenerate in step {e + 1} "
+                                   f"({ens.degenerate})")
+            if (st != 0).any():
+                raise RuntimeError(f"run_md: the MD kernel reported statuses {st.astype(int).tolist()}")
         if e == steps:
             break
-        new_pos = back[B:].reshape(-1, 3)
         for b in range(B):
-            host_pos[b] = new_pos[aoff[b]:aoff[b + 1]]
             if not np.isfinite(host_pos[b]).all():
                 raise RuntimeError(f"run_md: the positions of crystal {b} are not finite after step {e + 1}")
-    return MDResult(pos, mom, forces, energy, ekin, temp, aoff_d, torch.stack(traj) if traj else None)
+    return torch.stack(traj) if traj else None
 
 
 def _per_crystal(v, B: int, name: str, unit: str, ok) -> list:
     vals = [v] * B if np.ndim(v) == 0 else list(v)
-    if v is None or len(vals) != B or not all(_real(x) and ok(x) for x in vals):
+    if v is None or len(vals) != B or not all(calculator.real(x) and ok(x) for x in vals):
         raise ValueError(f"npt_berendsen needs {name} ({unit}): a finite number{'' if name == 'pressure' else ' >= 0'} "
                          f"or {B} of them, got {v!r}")
     return [float(x) for x in vals]
 
 
-def _run_npt(model, lats, Xs, atom_features, aoff, pos, mom, m_d, T0, dev, *, steps, dt, taut, pressure,
-             compressibility, taup, stress_wt, trajectory_interval, graph, force_multiplier) -> NPTResult:
-    """run_md's NPT Berendsen loop: per step, phase 0 after the logged evaluation, then evaluation A at the rescaled
+def _npt_berendsen(model, lats, run, *, taut, pressure, compressibility, taup, stress_wt, **kw) -> _Ensemble:
+    """run_md's NPT Berendsen: per step, phase 0 after the logged evaluation, then evaluation A at the rescaled
     structure and phase 1 (see csrc/md_device.cu)."""
-    B, N = len(Xs), int(aoff[-1])
+    aoff_d, m_d, T0, pos, mom, forces, status, log = run
+    B, dev = len(lats), pos.device
     if model.config.stresswise_weight == 0:
         raise ValueError("run_md(ensemble='npt_berendsen') needs a model that computes stress (stresswise_weight != 0)")
     P0 = _per_crystal(pressure, B, "pressure", "bar", lambda x: True)
     comp = _per_crystal(compressibility, B, "compressibility", "1/bar", lambda x: x >= 0)
-    if not _real(taup) or not taup > 0:
-        raise ValueError(f"taup must be a finite number > 0 (fs), got {taup!r}")
-    if not _real(stress_wt):
-        raise ValueError(f"stress_wt must be a finite real number, got {stress_wt!r}")
+    calculator.check_positive("taup", taup, "fs")
+    calculator.check_real("stress_wt", stress_wt)
     f64 = dict(dtype=torch.float64, device=dev)
     P0_d = torch.tensor([v * BAR for v in P0], **f64)          # NPTBerendsen: pressure * (1e5 * units.Pascal)
     comp_d = torch.tensor([v / BAR for v in comp], **f64)      # compressibility / (1e5 * units.Pascal)
     cells = torch.from_numpy(np.ascontiguousarray(np.stack(lats))).to(dev)
-    forces = torch.zeros(N, 3, device=dev, dtype=torch.float32)
-    energy = torch.zeros(steps + 1, B, device=dev, dtype=torch.float32)
-    ekin, temp, press = (torch.zeros(steps + 1, B, **f64) for _ in range(3))
-    cell_log = torch.zeros(steps + 1, B, 3, 3, **f64)
-    stress_log = torch.zeros(steps + 1, B, 6, device=dev, dtype=torch.float32)
-    status = torch.zeros(B, device=dev, dtype=torch.int32)
-    aoff_d = torch.from_numpy(aoff).to(dev)
-    host_cells, host_pos = [np.array(c, dtype=np.float64) for c in lats], [x.copy() for x in Xs]
-    kw = dict(steps=steps, dt=dt, kB=KB, taut=taut, taup=float(taup) * FS, force_multiplier=force_multiplier,
-              stress_wt=float(stress_wt))
-    traj = []
+    kw.update(taut=taut, taup=float(taup) * FS, stress_wt=float(stress_wt))
 
-    def evaluate(with_stress):
-        with ops._span("md_build", 0):
-            g, lg, lat = _graphs(model, list(zip(host_cells, host_pos)), atom_features, dev, **graph)
-        with ops._span("md_model", 0):
-            with torch.enable_grad():
-                res = _evaluate(model, g, lg, lat)
-                if with_stress:
-                    return g, res, _forces_and_stress_as_alone(model, g, res, B)
-                return g, res, (_forces_as_alone(model, g, res, B), None)
-
-    def read_back(e, phase, with_cells):
-        with ops._span("md_readback", 0):
-            # one copy: the statuses, then (the cells and) the positions the next graph build needs
-            back = torch.cat([status.to(torch.float64)] + ([cells.reshape(-1)] if with_cells else []) +
-                             [pos.reshape(-1)]).cpu().numpy()
-        st = back[:B]
-        if (st == ops.MD_BAD_INPUT).any():
-            raise RuntimeError("alignn_b200_md_npt_step: the model's forces do not match the crystals' atom counts")
-        bad = np.flatnonzero(st == ops.MD_CELL_DEGENERATE)
-        if bad.size:
-            raise RuntimeError(f"run_md: the cell of crystal {int(bad[0])} became degenerate in step {e + 1} (its volume "
-                               "or the barostat's scale factor is not finite and positive)")
-        if (st != 0).any():
-            raise RuntimeError(f"run_md: the MD kernel reported statuses {st.astype(int).tolist()}")
-        o = B
-        if with_cells:
-            new_cells = back[B:B + 9 * B].reshape(B, 3, 3)
-            o += 9 * B
-            for b in range(B):
-                host_cells[b] = new_cells[b]
-        new_pos = back[o:].reshape(-1, 3)
-        for b in range(B):
-            host_pos[b] = new_pos[aoff[b]:aoff[b + 1]]
-            if phase == 1 and not np.isfinite(host_pos[b]).all():
-                raise RuntimeError(f"run_md: the positions of crystal {b} are not finite after step {e + 1}")
-
-    for e in range(steps + 1):
-        g, res, (grad, stress) = evaluate(True)                     # logged evaluation e (B of step e)
-        out = res["out"].detach().reshape(-1)
-        energy[e] = out * g.batch_num_nodes_on_device().to(out.dtype)
-        if trajectory_interval is not None and e % trajectory_interval == 0:
-            traj.append(pos.clone())
-        cell_log[e] = cells
-        with ops._span("md_step", 0):
-            ops.md_npt_step(grad, stress, aoff_d, m_d, T0, P0_d, comp_d, cells, pos, mom, forces, stress_log[e], ekin[e],
-                            temp[e], press[e], status, evaluation=e, phase=0, **kw)
-        read_back(e, 0, e < steps)
-        if e == steps:
-            break
-        _, _, (grad, _) = evaluate(False)                           # evaluation A of step e + 1
-        with ops._span("md_step", 0):
-            ops.md_npt_step(grad, stress, aoff_d, m_d, T0, P0_d, comp_d, cells, pos, mom, forces, stress_log[e], ekin[e],
-                            temp[e], press[e], status, evaluation=e, phase=1, **kw)
-        read_back(e, 1, False)
-    return NPTResult(pos, mom, forces, energy, ekin, temp, aoff_d, torch.stack(traj) if traj else None, cell_log,
-                     stress_log, press)
+    def launch(e, phase, grad, stress):
+        ops.md_npt_step(grad, stress, aoff_d, m_d, T0, P0_d, comp_d, cells, pos, mom, forces, log.stress[e],
+                        log.kinetic_energy[e], log.temperature[e], log.pressure[e], status, evaluation=e, phase=phase,
+                        **kw)
+    return _Ensemble(launch, True, cells, 2, "md_npt_step",
+                     "its volume or the barostat's scale factor is not finite and positive")
 
 
 def upper_triangular(structures):
@@ -443,11 +392,11 @@ def _nose_hoover_constants(sizes, T0, ttime, pfactor, cells):
     return tf, pf, de
 
 
-def _run_nose_hoover(model, lats, Xs, atom_features, aoff, pos, mom, m_d, T0, dev, *, steps, dt, externalstress,
-                     ttime, pfactor, stress_wt, trajectory_interval, graph, force_multiplier) -> NPTResult:
-    """run_md's loop for ASE's NPT: per evaluation e one graph build on the current cells, the model with stress and one
-    `md_nose_hoover_step` launch (see csrc/md_device.cu)."""
-    B, N = len(Xs), int(aoff[-1])
+def _nose_hoover(model, lats, sizes, run, *, externalstress, ttime, pfactor, stress_wt, **kw) -> _Ensemble:
+    """run_md's ASE NPT: per evaluation e one `md_nose_hoover_step` launch on the model's forces and stress (see
+    csrc/md_device.cu)."""
+    aoff_d, m_d, T0, pos, mom, forces, status, log = run
+    B, N, dev = len(lats), pos.shape[0], pos.device
     if model.config.stresswise_weight == 0:
         raise ValueError("run_md(ensemble='npt_nose_hoover') needs a model that computes stress (stresswise_weight != 0)")
     for b, lat in enumerate(lats):
@@ -455,16 +404,15 @@ def _run_nose_hoover(model, lats, Xs, atom_features, aoff, pos, mom, m_d, T0, de
             raise ValueError(f"run_md(ensemble='npt_nose_hoover'): the cell of crystal {b} is not upper triangular; ASE's "
                              "NPT needs lattice rows a, b, c with b in the yz-plane and c along z "
                              "(alignn_b200.upper_triangular rotates structures into that form)")
-    if ttime is not None and not (_real(ttime) and ttime > 0):
+    if ttime is not None and not (calculator.real(ttime) and ttime > 0):
         raise ValueError(f"ttime must be None or a finite number > 0 (fs), got {ttime!r}")
-    if pfactor is not None and not (_real(pfactor) and pfactor > 0):
+    if pfactor is not None and not (calculator.real(pfactor) and pfactor > 0):
         raise ValueError(f"pfactor must be None or a finite number > 0 (ASE units, amu/A), got {pfactor!r}")
-    if not _real(stress_wt):
-        raise ValueError(f"stress_wt must be a finite real number, got {stress_wt!r}")
+    calculator.check_real("stress_wt", stress_wt)
     if externalstress is None and pfactor is not None:
         raise ValueError("run_md(ensemble='npt_nose_hoover'): pfactor needs an externalstress")
     ext = _external_stress(0.0 if externalstress is None else externalstress, B)
-    tf, pf, de = _nose_hoover_constants(np.diff(aoff), T0.cpu().tolist(), None if ttime is None else float(ttime) * FS,
+    tf, pf, de = _nose_hoover_constants(sizes, T0.cpu().tolist(), None if ttime is None else float(ttime) * FS,
                                         None if pfactor is None else float(pfactor), lats)
     f64 = dict(dtype=torch.float64, device=dev)
     tf_d, pf_d, de_d = (torch.tensor(v, **f64) for v in (tf, pf, de))
@@ -472,52 +420,11 @@ def _run_nose_hoover(model, lats, Xs, atom_features, aoff, pos, mom, m_d, T0, de
     cells = torch.from_numpy(np.ascontiguousarray(np.stack(lats))).to(dev)
     state = torch.zeros(B, ops.MD_NH_STATE, **f64)
     q, q_future = torch.zeros(N, 3, **f64), torch.zeros(N, 3, **f64)
-    forces = torch.zeros(N, 3, device=dev, dtype=torch.float32)
-    energy = torch.zeros(steps + 1, B, device=dev, dtype=torch.float32)
-    ekin, temp, press = (torch.zeros(steps + 1, B, **f64) for _ in range(3))
-    cell_log = torch.zeros(steps + 1, B, 3, 3, **f64)
-    stress_log = torch.zeros(steps + 1, B, 6, device=dev, dtype=torch.float32)
-    status = torch.zeros(B, device=dev, dtype=torch.int32)
-    aoff_d = torch.from_numpy(aoff).to(dev)
-    host_cells, host_pos = [np.array(c, dtype=np.float64) for c in lats], [x.copy() for x in Xs]
-    traj = []
-    for e in range(steps + 1):
-        with ops._span("md_build", 0):
-            g, lg, lat = _graphs(model, list(zip(host_cells, host_pos)), atom_features, dev, **graph)
-        with ops._span("md_model", 0):
-            with torch.enable_grad():
-                res = _evaluate(model, g, lg, lat)
-                grad, stress = _forces_and_stress_as_alone(model, g, res, B)
-            out = res["out"].detach().reshape(-1)
-            energy[e] = out * g.batch_num_nodes_on_device().to(out.dtype)
-        if trajectory_interval is not None and e % trajectory_interval == 0:
-            traj.append(pos.clone())
-        cell_log[e] = cells
-        with ops._span("md_step", 0):
-            ops.md_nose_hoover_step(grad, stress, aoff_d, m_d, tf_d, pf_d, de_d, ext_d, cells, state, pos, mom, q,
-                                    q_future, forces, stress_log[e], ekin[e], temp[e], press[e], status, evaluation=e,
-                                    steps=steps, dt=dt, kB=KB, force_multiplier=force_multiplier,
-                                    stress_wt=float(stress_wt))
-        with ops._span("md_readback", 0):
-            # one copy: the statuses and, unless this was the last evaluation, the next cells and positions
-            back = torch.cat([status.to(torch.float64)] +
-                             ([cells.reshape(-1), pos.reshape(-1)] if e < steps else [])).cpu().numpy()
-        st = back[:B]
-        if (st == ops.MD_BAD_INPUT).any():
-            raise RuntimeError("alignn_b200_md_nose_hoover_step: the model's forces do not match the crystals' atom "
-                               "counts")
-        bad = np.flatnonzero(st == ops.MD_CELL_DEGENERATE)
-        if bad.size:
-            raise RuntimeError(f"run_md: the cell of crystal {int(bad[0])} became degenerate in step {e + 1} (its "
-                               "determinant, or that of the update's beta + I, is not finite and nonzero)")
-        if (st != 0).any():
-            raise RuntimeError(f"run_md: the MD kernel reported statuses {st.astype(int).tolist()}")
-        if e == steps:
-            break
-        new_cells, new_pos = back[B:10 * B].reshape(B, 3, 3), back[10 * B:].reshape(-1, 3)
-        for b in range(B):
-            host_cells[b], host_pos[b] = new_cells[b], new_pos[aoff[b]:aoff[b + 1]]
-            if not np.isfinite(host_pos[b]).all():
-                raise RuntimeError(f"run_md: the positions of crystal {b} are not finite after step {e + 1}")
-    return NPTResult(pos, mom, forces, energy, ekin, temp, aoff_d, torch.stack(traj) if traj else None, cell_log,
-                     stress_log, press)
+    kw.update(stress_wt=float(stress_wt))
+
+    def launch(e, phase, grad, stress):
+        ops.md_nose_hoover_step(grad, stress, aoff_d, m_d, tf_d, pf_d, de_d, ext_d, cells, state, pos, mom, q, q_future,
+                                forces, log.stress[e], log.kinetic_energy[e], log.temperature[e], log.pressure[e],
+                                status, evaluation=e, **kw)
+    return _Ensemble(launch, True, cells, 1, "md_nose_hoover_step",
+                     "its determinant, or that of the update's beta + I, is not finite and nonzero")

@@ -412,6 +412,38 @@ FIRE_BAD_INPUT = 3            # istate status of a crystal whose batch slice doe
 FIRE_MAX_STEPS = 2 ** 31 - 1  # steps travels as an int32
 
 
+def _operands(name, want, device) -> None:
+    """The device, dtype and contiguity checks of the wrapper `name`: every (tensor, dtype or tuple of dtypes) pair of
+    `want` is a contiguous CUDA tensor of that dtype on `device`."""
+    for t, dt in want:
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != device:
+            got = t.device if isinstance(t, torch.Tensor) else type(t).__name__
+            raise RuntimeError(f"{name} needs all operands on one CUDA device; got {got} and {device}")
+        if (t.dtype not in dt if isinstance(dt, tuple) else t.dtype != dt) or not t.is_contiguous():
+            raise RuntimeError(f"{name}: expected a contiguous {dt} tensor, got {t.dtype}")
+
+
+def _check_int(name, what, v, lo, hi, hi_text=None) -> None:
+    """v is an integer in [lo, hi] (hi_text: how the message names hi)."""
+    if isinstance(v, bool) or int(v) != v or not lo <= int(v) <= hi:
+        raise ValueError(f"{name}: {what} must be an integer in [{lo}, {hi_text or hi}], got {v!r}")
+
+
+def _md_counts(name, steps, evaluation) -> None:
+    _check_int(name, "steps", steps, 1, FIRE_MAX_STEPS)
+    _check_int(name, "evaluation", evaluation, 0, int(steps), "steps")
+
+
+def _fire_params(name, fire, fmax, steps, force_multiplier):
+    """The FireParams of one FIRE step: FIRE_DEFAULTS overridden by `fire`."""
+    par = dict(FIRE_DEFAULTS, **fire)
+    _check_int(name, "steps", steps, 1, FIRE_MAX_STEPS)
+    _check_int(name, "n_min", par["n_min"], 0, FIRE_MAX_STEPS)
+    return _lib.FireParams(float(par["maxstep"]), float(par["dtmax"]), float(par["finc"]), float(par["fdec"]),
+                           float(par["astart"]), float(par["fa"]), float(fmax), int(par["n_min"]), int(steps),
+                           float(force_multiplier))
+
+
 @_on_tensor_device
 def fire_step(grad: torch.Tensor, active: torch.Tensor, batch_offsets: torch.Tensor, atom_offsets: torch.Tensor,
               positions: torch.Tensor, velocities: torch.Tensor, forces: torch.Tensor, fstate: torch.Tensor,
@@ -426,27 +458,15 @@ def fire_step(grad: torch.Tensor, active: torch.Tensor, batch_offsets: torch.Ten
     FIRE_BAD_INPUT: slice j is not crystal active[j]'s atoms or lies outside grad -- nothing else is read or written for
     that crystal)}.  Enqueue only: the statuses are the caller's to read back.  `fire` overrides FIRE_DEFAULTS."""
     lib = _lib.load()
-    par = dict(FIRE_DEFAULTS, **fire)
-    want = ((grad, torch.float32), (active, torch.int32), (batch_offsets, torch.int32), (atom_offsets, torch.int64),
-            (positions, torch.float64), (velocities, torch.float64), (forces, torch.float32), (fstate, torch.float64),
-            (istate, torch.int32))
-    for t, dt in want:
-        if not t.is_cuda or t.device != grad.device:
-            raise RuntimeError(f"fire_step needs all operands on one CUDA device; got {t.device} and {grad.device}")
-        if t.dtype != dt or not t.is_contiguous():
-            raise RuntimeError(f"fire_step: expected a contiguous {dt} tensor, got {t.dtype}")
+    _operands("fire_step", ((grad, torch.float32), (active, torch.int32), (batch_offsets, torch.int32),
+                            (atom_offsets, torch.int64), (positions, torch.float64), (velocities, torch.float64),
+                            (forces, torch.float32), (fstate, torch.float64), (istate, torch.int32)), grad.device)
     B, A = atom_offsets.numel() - 1, active.numel()
     N = positions.numel() // 3
     if (velocities.numel() != 3 * N or forces.numel() != 3 * N or fstate.numel() != 2 * B or istate.numel() != 4 * B
             or batch_offsets.numel() != A + 1 or grad.dim() != 2 or grad.shape[1] != 3):
         raise ValueError("fire_step: inconsistent operand shapes")
-    if isinstance(steps, bool) or int(steps) != steps or not 1 <= int(steps) <= FIRE_MAX_STEPS:
-        raise ValueError(f"fire_step: steps must be an integer in [1, {FIRE_MAX_STEPS}], got {steps!r}")
-    if not 0 <= int(par["n_min"]) <= FIRE_MAX_STEPS:
-        raise ValueError(f"fire_step: n_min must be in [0, {FIRE_MAX_STEPS}], got {par['n_min']!r}")
-    p = _lib.FireParams(float(par["maxstep"]), float(par["dtmax"]), float(par["finc"]), float(par["fdec"]),
-                        float(par["astart"]), float(par["fa"]), float(fmax), int(par["n_min"]), int(steps),
-                        float(force_multiplier))
+    p = _fire_params("fire_step", fire, fmax, steps, force_multiplier)
     _lib.check(lib.alignn_b200_fire_step(C.byref(p), active.data_ptr(), A, atom_offsets.data_ptr(), batch_offsets.data_ptr(),
                                          B, grad.data_ptr(), grad.shape[0], positions.data_ptr(), velocities.data_ptr(), forces.data_ptr(),
                                          fstate.data_ptr(), istate.data_ptr(), stream_ptr()), "alignn_b200_fire_step")
@@ -471,17 +491,12 @@ def fire_cell_step(grad: torch.Tensor, stress: torch.Tensor, active: torch.Tenso
     initially I), cells (C = C0 F^T, initially cells0), cell_velocities (initially 0).  Status FIRE_CELL_DEGENERATE:
     the cell's volume is not finite and > 0, or expm(L) is not finite; the crystal is frozen."""
     lib = _lib.load()
-    par = dict(FIRE_DEFAULTS, **fire)
-    want = ((grad, torch.float32), (stress, torch.float32), (active, torch.int32), (batch_offsets, torch.int32),
-            (atom_offsets, torch.int64), (positions, torch.float64), (velocities, torch.float64), (forces, torch.float32),
-            (cells0, torch.float64), (logdef, torch.float64), (defgrad, torch.float64), (cells, torch.float64),
-            (cell_velocities, torch.float64), (cell_forces, torch.float64), (stress_out, torch.float32),
-            (fstate, torch.float64), (istate, torch.int32))
-    for t, dt in want:
-        if not t.is_cuda or t.device != grad.device:
-            raise RuntimeError(f"fire_cell_step needs all operands on one CUDA device; got {t.device} and {grad.device}")
-        if t.dtype != dt or not t.is_contiguous():
-            raise RuntimeError(f"fire_cell_step: expected a contiguous {dt} tensor, got {t.dtype}")
+    _operands("fire_cell_step",
+              ((grad, torch.float32), (stress, torch.float32), (active, torch.int32), (batch_offsets, torch.int32),
+               (atom_offsets, torch.int64), (positions, torch.float64), (velocities, torch.float64),
+               (forces, torch.float32), (cells0, torch.float64), (logdef, torch.float64), (defgrad, torch.float64),
+               (cells, torch.float64), (cell_velocities, torch.float64), (cell_forces, torch.float64),
+               (stress_out, torch.float32), (fstate, torch.float64), (istate, torch.int32)), grad.device)
     B, A = atom_offsets.numel() - 1, active.numel()
     N = positions.numel() // 3
     if (velocities.numel() != 3 * N or forces.numel() != 3 * N or fstate.numel() != 2 * B or istate.numel() != 4 * B
@@ -489,13 +504,7 @@ def fire_cell_step(grad: torch.Tensor, stress: torch.Tensor, active: torch.Tenso
             or stress.numel() != 9 * A or stress_out.numel() != 6 * B
             or any(t.numel() != 9 * B for t in (cells0, logdef, defgrad, cells, cell_velocities, cell_forces))):
         raise ValueError("fire_cell_step: inconsistent operand shapes")
-    if isinstance(steps, bool) or int(steps) != steps or not 1 <= int(steps) <= FIRE_MAX_STEPS:
-        raise ValueError(f"fire_cell_step: steps must be an integer in [1, {FIRE_MAX_STEPS}], got {steps!r}")
-    if not 0 <= int(par["n_min"]) <= FIRE_MAX_STEPS:
-        raise ValueError(f"fire_cell_step: n_min must be in [0, {FIRE_MAX_STEPS}], got {par['n_min']!r}")
-    p = _lib.FireCellParams(_lib.FireParams(float(par["maxstep"]), float(par["dtmax"]), float(par["finc"]),
-                                            float(par["fdec"]), float(par["astart"]), float(par["fa"]), float(fmax),
-                                            int(par["n_min"]), int(steps), float(force_multiplier)), float(stress_wt))
+    p = _lib.FireCellParams(_fire_params("fire_cell_step", fire, fmax, steps, force_multiplier), float(stress_wt))
     _lib.check(lib.alignn_b200_fire_cell_step(C.byref(p), active.data_ptr(), A, atom_offsets.data_ptr(), batch_offsets.data_ptr(),
                                               B, grad.data_ptr(), grad.shape[0], stress.data_ptr(), A, positions.data_ptr(),
                                               velocities.data_ptr(), forces.data_ptr(), cells0.data_ptr(), logdef.data_ptr(),
@@ -518,11 +527,7 @@ def _qn_operands(name, grad, stress, active, batch_offsets, atom_offsets, positi
     want += [(t, torch.float64) for t in rows_ops]
     if cell:
         want += [(stress, torch.float32), (cell_ops[-1], torch.float32)] + [(t, torch.float64) for t in cell_ops[:-1]]
-    for t, dt in want:
-        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != grad.device:
-            raise RuntimeError(f"{name} needs all operands on one CUDA device")
-        if t.dtype != dt or not t.is_contiguous():
-            raise RuntimeError(f"{name}: expected a contiguous {dt} tensor, got {t.dtype}")
+    _operands(name, want, grad.device)
     B, A = atom_offsets.numel() - 1, active.numel()
     N = positions.numel() // 3
     rows = N + 3 * B if cell else N
@@ -531,8 +536,7 @@ def _qn_operands(name, grad, stress, active, batch_offsets, atom_offsets, positi
             or (cell and (stress.numel() != 9 * A or cell_ops[-1].numel() != 6 * B
                           or any(t.numel() != 9 * B for t in cell_ops[:-1])))):
         raise ValueError(f"{name}: inconsistent operand shapes")
-    if isinstance(steps, bool) or int(steps) != steps or not 1 <= int(steps) <= FIRE_MAX_STEPS:
-        raise ValueError(f"{name}: steps must be an integer in [1, {FIRE_MAX_STEPS}], got {steps!r}")
+    _check_int(name, "steps", steps, 1, FIRE_MAX_STEPS)
     return B, A, N, rows, cell
 
 
@@ -565,8 +569,7 @@ def lbfgs_step(grad: torch.Tensor, stress, active: torch.Tensor, batch_offsets: 
             or slots < 1):
         raise ValueError("lbfgs_step: inconsistent operand shapes")
     memory = par["memory"]
-    if isinstance(memory, bool) or int(memory) != memory or not 1 <= int(memory) <= FIRE_MAX_STEPS:
-        raise ValueError(f"lbfgs_step: memory must be an integer >= 1, got {memory!r}")
+    _check_int("lbfgs_step", "memory", memory, 1, FIRE_MAX_STEPS)
     p = _lib.LbfgsParams(float(par["maxstep"]), float(par["alpha"]), float(par["damping"]), float(fmax), int(memory),
                          int(slots), int(steps), int(cell), float(force_multiplier), float(stress_wt))
     c0, ld, dg, ce, cf, so = _cell_ptrs(cell, cell_ops)
@@ -626,11 +629,7 @@ def bfgs_apply(group: torch.Tensor, omega: torch.Tensor, eigenvectors: torch.Ten
             (positions, torch.float64), (r0, torch.float64), (f0, torch.float64), (r, torch.float64), (f, torch.float64),
             (work, torch.float64), (istate, torch.int32)]
     want += [(t, torch.float64) for t in (cells0, logdef, defgrad, cells)] if cell else []
-    for t, dt in want:
-        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != r.device:
-            raise RuntimeError("bfgs_apply needs all operands on one CUDA device")
-        if t.dtype != dt or not t.is_contiguous():
-            raise RuntimeError(f"bfgs_apply: expected a contiguous {dt} tensor, got {t.dtype}")
+    _operands("bfgs_apply", want, r.device)
     if (omega.dim() != 2 or omega.shape[0] != G or tuple(eigenvectors.shape) != (G, dim, dim) or work.numel() != 9 * rows
             or any(t.numel() != 3 * rows for t in (r0, f0, f)) or istate.numel() != 4 * B):
         raise ValueError("bfgs_apply: inconsistent operand shapes")
@@ -668,11 +667,7 @@ def md_step(grad: torch.Tensor, atom_offsets: torch.Tensor, masses: torch.Tensor
             (temperature, torch.float64), (status, torch.int32)]
     if target_temperature is not None:
         want.append((target_temperature, torch.float64))
-    for t, dt_ in want:
-        if not t.is_cuda or t.device != grad.device:
-            raise RuntimeError(f"md_step needs all operands on one CUDA device; got {t.device} and {grad.device}")
-        if t.dtype != dt_ or not t.is_contiguous():
-            raise RuntimeError(f"md_step: expected a contiguous {dt_} tensor, got {t.dtype}")
+    _operands("md_step", want, grad.device)
     B = atom_offsets.numel() - 1
     N = positions.numel() // 3
     if (B < 1 or positions.numel() != 3 * N or momenta.numel() != 3 * N or forces.numel() != 3 * N
@@ -682,10 +677,7 @@ def md_step(grad: torch.Tensor, atom_offsets: torch.Tensor, masses: torch.Tensor
         raise ValueError("md_step: inconsistent operand shapes")
     if ensemble == MD_NVT_BERENDSEN and target_temperature is None:
         raise ValueError("md_step: NVT Berendsen needs target_temperature")
-    if isinstance(steps, bool) or int(steps) != steps or not 1 <= int(steps) <= FIRE_MAX_STEPS:
-        raise ValueError(f"md_step: steps must be an integer in [1, {FIRE_MAX_STEPS}], got {steps!r}")
-    if isinstance(evaluation, bool) or int(evaluation) != evaluation or not 0 <= int(evaluation) <= int(steps):
-        raise ValueError(f"md_step: evaluation must be an integer in [0, steps], got {evaluation!r}")
+    _md_counts("md_step", steps, evaluation)
     p = _lib.MdParams(float(dt), float(taut), float(kB), int(evaluation), int(steps), int(ensemble), float(force_multiplier))
     _lib.check(lib.alignn_b200_md_step(C.byref(p), atom_offsets.data_ptr(), B, grad.data_ptr(), grad.shape[0],
                                        masses.data_ptr(),
@@ -697,15 +689,6 @@ def md_step(grad: torch.Tensor, atom_offsets: torch.Tensor, masses: torch.Tensor
 
 MD_NVT_LANGEVIN, MD_NVT_ANDERSEN = 2, 3   # alignn_b200_md_thermostat_params.ensemble, also the noise stream's tags
 MD_ONE_ATOM = 6                           # status of a one-atom crystal under Langevin (ASE divides by n - 1)
-
-
-def _md_operands(what, want, device):
-    for t, dt_ in want:
-        if not t.is_cuda or t.device != device:
-            raise RuntimeError(f"{what} needs all operands on one CUDA device; got {t.device} and {device}")
-        ok = t.dtype in dt_ if isinstance(dt_, tuple) else t.dtype == dt_
-        if not ok or not t.is_contiguous():
-            raise RuntimeError(f"{what}: expected a contiguous {dt_} tensor, got {t.dtype}")
 
 
 @_on_tensor_device
@@ -726,12 +709,12 @@ def md_thermostat_step(grad: torch.Tensor, atom_offsets: torch.Tensor, masses: t
     andersen_prob per component and step.  sqrt(dt), dt ** 1.5 and 2 sqrt(3) are formed here, on the host, as numpy
     forms them.  Enqueue only: the statuses are the caller's to read back."""
     lib = _lib.load()
-    _md_operands("md_thermostat_step",
-                 [(grad, torch.float32), (atom_offsets, torch.int64), (masses, torch.float64),
-                  (target_temperature, torch.float64), (seeds, (torch.int64, torch.uint64)), (positions, torch.float64),
-                  (momenta, torch.float64), (velocities, torch.float64), (rnd_vel, torch.float64),
-                  (forces, torch.float32), (kinetic_energy, torch.float64), (temperature, torch.float64),
-                  (status, torch.int32)], grad.device)
+    _operands("md_thermostat_step",
+              [(grad, torch.float32), (atom_offsets, torch.int64), (masses, torch.float64),
+               (target_temperature, torch.float64), (seeds, (torch.int64, torch.uint64)), (positions, torch.float64),
+               (momenta, torch.float64), (velocities, torch.float64), (rnd_vel, torch.float64),
+               (forces, torch.float32), (kinetic_energy, torch.float64), (temperature, torch.float64),
+               (status, torch.int32)], grad.device)
     B = atom_offsets.numel() - 1
     N = positions.numel() // 3
     if (B < 1 or positions.numel() != 3 * N or any(t.numel() != 3 * N for t in (momenta, velocities, rnd_vel, forces))
@@ -739,10 +722,7 @@ def md_thermostat_step(grad: torch.Tensor, atom_offsets: torch.Tensor, masses: t
                                                                      target_temperature, seeds))
             or grad.dim() != 2 or grad.shape[1] != 3 or grad.shape[0] > N):
         raise ValueError("md_thermostat_step: inconsistent operand shapes")
-    if isinstance(steps, bool) or int(steps) != steps or not 1 <= int(steps) <= FIRE_MAX_STEPS:
-        raise ValueError(f"md_thermostat_step: steps must be an integer in [1, {FIRE_MAX_STEPS}], got {steps!r}")
-    if isinstance(evaluation, bool) or int(evaluation) != evaluation or not 0 <= int(evaluation) <= int(steps):
-        raise ValueError(f"md_thermostat_step: evaluation must be an integer in [0, steps], got {evaluation!r}")
+    _md_counts("md_thermostat_step", steps, evaluation)
     dt = float(dt)
     ok = math.isfinite(dt) and dt > 0                  # anything else the library rejects
     root_dt = math.sqrt(dt) if ok else float("nan")    # np.sqrt(dt): both correctly rounded
@@ -780,13 +760,13 @@ def md_npt_step(grad: torch.Tensor, stress: torch.Tensor, atom_offsets: torch.Te
     MD_CELL_DEGENERATE for a cell whose volume or barostat scale is not finite and > 0 (nothing of the crystal is
     written).  dt, taut and taup in ASE time units.  Enqueue only: the statuses are the caller's to read back."""
     lib = _lib.load()
-    _md_operands("md_npt_step",
-                 [(grad, torch.float32), (stress, torch.float32), (atom_offsets, torch.int64), (masses, torch.float64),
-                  (target_temperature, torch.float64), (target_pressure, torch.float64),
-                  (compressibility, torch.float64), (cells, torch.float64), (positions, torch.float64),
-                  (momenta, torch.float64), (forces, torch.float32), (stress_out, torch.float32),
-                  (kinetic_energy, torch.float64), (temperature, torch.float64), (pressure, torch.float64),
-                  (status, torch.int32)], grad.device)
+    _operands("md_npt_step",
+              [(grad, torch.float32), (stress, torch.float32), (atom_offsets, torch.int64), (masses, torch.float64),
+               (target_temperature, torch.float64), (target_pressure, torch.float64),
+               (compressibility, torch.float64), (cells, torch.float64), (positions, torch.float64),
+               (momenta, torch.float64), (forces, torch.float32), (stress_out, torch.float32),
+               (kinetic_energy, torch.float64), (temperature, torch.float64), (pressure, torch.float64),
+               (status, torch.int32)], grad.device)
     B = atom_offsets.numel() - 1
     N = positions.numel() // 3
     if (B < 1 or positions.numel() != 3 * N or momenta.numel() != 3 * N or forces.numel() != 3 * N
@@ -795,10 +775,7 @@ def md_npt_step(grad: torch.Tensor, stress: torch.Tensor, atom_offsets: torch.Te
                                              temperature, pressure, status))
             or grad.dim() != 2 or grad.shape[1] != 3 or grad.shape[0] > N):
         raise ValueError("md_npt_step: inconsistent operand shapes")
-    if isinstance(steps, bool) or int(steps) != steps or not 1 <= int(steps) <= FIRE_MAX_STEPS:
-        raise ValueError(f"md_npt_step: steps must be an integer in [1, {FIRE_MAX_STEPS}], got {steps!r}")
-    if isinstance(evaluation, bool) or int(evaluation) != evaluation or not 0 <= int(evaluation) <= int(steps):
-        raise ValueError(f"md_npt_step: evaluation must be an integer in [0, steps], got {evaluation!r}")
+    _md_counts("md_npt_step", steps, evaluation)
     p = _lib.MdNptParams(float(dt), float(taut), float(taup), float(kB), int(evaluation), int(steps), int(phase),
                          float(force_multiplier), float(stress_wt))
     _lib.check(lib.alignn_b200_md_npt_step(
@@ -835,12 +812,12 @@ def md_nose_hoover_step(grad: torch.Tensor, stress: torch.Tensor, atom_offsets: 
     dt in ASE time units.  Enqueue only: the statuses are the caller's to read back."""
     lib = _lib.load()
     f64 = torch.float64
-    _md_operands("md_nose_hoover_step",
-                 [(grad, torch.float32), (stress, torch.float32), (atom_offsets, torch.int64), (masses, f64),
-                  (tfact, f64), (pfact, f64), (desired_ekin, f64), (external_stress, f64), (cells, f64), (state, f64),
-                  (positions, f64), (momenta, f64), (q, f64), (q_future, f64), (forces, torch.float32),
-                  (stress_out, torch.float32), (kinetic_energy, f64), (temperature, f64), (pressure, f64),
-                  (status, torch.int32)], grad.device)
+    _operands("md_nose_hoover_step",
+              [(grad, torch.float32), (stress, torch.float32), (atom_offsets, torch.int64), (masses, f64),
+               (tfact, f64), (pfact, f64), (desired_ekin, f64), (external_stress, f64), (cells, f64), (state, f64),
+               (positions, f64), (momenta, f64), (q, f64), (q_future, f64), (forces, torch.float32),
+               (stress_out, torch.float32), (kinetic_energy, f64), (temperature, f64), (pressure, f64),
+               (status, torch.int32)], grad.device)
     B = atom_offsets.numel() - 1
     N = positions.numel() // 3
     if (B < 1 or positions.numel() != 3 * N or any(t.numel() != 3 * N for t in (momenta, q, q_future, forces))
@@ -849,10 +826,7 @@ def md_nose_hoover_step(grad: torch.Tensor, stress: torch.Tensor, atom_offsets: 
             or any(t.numel() != B for t in (tfact, pfact, desired_ekin, kinetic_energy, temperature, pressure, status))
             or grad.dim() != 2 or grad.shape[1] != 3 or grad.shape[0] > N):
         raise ValueError("md_nose_hoover_step: inconsistent operand shapes")
-    if isinstance(steps, bool) or int(steps) != steps or not 1 <= int(steps) <= FIRE_MAX_STEPS:
-        raise ValueError(f"md_nose_hoover_step: steps must be an integer in [1, {FIRE_MAX_STEPS}], got {steps!r}")
-    if isinstance(evaluation, bool) or int(evaluation) != evaluation or not 0 <= int(evaluation) <= int(steps):
-        raise ValueError(f"md_nose_hoover_step: evaluation must be an integer in [0, steps], got {evaluation!r}")
+    _md_counts("md_nose_hoover_step", steps, evaluation)
     p = _lib.MdNoseHooverParams(float(dt), float(kB), int(evaluation), int(steps), float(force_multiplier),
                                 float(stress_wt))
     _lib.check(lib.alignn_b200_md_nose_hoover_step(
@@ -899,14 +873,6 @@ def _supercell_arg(supercell):
     return C.cast((C.c_int32 * 3)(*s), C.c_void_p)
 
 
-def _phonon_operands(what, want, device):
-    for t, dt_ in want:
-        if not t.is_cuda or t.device != device:
-            raise RuntimeError(f"{what} needs all operands on one CUDA device; got {t.device} and {device}")
-        if t.dtype != dt_ or not t.is_contiguous():
-            raise RuntimeError(f"{what}: expected a contiguous {dt_} tensor, got {t.dtype}")
-
-
 @_on_tensor_device
 def phonon_force_constants(grad: torch.Tensor, atom_offsets: torch.Tensor, row_offsets: torch.Tensor,
                            fc_offsets: torch.Tensor, masses: torch.Tensor, force_constants: torch.Tensor,
@@ -923,10 +889,10 @@ def phonon_force_constants(grad: torch.Tensor, atom_offsets: torch.Tensor, row_o
     buffer, PHONON_NON_FINITE: a force product is not finite -- nothing else is read or written for it).  supercell is
     (N0, N1, N2); delta in A.  Enqueue only: the statuses are the caller's to read back."""
     lib = _lib.load()
-    _phonon_operands("phonon_force_constants", [(grad, torch.float32), (atom_offsets, torch.int64),
-                                                (row_offsets, torch.int64), (fc_offsets, torch.int64),
-                                                (masses, torch.float64), (force_constants, torch.float64),
-                                                (dynamical_matrix, torch.float64), (status, torch.int32)], grad.device)
+    _operands("phonon_force_constants", [(grad, torch.float32), (atom_offsets, torch.int64),
+                                         (row_offsets, torch.int64), (fc_offsets, torch.int64),
+                                         (masses, torch.float64), (force_constants, torch.float64),
+                                         (dynamical_matrix, torch.float64), (status, torch.int32)], grad.device)
     B = atom_offsets.numel() - 1
     if (B < 1 or row_offsets.numel() != B + 1 or fc_offsets.numel() != B + 1 or status.numel() != B
             or grad.dim() != 2 or grad.shape[1] != 3 or dynamical_matrix.numel() != force_constants.numel()):
@@ -950,10 +916,9 @@ def phonon_dynamical_matrix(dynamical_matrix: torch.Tensor, fc_offsets: torch.Te
     triangles); status [B] int32 (PHONON_BAD_INPUT: crystal c's D_N slice is not [Nc, modes, modes] inside the buffer;
     its pairs are not written).  Enqueue only."""
     lib = _lib.load()
-    _phonon_operands("phonon_dynamical_matrix", [(dynamical_matrix, torch.float64), (fc_offsets, torch.int64),
-                                                 (crystals, torch.int32), (qpoints, torch.float64),
-                                                 (out, torch.complex128), (status, torch.int32)],
-                     dynamical_matrix.device)
+    _operands("phonon_dynamical_matrix", [(dynamical_matrix, torch.float64), (fc_offsets, torch.int64),
+                                          (crystals, torch.int32), (qpoints, torch.float64),
+                                          (out, torch.complex128), (status, torch.int32)], dynamical_matrix.device)
     B, Q = fc_offsets.numel() - 1, crystals.numel()
     if B < 1 or status.numel() != B or qpoints.numel() != 3 * Q or out.numel() != Q * int(modes) * int(modes):
         raise ValueError("phonon_dynamical_matrix: inconsistent operand shapes")
@@ -979,8 +944,8 @@ def eos_fit(volumes: torch.Tensor, energies: torch.Tensor, params: torch.Tensor,
     EOS_NO_FIT or EOS_BAD_INPUT -- NaN parameters).  form is one of EOS_FORMS' values.  Enqueue only: the statuses are
     the caller's to read back."""
     lib = _lib.load()
-    _phonon_operands("eos_fit", [(volumes, torch.float64), (energies, torch.float64), (params, torch.float64),
-                                 (status, torch.int32)], volumes.device)
+    _operands("eos_fit", [(volumes, torch.float64), (energies, torch.float64), (params, torch.float64),
+                          (status, torch.int32)], volumes.device)
     if (volumes.dim() != 2 or energies.shape != volumes.shape or params.shape != (volumes.shape[0], 4)
             or status.shape != (volumes.shape[0],)):
         raise ValueError("eos_fit: inconsistent operand shapes")

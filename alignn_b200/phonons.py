@@ -12,15 +12,12 @@ blocks.  Each crystal gets the result it would get run alone; `oracle/phonon_ora
 from __future__ import annotations
 
 import math
-import numbers
 from typing import List, NamedTuple, Optional
 
 import numpy as np
 import torch
 
-from . import neighbors, ops
-from .md import _host_array, _real
-from .relax import _check_batch, _check_model, _evaluate_chunks
+from . import calculator, neighbors, ops
 
 # ase.units (ASE 3.22.1, CODATA 2014): Phonons.band_structure's s, sqrt(eV / A^2 / amu) -> eV
 _hbar = 6.626070040e-34 / (2 * math.pi)
@@ -74,7 +71,7 @@ def monkhorst_pack(size) -> np.ndarray:
 
 def _int_triple(v, name):
     if (not isinstance(v, (tuple, list)) or len(v) != 3 or
-            any(isinstance(x, bool) or not isinstance(x, numbers.Integral) or x < 1 for x in v)):
+            any(not calculator.integer(x) or x < 1 for x in v)):
         raise ValueError(f"{name} must be three integers >= 1, got {v!r}")
     return tuple(int(x) for x in v)
 
@@ -83,16 +80,13 @@ def _check(supercell, delta, qpoints, dos_kpts, dos_npts, dos_width, force_multi
     sc = _int_triple(supercell, "supercell")
     if int(np.prod(sc)) > ops.PHONON_MAX_CELLS:
         raise ValueError(f"supercell has {int(np.prod(sc))} cells, more than {ops.PHONON_MAX_CELLS}")
-    if not _real(delta) or not delta > 0:
-        raise ValueError(f"delta must be a finite number > 0 (A), got {delta!r}")
-    if not _real(force_multiplier):
-        raise ValueError(f"force_multiplier must be a finite real number, got {force_multiplier!r}")
+    calculator.check_positive("delta", delta, "A")
+    calculator.check_real("force_multiplier", force_multiplier)
     kpts = None if dos_kpts is None else _int_triple(dos_kpts, "dos_kpts")
-    if isinstance(dos_npts, bool) or not isinstance(dos_npts, numbers.Integral) or dos_npts < 2:
+    if not calculator.integer(dos_npts) or dos_npts < 2:
         raise ValueError(f"dos_npts must be an integer >= 2, got {dos_npts!r}")
-    if not _real(dos_width) or not dos_width > 0:
-        raise ValueError(f"dos_width must be a finite number > 0 (eV), got {dos_width!r}")
-    if isinstance(max_batch_atoms, bool) or not isinstance(max_batch_atoms, numbers.Integral):
+    calculator.check_positive("dos_width", dos_width, "eV")
+    if not calculator.integer(max_batch_atoms):
         raise ValueError(f"max_batch_atoms must be an integer, got {max_batch_atoms!r}")
     qs = None
     if qpoints is not None:
@@ -148,15 +142,13 @@ def phonons(model, structures, atom_features: torch.Tensor, masses, *, supercell
     max_batch_atoms: the most atoms one model call takes, at least the largest supercell (Nc n).
 
     A crystal whose forces are not finite raises RuntimeError naming it."""
-    _check_model("phonons", model)
-    lats, Xs, dev = _check_batch("phonons", model, structures, atom_features, neighbor_strategy, max_neighbors)
+    calculator.check_model("phonons", model)
+    lats, Xs, dev = calculator.check_batch("phonons", model, structures, atom_features, neighbor_strategy, max_neighbors)
     B = len(Xs)
     sc, kpts, qs = _check(supercell, delta, qpoints, dos_kpts, dos_npts, dos_width, force_multiplier, max_batch_atoms, B)
     sizes = [x.shape[0] for x in Xs]
     aoff = neighbors.ragged_offsets(sizes)
-    m = _host_array(masses, "masses", (int(aoff[-1]),))
-    if not (m > 0).all():
-        raise ValueError("masses must all be > 0 (amu)")
+    m = calculator.host_masses(masses, int(aoff[-1]))
     Nc = int(np.prod(sc))
     if max_batch_atoms < Nc * max(sizes):
         raise ValueError(f"max_batch_atoms must be at least the largest supercell, {Nc * max(sizes)} atoms, "
@@ -169,9 +161,11 @@ def phonons(model, structures, atom_features: torch.Tensor, masses, *, supercell
         tiled = [atom_features[aoff[b]:aoff[b + 1]].repeat(Nc, 1) for b in range(B)]
     roff = neighbors.ragged_offsets([6 * n * Nc * n for n in sizes])
     jobs = [(b, k) for b in range(B) for k in range(6 * sizes[b])]
-    _, grad_all = _evaluate_chunks(model, [(sets[b][0], sets[b][1][k]) for b, k in jobs], lambda j: tiled[jobs[j][0]],
-                                   dev, neighbor_strategy=neighbor_strategy, cutoff=cutoff, max_neighbors=max_neighbors,
-                                   cutoff_extra=cutoff_extra, max_batch_atoms=max_batch_atoms, span="phonon")
+    graph = dict(neighbor_strategy=neighbor_strategy, cutoff=cutoff, max_neighbors=max_neighbors,
+                 cutoff_extra=cutoff_extra)
+    _, grad_all = calculator.evaluate_chunks(model, [(sets[b][0], sets[b][1][k]) for b, k in jobs],
+                                             lambda j: tiled[jobs[j][0]], dev, graph, max_batch_atoms=max_batch_atoms,
+                                             span="phonon")
 
     # ---- force constants: one launch
     foff = neighbors.ragged_offsets([Nc * 9 * n * n for n in sizes])
